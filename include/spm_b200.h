@@ -223,10 +223,10 @@ typedef struct {
 } spm_engine_info;
 int spm_engine_get_info(const spm_engine *e, spm_engine_info *info);
 
-/* Tuning knobs (benchmark use).  lanes_per_sentence selects the unigram kernel: 1 = one sentence
- * per lane (default), 32 = one sentence per warp with the Viterbi window in registers,
- * 4/8/16 (and 64 = 32 lanes) = the general tile kernel; smem_norm_cap = per-sentence
- * shared-memory capacity in normalized bytes; ctas_per_sm >= 32 is read as threads per CTA.
+/* Tuning knobs (benchmark use).  lanes_per_sentence selects the encode kernels: 1 = the lane
+ * kernels, one sentence per lane (default), 32 = the general kernels, one sentence per warp, for
+ * every batch; any other value is rejected.  smem_norm_cap = per-sentence shared-memory capacity
+ * of the general kernels in normalized bytes; ctas_per_sm >= 32 is read as threads per CTA.
  * 0 keeps the current value. */
 int spm_engine_set_tuning(spm_engine *e, int lanes_per_sentence, int smem_norm_cap, int ctas_per_sm);
 

@@ -125,17 +125,17 @@ __device__ __forceinline__ uint32_t ordered_bits(uint32_t f) {
 }
 
 template <bool SPANS>
-__device__ __forceinline__ bool encode_bpe_sentence(const KModel &M, const KBatch &B, const Tile<32> &T, const HotTrie &H,
+__device__ __forceinline__ bool encode_bpe_sentence(const KModel &M, const KBatch &B, const Tile &T, const HotTrie &H,
                                                     const BpeMem &bm, const uint8_t *in, uint32_t len, uint32_t sent,
                                                     uint32_t *need) {
   TileMem tm{};
   tm.text = bm.text;
   tm.n2o = bm.n2o;
   tm.ncap = bm.ncap;
-  const NormResult nr = normalize_tile<32, SPANS>(M, T, in, len, tm);
+  const NormResult nr = normalize_tile<SPANS>(M, T, in, len, tm);
   const uint32_t n = nr.n;
   if (n > bm.ncap) { *need = n; return false; }
-  if (SPANS) publish_norm_tile<32>(B, T, tm, sent, n, n > 0);
+  if (SPANS) publish_norm_tile(B, T, tm, sent, n, n > 0);
   if (n == 0) {
     if (T.lane == 0) { B.sent_start[sent] = 0; B.sent_count[sent] = 0; }
     return true;
@@ -328,7 +328,7 @@ __device__ __forceinline__ bool encode_bpe_sentence(const KModel &M, const KBatc
       T.sync();
     }
   }
-  finish_tokens<32, SPANS>(M, B, T, text, tend, tid, sent, n_tok);
+  finish_tokens<SPANS>(M, B, T, text, tend, tid, sent, n_tok);
   return true;
 }
 
@@ -342,7 +342,7 @@ __global__ void __launch_bounds__(512, 1) encode_bpe_kernel(const KModel M, cons
   uint8_t *tiles = reinterpret_cast<uint8_t *>(s_val + M.hot_val);
   stage_hot_trie(M, mbar, s_link, s_val);
   HotTrie H{s_link, s_val, M.trie_link, M.trie_val, M.hot_link, M.hot_val};
-  const Tile<32> T;
+  const Tile T;
   const BpeMem bm = carve_bpe(tiles + static_cast<size_t>(threadIdx.x >> 5) * B.tile_bytes, B.ncap, SPANS);
   for (;;) {
     uint32_t sent = 0;
@@ -382,7 +382,7 @@ __global__ void __launch_bounds__(256) encode_bpe_long_kernel(const KModel M, co
   uint32_t *s_val = s_link + M.hot_link;
   stage_hot_trie(M, mbar, s_link, s_val);
   HotTrie H{s_link, s_val, M.trie_link, M.trie_val, M.hot_link, M.hot_val};
-  const Tile<32> T;
+  const Tile T;
   const uint32_t warps_per_cta = blockDim.x >> 5;
   for (uint32_t w = blockIdx.x * warps_per_cta + (threadIdx.x >> 5); w < B.long_n; w += gridDim.x * warps_per_cta) {
     const uint32_t sent = B.long_list[2 * w];

@@ -1,35 +1,45 @@
-// bpe_lane2_kernel.cuh -- K3 fast path, second generation: BPE merge with WORDS as the unit of work.
+// bpe_lane2_kernel.cuh -- K3 fast path: BPE merge, one sentence per LANE, with WORDS as the unit of merge work.
 //
 // Reference: bpe::Model::SampleEncode with alpha = 0 (src/bpe_model.cc:38-203): repeat "merge the live
-// adjacent pair with the greatest score, leftmost on ties" until no adjacent pair is a piece.  Under the
-// engine's word-split condition (no piece has U+2581 past byte 0; bpe_lane_kernel.cuh) a sentence falls apart
-// into independent words and the ids of a word are a pure function of its bytes.
+// adjacent pair with the greatest score, leftmost on ties" (the agenda's order, :51-57) until no adjacent pair is
+// a piece.
 //
-// Motivation: with one sentence per lane and one word at a time, only a quarter of the lanes are active per
-// instruction -- every lane waits for the longest word of the warp, at every word.  Here the warp works in two converged phases:
+// Exact decomposition used here (SURVEY.md 7, verified there on 20,000 sentences and by the parity tests): when no
+// piece contains U+2581 anywhere but at byte 0 (the default split_by_whitespace=true vocabulary; checked at load,
+// kFlagBpeWordSplit), a merge can never join a symbol with a following "▁..." symbol, so a sentence falls apart into
+// independent words (▁ + following characters).  The greedy loop only ever compares raw piece scores, so running it
+// per word gives exactly the reference's ids, and the ids of a word are a pure function of its bytes.
+//
+// Merging each lane's own words one at a time would leave most lanes idle: every lane would wait for the longest word
+// of the warp, at every word.  Instead the warp works in two converged phases:
 //   A  every lane scans ITS sentence byte by byte, walking the piece trie from the start of each word.  A word
 //      that is itself a piece whose merge sequence reproduces it (M.word_fast[unit] = its id, computed at load
 //      by running the reference's merge loop on the piece, engine.cu) is finished with that one id: 73 % of the
 //      words of the English corpus.  Any other word is appended to a per-warp list in shared memory and gets a
 //      run of slots (one per character, the most symbols it can end with) in its sentence's symbol log.
 //   B  whenever the list fills up (and at the end), the 32 lanes each take one listed WORD -- of any sentence of
-//      the warp -- and run the exact merge loop of bpe_lane_kernel.cuh on it; the symbols go to the reserved log
-//      slots, unused slots are marked empty.
-//   K4 each lane turns its sentence's log into ids (unk-run merging / byte fallback) as before.
+//      the warp -- and run the merge loop on it (bpe_merge_word) with tiny symbol arrays in shared memory
+//      ([slot][lane], bank == lane) that cache the trie node of every symbol, so that "is left+right a piece?"
+//      walks only the right symbol's bytes; the symbols go to the reserved log slots, unused slots are marked empty.
+//   K4 each lane turns its sentence's log into ids (unk-run merging / byte fallback).
 //
-// Engine-side preconditions as for encode_bpe_lane_kernel.  A word of more than kBpeWordSyms characters runs the same
-// merge loop with its symbol arrays in HBM scratch (rare; no sentence is deferred for it: the fused host path has no
-// second pass).
+// Engine-side preconditions (else the general warp kernel of bpe_kernel.cuh runs): kFlagBpeWordSplit,
+// escape_whitespaces, no user-defined symbols, no UNUSED pieces.  A word of more than kBpeWordSyms characters runs
+// the same merge loop with its symbol arrays in HBM scratch (rare; no sentence is deferred for it: the fused host
+// path has no second pass).
 #ifndef SPM_B200_BPE_LANE2_KERNEL_CUH_
 #define SPM_B200_BPE_LANE2_KERNEL_CUH_
 
-#include "bpe_lane_kernel.cuh"
+#include "lane_kernel.cuh"
 
 namespace spm_b200 {
 
+constexpr uint32_t kBpeWordSyms = 24;       // symbols of one word held in shared memory
+constexpr uint32_t kBpeDead = 0x3FFFFFu;    // 22-bit node field: not a trie path / not a piece
 constexpr uint32_t kBpeListCap = 128;       // slow words listed per warp before a phase-B drain
 constexpr uint32_t kBpeLogEmpty = 0xFFFFFFFFu;
-constexpr uint32_t kBpeLane2WarpBytes = kBpeLaneWarpBytes + kBpeListCap * 8;
+constexpr uint32_t kBpeSymArrayBytes = kBpeWordSyms * 32 * 4 * 3;               // sym, pn, ps of 32 lanes
+constexpr uint32_t kBpeLane2WarpBytes = kBpeSymArrayBytes + kBpeListCap * 8;   // + the word list
 
 // ---- word cache ----
 // Under the word-split condition the ids of a word are a pure function of its bytes, and natural text repeats its
@@ -227,7 +237,7 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
   LaneCtx c;
-  c.pol = slab_policy(B.slab_l2);
+  c.pol = slab_policy();
   uint32_t *sym, *pn, *list;
   float *ps;
   uint32_t *text_all, *log_all;  // the warp's slab without the lane offset (phase B reads other lanes' columns)
@@ -236,7 +246,7 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
     sym = reinterpret_cast<uint32_t *>(a) + lane;                             // node(22) | byte_len << 22
     pn = reinterpret_cast<uint32_t *>(a + kBpeWordSyms * 32 * 4) + lane;      // pair node(22) | offset_in_word << 22
     ps = reinterpret_cast<float *>(a + kBpeWordSyms * 32 * 8) + lane;         // pair score
-    list = reinterpret_cast<uint32_t *>(a + kBpeLaneWarpBytes);               // [kBpeListCap][2]
+    list = reinterpret_cast<uint32_t *>(a + kBpeSymArrayBytes);               // [kBpeListCap][2]
     uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
     text_all = reinterpret_cast<uint32_t *>(slab);
     log_all = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32;
@@ -515,7 +525,7 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
         }
       }
     }
-    if (B.slab_discard) slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
+    slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
     const uint32_t t_g3 = tst ? static_cast<uint32_t>(clock64()) : 0u;
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();

@@ -103,8 +103,6 @@ struct KBatch {
   uint32_t *seg_copied;               // [segments]
   uint32_t *drained_upto;
   unsigned long long *host_progress;
-  uint32_t slab_discard;              // lane kernels: discard.L2 the used slab rows at the end of a group (lane_kernel.cuh)
-  uint32_t slab_l2;                   // L2 eviction priority of the lane kernels' slab accesses: 0 normal, 1 evict_last, 2 evict_first
   unsigned long long *kstats;         // [4] cycles (lane 0 of each warp): input wait, compaction, look-back wait, groups; or null
   // outputs of the encode kernel
   int32_t *tmp_ids;              // ids in completion order

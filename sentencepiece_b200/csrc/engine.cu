@@ -27,7 +27,6 @@
 
 #include "../../include/spm_b200.h"
 #include "bpe_kernel.cuh"
-#include "bpe_lane_kernel.cuh"
 #include "bpe_lane2_kernel.cuh"
 #include "device_model.h"
 #include "kernels.cuh"
@@ -38,7 +37,6 @@
 #include "nbest_kernel.cuh"
 #include "lattice_kernel.cuh"
 #include "trie_builder.h"
-#include "unigram_warp.cuh"
 
 using namespace spm_b200;
 
@@ -150,18 +148,15 @@ struct spm_engine {
   // sentences with the cache emptied before every step (bench.py, H100 SXM at a 400 W limit, one run each): 2^20
   // 5.80 ms, 2^22 5.73 ms (256 MB of HBM), 2^24 5.93 ms (emptying 1 GB costs more than the extra hits save)
   int bpe_cache_log2 = 22;
-  int bpe_lane_version = 2;  // SPM_B200_BPE_LANE_V
   bool fast_words = true;  // SPM_B200_FASTWORDS
   int upload_word_safe();
   KModel km{};
 
   // tuning
-  int G = 1;  // 1: lane kernel (sentence per lane); 32: warp kernel; 4/8/16: tile kernel; 64: tile kernel, 32 lanes
+  int G = 1;  // 1: lane kernels (sentence per lane); 32: the general kernels (sentence per warp) for every batch
   int threads = 1024;
   uint32_t ncap = 256;
-  uint32_t slab_discard = 1;  // SPM_B200_SLAB_DISCARD=0 turns it off (KBatch::slab_discard)
-  uint32_t slab_l2 = 0;    // SPM_B200_SLAB_L2: L2 eviction priority of the slab accesses (KBatch::slab_l2)
-  uint32_t lane_cap = 512;  // normalized-byte capacity per sentence of the lane kernel's slabs
+  static constexpr uint32_t lane_cap = 512;  // normalized-byte capacity per sentence of the lane kernel's slabs
   int ctas_per_sm = 1;
 
   // per-call buffers (grow only)
@@ -183,6 +178,8 @@ struct spm_engine {
   DevBuf<unsigned long long> p_id_offsets[2];
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
+  int ensure_copy_streams();  // creates the copy streams and the slot events on first use
+  int grow_pinned_ids(unsigned long long have, uint64_t more, size_t done, size_t n);
   size_t pipeline_min_sentences = 300000, pipeline_chunk_sentences = 65536;
   DevBuf<uint32_t> d_order, d_order_hist;  // K0: length-bucketed processing order
   int build_order(const uint64_t *d_offs, size_t n, cudaStream_t st, const uint32_t **order, uint32_t seg);
@@ -199,6 +196,7 @@ struct spm_engine {
   PinBuf<uint32_t> h_marks;
   PinBuf<unsigned long long> h_progress;
   cudaEvent_t ev_offs = nullptr;
+  void feed_input(const char *bytes, const uint64_t *offsets, size_t n, size_t piece, std::atomic<int> *rc);
   int encode_host_streamed(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
                            const uint64_t **id_offsets);
   int encode_host_fused(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids, const uint64_t **id_offsets);
@@ -208,11 +206,11 @@ struct spm_engine {
   DevBuf<uint32_t> d_seg_done, d_sent_rel;
   DevBuf<unsigned long long> d_seg_words;
   // Launch geometry of the lane kernels for an ids-only batch; ok == false: the model / tuning is outside the lane
-  // kernels (the tile, warp or general BPE kernels take the batch).  Shared memory per warp grows with the longest
+  // kernels (the general warp-per-sentence kernels take the batch).  Shared memory per warp grows with the longest
   // piece (ring of max piece length + 2 slots), so the warps per CTA shrink until the rings fit.
   struct LaneGeom {
     bool ok = false;
-    int version = 1;       // BPE: 1 = encode_bpe_lane_kernel (sentence per lane), 2 = encode_bpe_lane2_kernel (word lists)
+    int version = 1;       // unigram: 2 = encode_unigram_lane_kernel (whole-word shortcut), 1 = the plain instantiation
     int threads = 0;
     uint32_t R = 0, smem = 0;
   };
@@ -232,14 +230,12 @@ struct spm_engine {
     if (model.model_type == SPM_BPE) {
       if (!((km.flags & kFlagBpeWordSplit) && (km.flags & kFlagEscapeWs) && !(km.flags & (kFlagHasUserSymbols | kFlagHasUnused))))
         return g;
-      g.version = bpe_lane_version == 2 ? 2 : 1;
-      const size_t per_warp = g.version == 2 ? kBpeLane2WarpBytes : kBpeLaneWarpBytes;
-      // (launch bounds: 704 threads for lane2 -- 22 warps is what the shared-memory arrays allow -- 768 for lane v1)
-      const int warps = static_cast<int>(std::min<size_t>(std::min(threads, g.version == 2 ? 704 : 768) / 32, avail / per_warp));
+      // (launch bounds: 704 threads -- 22 warps is what the shared-memory arrays allow)
+      const int warps = static_cast<int>(std::min<size_t>(std::min(threads, 704) / 32, avail / kBpeLane2WarpBytes));
       if (warps < 4) return g;
       g.ok = true;
       g.threads = warps * 32;
-      g.smem = static_cast<uint32_t>(kLaneTableBytes + static_cast<size_t>(warps) * per_warp);
+      g.smem = static_cast<uint32_t>(kLaneTableBytes + static_cast<size_t>(warps) * kBpeLane2WarpBytes);
       return g;
     }
     if (trie.max_key_len > 62) return g;
@@ -717,23 +713,20 @@ struct LaunchGeom {
   uint32_t hot_link, hot_val, tile_bytes, smem_bytes, tiles;
 };
 
-// Shared memory split: tiles first (threads/G of them), the rest goes to the hot
-// trie prefix (3:1 link:val, both multiples of 4 units for the 16-byte bulk copy).
-LaunchGeom plan_geometry(const spm_engine &e, bool spans, int G, int threads, uint32_t ncap, uint32_t K) {
+// Shared memory of the general (warp-per-sentence) kernels: `tiles` scratch areas of `tile_bytes` first, the rest
+// goes to the hot trie prefix (3:1 link:val, both multiples of 4 units for the 16-byte bulk copy).
+LaunchGeom plan_geometry(const spm_engine &e, uint32_t tile_bytes, uint32_t tiles) {
   LaunchGeom g{};
-  g.tiles = static_cast<uint32_t>(threads / G);
-  g.tile_bytes = tile_bytes_for(ncap, G, K, spans);
+  g.tiles = tiles;
+  g.tile_bytes = tile_bytes;
   const size_t budget = e.smem_optin / std::max(1, e.ctas_per_sm) - (e.ctas_per_sm > 1 ? 1024 : 0);
-  const size_t fixed = 16 + static_cast<size_t>(g.tiles) * g.tile_bytes + 128;
-  size_t hot = budget > fixed ? budget - fixed : 0;
-  if (const char *lim = getenv("SPM_B200_HOT_LIMIT")) hot = std::min<size_t>(hot, strtoull(lim, nullptr, 10));  // experiments
+  const size_t fixed = 16 + static_cast<size_t>(tiles) * tile_bytes + 128;
+  const size_t hot = budget > fixed ? budget - fixed : 0;
   const uint32_t units = e.km.trie_units;
-  uint32_t hl = static_cast<uint32_t>(std::min<size_t>(units, (hot * 3 / 4) / 4)) & ~3u;
-  uint32_t hv = static_cast<uint32_t>(std::min<size_t>(units, (hot - static_cast<size_t>(hl) * 4) / 4)) & ~3u;
-  // if the whole link array fits, give the remainder to val
-  g.hot_link = hl;
-  g.hot_val = hv;
-  g.smem_bytes = static_cast<uint32_t>(16 + static_cast<size_t>(hl + hv) * 4 + static_cast<size_t>(g.tiles) * g.tile_bytes);
+  g.hot_link = static_cast<uint32_t>(std::min<size_t>(units, (hot * 3 / 4) / 4)) & ~3u;
+  // if the whole link array fits, the remainder goes to val
+  g.hot_val = static_cast<uint32_t>(std::min<size_t>(units, (hot - static_cast<size_t>(g.hot_link) * 4) / 4)) & ~3u;
+  g.smem_bytes = static_cast<uint32_t>(16 + static_cast<size_t>(g.hot_link + g.hot_val) * 4 + static_cast<size_t>(tiles) * tile_bytes);
   return g;
 }
 
@@ -746,22 +739,15 @@ cudaError_t set_smem(KernelT k, size_t bytes) {
 
 int spm_engine::configure_kernel_attrs() {
   const size_t mx = smem_optin;
-  CUDA_TRY(set_smem(encode_unigram_kernel<4, false>, mx));
-  CUDA_TRY(set_smem(encode_unigram_kernel<8, false>, mx));
-  CUDA_TRY(set_smem(encode_unigram_kernel<16, false>, mx));
-  CUDA_TRY(set_smem(encode_unigram_kernel<32, false>, mx));
-  CUDA_TRY(set_smem(encode_unigram_kernel<8, true>, mx));
-  CUDA_TRY(set_smem(encode_unigram_kernel<32, true>, mx));
+  CUDA_TRY(set_smem(encode_unigram_kernel<false>, mx));
+  CUDA_TRY(set_smem(encode_unigram_kernel<true>, mx));
   CUDA_TRY(set_smem(encode_unigram_long_kernel<false>, mx));
   CUDA_TRY(set_smem(encode_unigram_long_kernel<true>, mx));
   CUDA_TRY(set_smem(encode_unigram_lane_kernel, mx));
   CUDA_TRY(set_smem(encode_unigram_lane_plain_kernel, mx));
-  CUDA_TRY(set_smem(encode_bpe_lane_kernel, mx));
   CUDA_TRY(set_smem(encode_bpe_lane2_kernel, mx));
   CUDA_TRY(set_smem(nbest_lane_kernel<kNbestTop, 1024>, mx));
   CUDA_TRY(set_smem(lattice_lane_kernel, mx));
-  CUDA_TRY(set_smem(encode_unigram_warp_kernel<512>, mx));
-  CUDA_TRY(set_smem(encode_unigram_warp_kernel<1024>, mx));
   CUDA_TRY(set_smem(encode_bpe_kernel<false>, mx));
   CUDA_TRY(set_smem(encode_bpe_kernel<true>, mx));
   CUDA_TRY(set_smem(encode_bpe_long_kernel<false>, mx));
@@ -835,32 +821,16 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
   last_deferred = 0;
   const uint32_t n32 = static_cast<uint32_t>(n);
   const bool bpe = model.model_type == SPM_BPE;
-  const int tileG = (G == 4 || G == 8 || G == 16) ? G : 32;
-  const int useG = bpe ? 32 : ((spans && tileG != 32) ? 8 : tileG);
   const int tile_threads = std::min(threads, 512);
   const uint32_t K = km.match_slots;
-  LaunchGeom geom = plan_geometry(*this, spans, useG, tile_threads, ncap, K);
-  // fast paths: sentence per lane (lane kernels), or warp per sentence with a register-resident Viterbi window
+  // fast path: sentence per lane (lane kernels); else the general kernels, a warp per sentence
   const LaneGeom lg = spans ? LaneGeom{} : lane_geometry();
   const bool lane_path = !bpe && lg.ok;
   const bool bpe_lane_path = bpe && lg.ok;
-  const bool warp_path = !bpe && !spans && trie.max_key_len <= 32 && G == 32;
-  const int launch_threads = warp_path ? threads : tile_threads;
-  if (bpe || warp_path) {
-    // these kernels own a warp per sentence and their own scratch layout
-    geom.tiles = launch_threads / 32;
-    geom.tile_bytes = bpe ? bpe_tile_bytes(ncap, spans) : warp_bytes_for(ncap, K);
-    const size_t fixed = 16 + static_cast<size_t>(geom.tiles) * geom.tile_bytes + 128;
-    const size_t hot = smem_optin > fixed ? smem_optin - fixed : 0;
-    geom.hot_link = static_cast<uint32_t>(std::min<size_t>(km.trie_units, (hot * 3 / 4) / 4)) & ~3u;
-    geom.hot_val = static_cast<uint32_t>(std::min<size_t>(km.trie_units, (hot - static_cast<size_t>(geom.hot_link) * 4) / 4)) & ~3u;
-    geom.smem_bytes = static_cast<uint32_t>(16 + static_cast<size_t>(geom.hot_link + geom.hot_val) * 4 +
-                                            static_cast<size_t>(geom.tiles) * geom.tile_bytes);
-  }
+  LaunchGeom geom = plan_geometry(*this, bpe ? bpe_tile_bytes(ncap, spans) : tile_bytes_for(ncap, K, spans), tile_threads / 32);
   if (lane_path || bpe_lane_path) {
     geom.tiles = lg.threads / 32;
-    geom.tile_bytes = bpe ? (lg.version == 2 ? kBpeLane2WarpBytes : kBpeLaneWarpBytes)
-                          : (lg.version == 2 ? lane_ring_bytes(lg.R) : lg.R * 32 * 8);
+    geom.tile_bytes = bpe ? kBpeLane2WarpBytes : (lg.version == 2 ? lane_ring_bytes(lg.R) : lg.R * 32 * 8);
     geom.hot_link = geom.hot_val = 0;  // the lane kernels read the trie through L1: rings / word arrays get the shared memory
     geom.smem_bytes = lg.smem;
     const size_t warps_total = static_cast<size_t>(sm_count) * ctas_per_sm * geom.tiles;
@@ -900,7 +870,6 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 4 * sizeof(unsigned long long), st));
     KBatch B{};
-    B.slab_l2 = slab_l2; B.slab_discard = slab_discard;
     B.bytes = d_bytes_base;
     B.offsets = d_offs;
     B.n = n32;
@@ -930,18 +899,14 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       B.kstats = d_kstats.p;
     }
     if (lane_path || bpe_lane_path) {
-      uint32_t seg = cur_ready ? (1u << cur_piece_shift) : 0u;
-      if (const char *v = getenv("SPM_B200_SORT_SEG")) seg = static_cast<uint32_t>(atoi(v));  // experiment knob
-      const int rc = build_order(d_offs, n, st, &B.order, seg);
+      const int rc = build_order(d_offs, n, st, &B.order, cur_ready ? (1u << cur_piece_shift) : 0u);
       if (rc) return rc;
       B.ready = cur_ready;
       B.ready_base = cur_ready_base;
       B.piece_shift = cur_piece_shift;
     }
-    if (bpe_lane_path && lg.version == 2) {
+    if (bpe_lane_path) {
       encode_bpe_lane2_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
-    } else if (bpe_lane_path) {
-      encode_bpe_lane_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap);
     } else if (bpe) {
       if (spans) encode_bpe_kernel<true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
       else encode_bpe_kernel<false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
@@ -949,19 +914,10 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       encode_unigram_lane_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
     } else if (lane_path) {
       encode_unigram_lane_plain_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
-    } else if (warp_path) {
-      if (threads <= 512) encode_unigram_warp_kernel<512><<<grid, threads, geom.smem_bytes, st>>>(M, B);
-      else encode_unigram_warp_kernel<1024><<<grid, threads, geom.smem_bytes, st>>>(M, B);
     } else if (spans) {
-      if (useG == 32) encode_unigram_kernel<32, true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
-      else encode_unigram_kernel<8, true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
+      encode_unigram_kernel<true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
     } else {
-      switch (useG) {
-        case 4: encode_unigram_kernel<4, false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B); break;
-        case 8: encode_unigram_kernel<8, false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B); break;
-        case 16: encode_unigram_kernel<16, false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B); break;
-        default: encode_unigram_kernel<32, false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B); break;
-      }
+      encode_unigram_kernel<false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
     }
     CUDA_TRY(cudaGetLastError());
     ++last_launches;
@@ -988,16 +944,11 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       // ---- second chance: the sentences a lane kernel could not take (long words, long
       //      sentences) go through the shared-memory warp kernels before the HBM-scratch path ----
       last_deferred = n_def;
-      LaunchGeom g2{};
-      g2.tiles = tile_threads / 32;
-      g2.tile_bytes = bpe ? bpe_tile_bytes(ncap, false) : tile_bytes_for(ncap, 32, K, false);
-      const size_t fixed2 = 16 + static_cast<size_t>(g2.tiles) * g2.tile_bytes + 128;
-      const size_t hot2 = smem_optin > fixed2 ? smem_optin - fixed2 : 0;
+      const LaunchGeom g2 =
+          plan_geometry(*this, bpe ? bpe_tile_bytes(ncap, false) : tile_bytes_for(ncap, K, false), tile_threads / 32);
       KModel M2 = km;
-      M2.hot_link = static_cast<uint32_t>(std::min<size_t>(km.trie_units, (hot2 * 3 / 4) / 4)) & ~3u;
-      M2.hot_val = static_cast<uint32_t>(std::min<size_t>(km.trie_units, (hot2 - static_cast<size_t>(M2.hot_link) * 4) / 4)) & ~3u;
-      const uint32_t smem2 = static_cast<uint32_t>(16 + static_cast<size_t>(M2.hot_link + M2.hot_val) * 4 +
-                                                   static_cast<size_t>(g2.tiles) * g2.tile_bytes);
+      M2.hot_link = g2.hot_link;
+      M2.hot_val = g2.hot_val;
       KBatch B2 = B;
       B2.sub_list = d_deferred.p;
       B2.sub_n = n_def;
@@ -1007,8 +958,8 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       B2.ncap = ncap;
       B2.tile_bytes = g2.tile_bytes;
       const int grid2 = static_cast<int>(std::min<uint32_t>(static_cast<uint32_t>(grid), (n_def + g2.tiles - 1) / g2.tiles));
-      if (bpe) encode_bpe_kernel<false><<<grid2, tile_threads, smem2, st>>>(M2, B2);
-      else encode_unigram_kernel<32, false><<<grid2, tile_threads, smem2, st>>>(M2, B2);
+      if (bpe) encode_bpe_kernel<false><<<grid2, tile_threads, g2.smem_bytes, st>>>(M2, B2);
+      else encode_unigram_kernel<false><<<grid2, tile_threads, g2.smem_bytes, st>>>(M2, B2);
       CUDA_TRY(cudaGetLastError());
       ++last_launches;
       CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
@@ -1043,7 +994,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
         need += 8;
         h_deferred.p[2 * k + 1] = need;
         const uint32_t lk = bpe ? 1 : K;
-        const unsigned long long bytes = bpe ? bpe_tile_bytes(need, spans) : tile_bytes_for(need, 32, lk, spans);
+        const unsigned long long bytes = bpe ? bpe_tile_bytes(need, spans) : tile_bytes_for(need, lk, spans);
         offs[k + 1] = offs[k] + ((bytes + 255ull) & ~255ull);
       }
       CUDA_TRY(d_long_scratch.ensure(offs[n_def] + 256));
@@ -1139,6 +1090,57 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
   return SPM_OK;
 }
 
+int spm_engine::ensure_copy_streams() {
+  if (s_h2d) return SPM_OK;
+  CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
+  CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
+  for (int k = 0; k < 2; ++k) {
+    CUDA_TRY(cudaEventCreateWithFlags(&ev_in[k], cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
+    CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
+  }
+  return SPM_OK;
+}
+
+// Makes the pinned result buffer hold `have` + `more` ids (rare), keeping the `have` ids that have already arrived;
+// the new size extrapolates the ids per sentence of the first `done` of the batch's n sentences.
+int spm_engine::grow_pinned_ids(unsigned long long have, uint64_t more, size_t done, size_t n) {
+  if (have + more + 1 <= h_ids.cap) return SPM_OK;
+  CUDA_TRY(cudaStreamSynchronize(s_d2h));
+  PinBuf<int32_t> bigger;
+  const double per_sent = static_cast<double>(have + more) / static_cast<double>(done);
+  CUDA_TRY(bigger.ensure(static_cast<size_t>(per_sent * 1.25 * n) + more + 4096));
+  if (have) memcpy(bigger.p, h_ids.p, have * sizeof(int32_t));
+  h_ids.release();
+  h_ids = bigger;
+  return SPM_OK;
+}
+
+// Input feeder of the streamed host paths, run on a helper thread so that the first encode kernel is launched right
+// away: the bytes of the batch go to s_bytes in pieces of `piece` sentences, each followed by a 4-byte copy that
+// advances the device-side watermark d_ready.  Cuts between the copies sit on 128-byte lines of the device buffer
+// (ByteStream in lane_kernel.cuh over-reads within a line).  *rc = 1 when a copy could not be queued.
+void spm_engine::feed_input(const char *bytes, const uint64_t *offsets, size_t n, size_t piece, std::atomic<int> *rc) {
+  if (cudaSetDevice(device) != cudaSuccess) { *rc = 1; return; }
+  const uint64_t total_bytes = offsets[n] - offsets[0];
+  const size_t P = (n + piece - 1) / piece;
+  uint64_t done_bytes = 0;
+  for (size_t p = 0; p < P; ++p) {
+    const size_t hi = std::min(n, (p + 1) * piece);
+    uint64_t cut = offsets[hi] - offsets[0];
+    cut = hi == n ? total_bytes : std::min<uint64_t>(total_bytes, (cut + 127u) & ~uint64_t{127});
+    if (cut > done_bytes &&
+        cudaMemcpyAsync(s_bytes.p + done_bytes, bytes + offsets[0] + done_bytes, cut - done_bytes, cudaMemcpyHostToDevice,
+                        s_h2d) != cudaSuccess) { *rc = 1; return; }
+    done_bytes = std::max(done_bytes, cut);
+    h_marks.p[p] = static_cast<uint32_t>(hi);
+    if (cudaMemcpyAsync(d_ready.p, h_marks.p + p, sizeof(uint32_t), cudaMemcpyHostToDevice, s_h2d) != cudaSuccess) {
+      *rc = 1;
+      return;
+    }
+  }
+}
+
 // Large host batches: chunked three-stage pipeline.  H2D of chunk c+1 and D2H of chunk c-1
 // run on their own streams while chunk c is being encoded; inputs and outputs are double
 // buffered, the temporary buffers are only ever touched by the (serial) compute stream.
@@ -1147,22 +1149,13 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
   CUDA_TRY(cudaSetDevice(device));
   for (size_t i = 0; i < n; ++i)
     if (offsets[i + 1] < offsets[i]) { set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
-  if (!s_h2d) {
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_in[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
-    }
-  }
+  { const int rc = ensure_copy_streams(); if (rc) return rc; }
   // one sentence group (32 sentences) per resident warp and chunk: a launch cannot finish faster than
   // one group, so smaller chunks would only add idle warps
   const bool is_bpe = model.model_type == SPM_BPE;
   const LaneGeom lgw = lane_geometry();
   const size_t warps = static_cast<size_t>(sm_count) * ctas_per_sm * ((lgw.ok ? lgw.threads : std::min(threads, 512)) / 32);
-  size_t groups_per_warp = is_bpe ? 2 : 1;
-  if (const char *v = getenv("SPM_B200_CHUNK_GROUPS")) groups_per_warp = std::max(1, atoi(v));
+  const size_t groups_per_warp = is_bpe ? 2 : 1;
   const bool trace = getenv("SPM_B200_TRACE") != nullptr;
   const auto t_begin = std::chrono::steady_clock::now();
   auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
@@ -1210,15 +1203,7 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
     CUDA_TRY(cudaEventRecord(ev_out[k], stream));
     launches += last_launches;
     deferred += last_deferred;
-    if (id_base + tot + 1 > h_ids.cap) {  // grow the pinned result buffer (rare): keep what has already arrived
-      CUDA_TRY(cudaStreamSynchronize(s_d2h));
-      PinBuf<int32_t> bigger;
-      const double per_sent = static_cast<double>(id_base + tot) / static_cast<double>(hi);
-      CUDA_TRY(bigger.ensure(static_cast<size_t>(per_sent * 1.25 * n) + tot + 4096));
-      if (id_base) memcpy(bigger.p, h_ids.p, id_base * sizeof(int32_t));
-      h_ids.release();
-      h_ids = bigger;
-    }
+    { const int rc2 = grow_pinned_ids(id_base, tot, hi, n); if (rc2) return rc2; }
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_ids.p + id_base, p_ids[k].p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_id_offsets.p + lo, p_id_offsets[k].p, (hi - lo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
@@ -1252,15 +1237,7 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
 int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
                                      const uint64_t **id_offsets) {
   CUDA_TRY(cudaSetDevice(device));
-  if (!s_h2d) {
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_in[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
-    }
-  }
+  { const int rc = ensure_copy_streams(); if (rc) return rc; }
   if (!ev_offs) CUDA_TRY(cudaEventCreateWithFlags(&ev_offs, cudaEventDisableTiming));
   const bool trace = getenv("SPM_B200_TRACE") != nullptr;
   const auto t_begin = std::chrono::steady_clock::now();
@@ -1271,8 +1248,7 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
   const bool is_bpe = model.model_type == SPM_BPE;
   const LaneGeom lgw = lane_geometry();
   const size_t warps = static_cast<size_t>(sm_count) * ctas_per_sm * ((lgw.ok ? lgw.threads : std::min(threads, 512)) / 32);
-  size_t groups_per_warp = is_bpe ? 4 : 2;
-  if (const char *v = getenv("SPM_B200_CHUNK_GROUPS")) groups_per_warp = std::max(1, atoi(v));
+  const size_t groups_per_warp = is_bpe ? 4 : 2;
   const size_t min_chunk = std::max<size_t>(kPiece, warps * 32 * groups_per_warp);
   const size_t want_chunks = std::max<size_t>(1, n / min_chunk);
   const size_t chunk = ((P + want_chunks - 1) / want_chunks) * kPiece;
@@ -1297,27 +1273,8 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
       return SPM_ERR_ARG;
     }
   }
-  // The copies are issued by a helper thread so that the first encode kernel is launched right away.  Cuts between
-  // the copies sit on 128-byte lines of the device buffer (ByteStream in lane_kernel.cuh over-reads within a line).
   std::atomic<int> feed_rc{0};
-  std::thread feeder([&]() {
-    if (cudaSetDevice(device) != cudaSuccess) { feed_rc = 1; return; }
-    uint64_t done_bytes = 0;
-    for (size_t p = 0; p < P; ++p) {
-      const size_t hi = std::min(n, (p + 1) * kPiece);
-      uint64_t cut = offsets[hi] - offsets[0];
-      cut = hi == n ? total_bytes : std::min<uint64_t>(total_bytes, (cut + 127u) & ~uint64_t{127});
-      if (cut > done_bytes &&
-          cudaMemcpyAsync(s_bytes.p + done_bytes, bytes + offsets[0] + done_bytes, cut - done_bytes, cudaMemcpyHostToDevice,
-                          s_h2d) != cudaSuccess) { feed_rc = 1; return; }
-      done_bytes = std::max(done_bytes, cut);
-      h_marks.p[p] = static_cast<uint32_t>(hi);
-      if (cudaMemcpyAsync(d_ready.p, h_marks.p + p, sizeof(uint32_t), cudaMemcpyHostToDevice, s_h2d) != cudaSuccess) {
-        feed_rc = 1;
-        return;
-      }
-    }
-  });
+  std::thread feeder([&]() { feed_input(bytes, offsets, n, kPiece, &feed_rc); });
   struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{feeder};
   CUDA_TRY(cudaStreamWaitEvent(stream, ev_offs, 0));
   uint64_t launches = 0, deferred = 0;
@@ -1339,15 +1296,7 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
     CUDA_TRY(cudaEventRecord(ev_out[k], stream));
     launches += last_launches;
     deferred += last_deferred;
-    if (id_base + tot + 1 > h_ids.cap) {  // grow the pinned result buffer (rare): keep what has already arrived
-      CUDA_TRY(cudaStreamSynchronize(s_d2h));
-      PinBuf<int32_t> bigger;
-      const double per_sent = static_cast<double>(id_base + tot) / static_cast<double>(hi);
-      CUDA_TRY(bigger.ensure(static_cast<size_t>(per_sent * 1.25 * n) + tot + 4096));
-      if (id_base) memcpy(bigger.p, h_ids.p, id_base * sizeof(int32_t));
-      h_ids.release();
-      h_ids = bigger;
-    }
+    { const int rc2 = grow_pinned_ids(id_base, tot, hi, n); if (rc2) return rc2; }
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_ids.p + id_base, p_ids[k].p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_id_offsets.p + lo, p_id_offsets[k].p, (hi - lo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
@@ -1381,28 +1330,13 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
 int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
                                   const uint64_t **id_offsets) {
   CUDA_TRY(cudaSetDevice(device));
-  if (!s_h2d) {
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_in[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
-    }
-  }
+  { const int rc = ensure_copy_streams(); if (rc) return rc; }
   if (!ev_offs) CUDA_TRY(cudaEventCreateWithFlags(&ev_offs, cudaEventDisableTiming));
   const bool trace = getenv("SPM_B200_TRACE") != nullptr;
   const auto t_begin = std::chrono::steady_clock::now();
   auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
-  uint32_t kPieceShift = 15;
-  uint32_t kSegShift = 10;
-  if (const char *v = getenv("SPM_B200_SEG_SHIFT")) kSegShift = std::min<uint32_t>(kPieceShift, std::max(8, atoi(v)));  // experiment knob
-  if (const char *v = getenv("SPM_B200_PIECE_SHIFT")) kPieceShift = std::min(20, std::max(10, atoi(v)));
-  // experiment knobs (what the fused path loses against the device-resident one): bit 0 no
-  // D2H copies while the kernel runs, bit 1 id_offsets to device memory + one copy at the end, bit 2 the whole input is
-  // staged before the launch, bit 3 input order instead of the segment-sorted one.  All give correct results.
-  int fx = 0;
-  if (const char *v = getenv("SPM_B200_FUSED_X")) fx = atoi(v);
+  constexpr uint32_t kPieceShift = 15;
+  constexpr uint32_t kSegShift = 10;
   const size_t kPiece = size_t{1} << kPieceShift;
   const size_t P = (n + kPiece - 1) / kPiece;
   const size_t S = (n + (size_t{1} << kSegShift) - 1) >> kSegShift;
@@ -1446,26 +1380,8 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(cudaEventRecord(ev_offs, s_h2d));
   if (offsets[n] < offsets[0]) { cudaStreamSynchronize(s_h2d); set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
   std::atomic<int> feed_rc{0};
-  std::thread feeder([&]() {
-    if (cudaSetDevice(device) != cudaSuccess) { feed_rc = 1; return; }
-    uint64_t done_bytes = 0;
-    for (size_t p = 0; p < P; ++p) {
-      const size_t hi = std::min(n, (p + 1) * kPiece);
-      uint64_t cut = offsets[hi] - offsets[0];
-      cut = hi == n ? total_bytes : std::min<uint64_t>(total_bytes, (cut + 127u) & ~uint64_t{127});
-      if (cut > done_bytes &&
-          cudaMemcpyAsync(s_bytes.p + done_bytes, bytes + offsets[0] + done_bytes, cut - done_bytes, cudaMemcpyHostToDevice,
-                          s_h2d) != cudaSuccess) { feed_rc = 1; return; }
-      done_bytes = std::max(done_bytes, cut);
-      h_marks.p[p] = static_cast<uint32_t>(hi);
-      if (cudaMemcpyAsync(d_ready.p, h_marks.p + p, sizeof(uint32_t), cudaMemcpyHostToDevice, s_h2d) != cudaSuccess) {
-        feed_rc = 1;
-        return;
-      }
-    }
-  });
+  std::thread feeder([&]() { feed_input(bytes, offsets, n, kPiece, &feed_rc); });
   struct Joiner { std::thread &t; ~Joiner() { if (t.joinable()) t.join(); } } joiner{feeder};
-  if (fx & 4) { feeder.join(); CUDA_TRY(cudaStreamSynchronize(s_h2d)); }
   // ---- one launch ----
   last_launches = 0;
   last_deferred = 0;
@@ -1477,7 +1393,6 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   KModel M = km;
   M.hot_link = M.hot_val = 0;
   KBatch B{};
-  B.slab_l2 = slab_l2; B.slab_discard = slab_discard;
   B.bytes = s_bytes.p - offsets[0];
   B.offsets = s_offsets.p;
   B.n = n32;
@@ -1503,7 +1418,6 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
     void *dp = nullptr;
     CUDA_TRY(cudaHostGetDevicePointer(&dp, h_id_offsets.p, 0));
     B.out_offsets = static_cast<unsigned long long *>(dp);
-    if (fx & 2) { CUDA_TRY(d_id_offsets.ensure(n + 1)); B.out_offsets = d_id_offsets.p; }
     CUDA_TRY(cudaHostGetDevicePointer(&dp, h_progress.p, 0));
     B.host_progress = static_cast<unsigned long long *>(dp);
   }
@@ -1514,20 +1428,15 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   B.out_off_base = 0;
   B.kstats = trace ? d_ctrl64.p + 4 : nullptr;
   CUDA_TRY(cudaEventRecord(ev[0], st));
-  // processing order: sorted within blocks of 2^sort_shift sentences (drain segment <= block <= input piece); the
-  // completion of a drain segment is counted per sentence (drain.cuh), so the two granularities are independent.
-  // Sorting whole pieces makes all 32 segments of a piece finish in the same last few groups, whose warps then compact
-  // them one after the other, which serializes the drain; the default stays at the segment size.
-  uint32_t sort_shift = kSegShift;
-  if (const char *v = getenv("SPM_B200_SORT_SHIFT")) sort_shift = std::min<uint32_t>(kPieceShift, std::max<uint32_t>(kSegShift, atoi(v)));
-  const bool fused_sort = !(fx & 8);  // bit 3: input order (completion is counted per sentence: any order drains)
-  if (fused_sort) {
-    const int rc = build_order(s_offsets.p, n, st, &B.order, 1u << sort_shift);
+  // processing order: sorted within each drain segment.  Sorting whole input pieces instead makes all 32 segments of a
+  // piece finish in the same last few groups, whose warps then compact them one after the other, which serializes the
+  // drain.
+  {
+    const int rc = build_order(s_offsets.p, n, st, &B.order, 1u << kSegShift);
     if (rc) return rc;
     if (!B.order) { set_error("fused path needs the segment order"); return SPM_ERR_ARG; }
   }
-  if (bpe && lg.version == 2) encode_bpe_lane2_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
-  else if (bpe) encode_bpe_lane_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap);
+  if (bpe) encode_bpe_lane2_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
   else if (lg.version == 2) encode_unigram_lane_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
   else encode_unigram_lane_plain_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
   CUDA_TRY(cudaGetLastError());
@@ -1550,15 +1459,14 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
     if (q != cudaSuccess && q != cudaErrorNotReady) CUDA_TRY(q);
     const unsigned long long pr = *reinterpret_cast<volatile unsigned long long *>(h_progress.p);
     if (pr > seen && pr <= h_ids.cap) seen = pr;
-    if (!(fx & 1) && seen - copied >= min_copy) {
+    if (seen - copied >= min_copy) {
       CUDA_TRY(cudaMemcpyAsync(h_ids.p + copied, d_ids.p + copied, (seen - copied) * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
       copied = seen;
     }
     if (q == cudaSuccess) break;
   }
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (feeder.joinable()) feeder.join();
-  if (fx & 2) CUDA_TRY(cudaMemcpy(h_id_offsets.p, d_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+  feeder.join();
   if (trace) fprintf(stderr, "[trace] fused kernel done at %.3f ms; warp-cycles: input wait %.1f M, compaction %.1f M (look-back %.1f M), "
                      "%llu groups on %d warps\n", now_ms(), h_ctrl64.p[4] * 1e-6, h_ctrl64.p[5] * 1e-6, h_ctrl64.p[6] * 1e-6,
                      static_cast<unsigned long long>(h_ctrl64.p[7]), grid * (lane_threads / 32));
@@ -1675,15 +1583,7 @@ void parallel_memcpy(void *dst, const void *src, size_t bytes) {
 // decode + scan + gather, and D2H of the text on three streams; inputs and outputs are double buffered.
 int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
                                       const uint64_t **text_offsets) {
-  if (!s_h2d) {
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_h2d, cudaStreamNonBlocking));
-    CUDA_TRY(cudaStreamCreateWithFlags(&s_d2h, cudaStreamNonBlocking));
-    for (int k = 0; k < 2; ++k) {
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_in[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
-      CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
-    }
-  }
+  { const int rc = ensure_copy_streams(); if (rc) return rc; }
   cudaStream_t st = stream;
   const bool trace = getenv("SPM_B200_TRACE") != nullptr;
   const auto t_begin = std::chrono::steady_clock::now();
@@ -1880,7 +1780,6 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 4 * sizeof(unsigned long long), st));
     KBatch B{};
-    B.slab_l2 = slab_l2; B.slab_discard = slab_discard;
     B.bytes = d_bytes.p - base;
     B.offsets = d_offsets.p;
     B.n = static_cast<uint32_t>(n);
@@ -1985,7 +1884,6 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
       CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
       CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 4 * sizeof(unsigned long long), st));
       KBatch B{};
-      B.slab_l2 = slab_l2; B.slab_discard = slab_discard;
       B.bytes = d_bytes.p - base;
       B.offsets = d_offsets.p;
       B.n = static_cast<uint32_t>(m);
@@ -2146,15 +2044,11 @@ static int create_common(spm_engine *e, int device, spm_engine **out) {
     return fail(SPM_ERR_CUDA, "this build targets sm_90a (H100); found compute capability " + std::to_string(prop.major) +
                                   "." + std::to_string(prop.minor));
   e->sm_count = prop.multiProcessorCount;
-  if (const char *v = getenv("SPM_B200_SORT")) e->sort_by_length = atoi(v) != 0;  // A/B knob
+  if (const char *v = getenv("SPM_B200_SORT")) e->sort_by_length = atoi(v) != 0;
   if (const char *v = getenv("SPM_B200_FUSED")) e->fused_host_path = atoi(v) != 0;
   if (const char *v = getenv("SPM_B200_FASTWORDS")) e->force_fast_words = atoi(v) != 0 ? 1 : 0;
   if (const char *v = getenv("SPM_B200_KSTATS")) e->kstats = atoi(v) != 0;
   if (const char *v = getenv("SPM_B200_BPE_CACHE")) e->bpe_cache_log2 = std::min(24, std::max(0, atoi(v)));
-  if (const char *v = getenv("SPM_B200_SLAB_DISCARD")) e->slab_discard = static_cast<uint32_t>(atoi(v));
-  if (const char *v = getenv("SPM_B200_SLAB_L2")) e->slab_l2 = static_cast<uint32_t>(atoi(v));
-  if (const char *v = getenv("SPM_B200_LANE_CAP")) e->lane_cap = std::min(1020, std::max(64, atoi(v))) & ~3;
-  if (const char *v = getenv("SPM_B200_BPE_LANE_V")) e->bpe_lane_version = atoi(v);
   e->smem_optin = prop.sharedMemPerBlockOptin;
   if (cudaSetDevice(device) != cudaSuccess) return fail(SPM_ERR_CUDA, "cudaSetDevice failed");
   int rc = e->build_tables();
@@ -2417,7 +2311,9 @@ int spm_engine_get_info(const spm_engine *e, spm_engine_info *info) {
   info->min_score = e->min_score;
   info->max_score = e->max_score;
   info->trie_units = e->km.trie_units;
-  const LaunchGeom g = plan_geometry(*e, false, e->G, e->threads, e->ncap, e->km.match_slots);
+  const uint32_t tile_bytes = e->model.model_type == SPM_BPE ? bpe_tile_bytes(e->ncap, false)
+                                                              : tile_bytes_for(e->ncap, e->km.match_slots, false);
+  const LaunchGeom g = plan_geometry(*e, tile_bytes, std::min(e->threads, 512) / 32);
   info->trie_hot_units = g.hot_link;
   info->charsmap_units = e->charsmap_units;
   info->last_kernel_launches = e->last_launches;
@@ -2433,7 +2329,7 @@ int spm_engine_set_tuning(spm_engine *e, int lanes, int cap, int ctas) {
   if (!e) return SPM_ERR_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   if (lanes) {
-    if (lanes != 1 && lanes != 4 && lanes != 8 && lanes != 16 && lanes != 32 && lanes != 64) { e->set_error("lanes_per_sentence must be 1, 4, 8, 16, 32 or 64"); return SPM_ERR_ARG; }
+    if (lanes != 1 && lanes != 32) { e->set_error("lanes_per_sentence must be 1 or 32"); return SPM_ERR_ARG; }
     e->G = lanes;
   }
   if (cap) {

@@ -1,10 +1,10 @@
-// kernels.cuh -- sm_90a kernels of the batched subword-encode engine.
+// kernels.cuh -- sm_90a kernels of the batched subword-encode engine: the general path.
 //
-// One sentence is owned by a TILE of G lanes of a warp (G = 32 is the literal
-// "one sentence per warp"; G = 8/16 packs 4/2 sentences into a warp so that the
-// inherently serial parts of the reference algorithm -- the Viterbi relaxation
-// order and the back-trace -- waste fewer lanes).  All cross-lane traffic is
-// warp shuffles / ballots / redux restricted to the tile's lane mask.
+// One sentence is owned by one warp (a TILE of 32 lanes).  The 32 lanes split the
+// parallel parts of the reference algorithm -- normalizing from every byte position,
+// walking the piece trie from every character start -- and take the inherently serial
+// parts -- the Viterbi relaxation order and the back-trace -- in the reference's
+// order.  All cross-lane traffic is warp shuffles / ballots / redux.
 //
 // Per sentence, entirely inside shared memory:
 //   K1 normalize   Normalizer::Normalize + NormalizePrefix   normalizer.cc:71-253
@@ -29,28 +29,20 @@ namespace spm_b200 {
 
 // ---------------------------------------------------------------- tile ----
 
-template <int G>
 struct Tile {
-  uint32_t mask;  // lanes of this tile inside the warp
-  int lane;       // lane inside the tile
-  int shift;      // first warp lane of the tile
-  __device__ __forceinline__ Tile() {
-    const int l = threadIdx.x & 31;
-    lane = l % G;
-    shift = l - lane;
-    mask = (G == 32) ? 0xFFFFFFFFu : (((1u << G) - 1u) << shift);
-  }
-  __device__ __forceinline__ uint32_t ballot(bool p) const { return __ballot_sync(mask, p) >> shift; }
+  int lane;  // lane inside the warp
+  __device__ __forceinline__ Tile() : lane(threadIdx.x & 31) {}
+  __device__ __forceinline__ uint32_t ballot(bool p) const { return __ballot_sync(0xFFFFFFFFu, p); }
   template <typename T>
-  __device__ __forceinline__ T shfl(T v, int src) const { return __shfl_sync(mask, v, src, G); }
-  __device__ __forceinline__ uint32_t red_or(uint32_t v) const { return __reduce_or_sync(mask, v); }
-  __device__ __forceinline__ uint32_t red_add(uint32_t v) const { return __reduce_add_sync(mask, v); }
-  __device__ __forceinline__ void sync() const { __syncwarp(mask); }
+  __device__ __forceinline__ T shfl(T v, int src) const { return __shfl_sync(0xFFFFFFFFu, v, src, 32); }
+  __device__ __forceinline__ uint32_t red_or(uint32_t v) const { return __reduce_or_sync(0xFFFFFFFFu, v); }
+  __device__ __forceinline__ uint32_t red_add(uint32_t v) const { return __reduce_add_sync(0xFFFFFFFFu, v); }
+  __device__ __forceinline__ void sync() const { __syncwarp(0xFFFFFFFFu); }
   // inclusive scan over the tile
   __device__ __forceinline__ uint32_t incl_scan(uint32_t v) const {
 #pragma unroll
-    for (int d = 1; d < G; d <<= 1) {
-      const uint32_t t = __shfl_up_sync(mask, v, d, G);
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, v, d, 32);
       if (lane >= d) v += t;
     }
     return v;
@@ -65,36 +57,36 @@ struct TileMem {
   float *score;     // [ncap + 4]   best_path_score per byte position
   uint32_t *bidx;   // [ncap + 4]   trie unit of the winning piece (kIdxUnk for UNK)
   uint16_t *blen;   // [ncap + 4]   byte length of the winning piece; 0 = unset (starts_at == -1)
-  uint32_t *mval;   // [G * K]      match buffer: score bits / marker
-  uint32_t *midx;   // [G * K]      match buffer: trie unit
-  uint16_t *mlen;   // [G * K]      match buffer: piece byte length
+  uint32_t *mval;   // [32 * K]     match buffer: score bits / marker
+  uint32_t *midx;   // [32 * K]     match buffer: trie unit
+  uint16_t *mlen;   // [32 * K]     match buffer: piece byte length
   uint32_t *n2o;    // [ncap + 4]   (spans) norm_to_orig
   uint8_t *stage;   // input staging (aliases score/bidx)
   uint32_t ncap;
   uint32_t stage_cap;
 };
 
-__host__ __device__ inline uint32_t tile_bytes_for(uint32_t ncap, uint32_t G, uint32_t K, bool spans) {
+__host__ __device__ inline uint32_t tile_bytes_for(uint32_t ncap, uint32_t K, bool spans) {
   uint32_t b = (ncap + 16);                 // text
   b += 4 * (ncap + 4) * 2;                  // score, bidx
   b += 2 * (ncap + 4);                      // blen
-  b += G * K * (4 + 4 + 2);                 // match buffer
+  b += 32 * K * (4 + 4 + 2);                // match buffer
   if (spans) b += 4 * (ncap + 4);
   return (b + 15u) & ~15u;
 }
 
-__device__ __forceinline__ TileMem carve_tile(uint8_t *base, uint32_t ncap, uint32_t G, uint32_t K, bool spans) {
+__device__ __forceinline__ TileMem carve_tile(uint8_t *base, uint32_t ncap, uint32_t K, bool spans) {
   TileMem m;
   uint8_t *p = base;
   m.score = reinterpret_cast<float *>(p); p += 4 * (ncap + 4);
   m.bidx = reinterpret_cast<uint32_t *>(p); p += 4 * (ncap + 4);
   m.stage = reinterpret_cast<uint8_t *>(m.score);
   m.stage_cap = 8 * (ncap + 4);
-  m.mval = reinterpret_cast<uint32_t *>(p); p += 4 * G * K;
-  m.midx = reinterpret_cast<uint32_t *>(p); p += 4 * G * K;
+  m.mval = reinterpret_cast<uint32_t *>(p); p += 4 * 32 * K;
+  m.midx = reinterpret_cast<uint32_t *>(p); p += 4 * 32 * K;
   m.n2o = reinterpret_cast<uint32_t *>(p); if (spans) p += 4 * (ncap + 4);
   m.blen = reinterpret_cast<uint16_t *>(p); p += 2 * (ncap + 4);
-  m.mlen = reinterpret_cast<uint16_t *>(p); p += 2 * G * K;
+  m.mlen = reinterpret_cast<uint16_t *>(p); p += 2 * 32 * K;
   m.text = p;
   m.ncap = ncap;
   return m;
@@ -219,8 +211,8 @@ struct NormResult {
 // chunk kinds
 enum : uint32_t { kChunkChar = 0, kChunkTarget = 1, kChunkFffd = 2, kChunkVerbatim = 3 };
 
-template <int G, bool SPANS>
-__device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile<G> &T, const uint8_t *in,
+template <bool SPANS>
+__device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile &T, const uint8_t *in,
                                                      uint32_t len, const TileMem &tm) {
   const bool rm = M.flags & kFlagRemoveExtraWs;
   const bool esc = M.flags & kFlagEscapeWs;
@@ -248,7 +240,7 @@ __device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile
   uint32_t first_q = 0;  // bytes consumed by the heading-space loop
   uint32_t carry = 0;    // bytes at the start of the window owned by a chunk of the previous one
 
-  for (uint32_t pos = 0; pos < len; pos += G) {
+  for (uint32_t pos = 0; pos < len; pos += 32) {
     const uint32_t q = pos + T.lane;
     const bool act = q < len;
     const uint32_t b = act ? in[q] : 0u;
@@ -296,17 +288,17 @@ __device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile
     const uint32_t actmask = T.ballot(act);
     uint32_t startmask;
     if (T.ballot(act && clen != 1) == 0) {
-      startmask = carry < static_cast<uint32_t>(G) ? (actmask & ~((1u << carry) - 1u)) : 0u;
+      startmask = carry < 32u ? (actmask & ~((1u << carry) - 1u)) : 0u;
     } else {
-      startmask = carry < static_cast<uint32_t>(G) ? (1u << carry) : 0u;
+      startmask = carry < 32u ? (1u << carry) : 0u;
       uint32_t nxt = T.lane + clen;
-      if (nxt > static_cast<uint32_t>(G)) nxt = G;
+      if (nxt > 32u) nxt = 32;
 #pragma unroll
-      for (int d = 1; d < G; d <<= 1) {  // pointer doubling: reach 2^k - 1 hops after k rounds
-        const uint32_t contrib = (((startmask >> T.lane) & 1u) && nxt < static_cast<uint32_t>(G)) ? (1u << nxt) : 0u;
+      for (int d = 1; d < 32; d <<= 1) {  // pointer doubling: reach 2^k - 1 hops after k rounds
+        const uint32_t contrib = (((startmask >> T.lane) & 1u) && nxt < 32u) ? (1u << nxt) : 0u;
         startmask |= T.red_or(contrib);
-        const uint32_t n2 = T.shfl(nxt, nxt < static_cast<uint32_t>(G) ? static_cast<int>(nxt) : 0);
-        nxt = nxt < static_cast<uint32_t>(G) ? n2 : static_cast<uint32_t>(G);
+        const uint32_t n2 = T.shfl(nxt, nxt < 32u ? static_cast<int>(nxt) : 0);
+        nxt = nxt < 32u ? n2 : 32u;
       }
       startmask &= actmask;
     }
@@ -314,9 +306,9 @@ __device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile
     if (startmask) {
       const int last = 31 - __clz(startmask);
       const uint32_t jl = T.shfl(static_cast<uint32_t>(T.lane) + clen, last);
-      carry = jl > static_cast<uint32_t>(G) ? jl - G : 0u;
+      carry = jl > 32u ? jl - 32 : 0u;
     } else {
-      carry -= G;
+      carry -= 32;
     }
     // ---- the chunk's replacement string: length, spaces, leading spaces, last byte ----
     uint32_t L = 0, nsp = 0, lead_sp = 0;
@@ -369,7 +361,7 @@ __device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile
     const uint32_t strip = p ? lead_sp : 0u;
     const uint32_t emit = st ? (L - strip) + (w - 1u) * (nsp - strip) : 0u;
     const uint32_t incl = T.incl_scan(emit);
-    const uint32_t total = T.shfl(incl, G - 1);
+    const uint32_t total = T.shfl(incl, 31);
     if (emit) {
       uint32_t o = out + incl - emit;
       for (uint32_t k = strip; k < L; ++k) {
@@ -435,19 +427,18 @@ __device__ __forceinline__ NormResult normalize_tile(const KModel &M, const Tile
 // parallel (they have distinct end positions).  This reproduces the reference's
 // relaxation order exactly, including Q1 (double candidate vs float-rounded best)
 // and Q2 (strict >, earliest start wins ties).
-template <int G>
-__device__ __forceinline__ void viterbi_tile(const KModel &M, const Tile<G> &T, const HotTrie &H, const TileMem &tm,
+__device__ __forceinline__ void viterbi_tile(const KModel &M, const Tile &T, const HotTrie &H, const TileMem &tm,
                                              uint32_t n) {
   const uint8_t *text = tm.text;
   const uint32_t K = M.match_slots;
-  for (uint32_t k = T.lane; k <= n; k += G) tm.blen[k] = 0;
+  for (uint32_t k = T.lane; k <= n; k += 32) tm.blen[k] = 0;
   if (T.lane == 0) tm.score[0] = 0.f;
   T.sync();
   const uint32_t root_link = H.link(0);
   uint32_t *mval = tm.mval + T.lane * K;
   uint32_t *midx = tm.midx + T.lane * K;
   uint16_t *mlen = tm.mlen + T.lane * K;
-  for (uint32_t wnd = 0; wnd < n; wnd += G) {
+  for (uint32_t wnd = 0; wnd < n; wnd += 32) {
     const uint32_t s = wnd + T.lane;
     uint32_t cnt = 0;
     bool active = false;
@@ -491,7 +482,7 @@ __device__ __forceinline__ void viterbi_tile(const KModel &M, const Tile<G> &T, 
       const uint32_t sj = wnd + j;
       const uint32_t cntj = T.shfl(cnt, j);
       const float till_here = tm.score[sj];  // best_path_score_till_here, :963-964
-      for (uint32_t m = T.lane; m < cntj; m += G) {
+      for (uint32_t m = T.lane; m < cntj; m += 32) {
         const uint32_t val = tm.mval[j * K + m];
         const uint32_t plen = tm.mlen[j * K + m];
         const uint32_t e = sj + plen;
@@ -529,8 +520,8 @@ __device__ __forceinline__ void viterbi_tile(const KModel &M, const Tile<G> &T, 
 // unknown pieces collapse into one id, or -- with byte fallback -- every byte of
 // an unknown piece becomes its <0xXX> id.  Tokens are appended to the batch's
 // temporary id buffer at a position claimed with one atomicAdd per sentence.
-template <int G, bool SPANS>
-__device__ __forceinline__ void finish_tokens(const KModel &M, const KBatch &B, const Tile<G> &T, const uint8_t *text,
+template <bool SPANS>
+__device__ __forceinline__ void finish_tokens(const KModel &M, const KBatch &B, const Tile &T, const uint8_t *text,
                                               const uint32_t *tend, const int32_t *tid, uint32_t sent, uint32_t n_tok) {
   // tokens k = 0..n_tok-1: exclusive end offset tend[k] in the normalized text, vocab id tid[k]
   constexpr uint32_t slot0 = 0;
@@ -538,7 +529,7 @@ __device__ __forceinline__ void finish_tokens(const KModel &M, const KBatch &B, 
   const int32_t unk = M.unk_id;
   // pass 1: count output tokens
   uint32_t count = 0;
-  for (uint32_t k0 = 0; k0 < n_tok; k0 += G) {
+  for (uint32_t k0 = 0; k0 < n_tok; k0 += 32) {
     const uint32_t k = k0 + T.lane;
     uint32_t c = 0;
     if (k < n_tok) {
@@ -563,7 +554,7 @@ __device__ __forceinline__ void finish_tokens(const KModel &M, const KBatch &B, 
   if (pos + count > B.tmp_cap) return;
   // pass 2: write
   uint32_t base = 0;
-  for (uint32_t k0 = 0; k0 < n_tok; k0 += G) {
+  for (uint32_t k0 = 0; k0 < n_tok; k0 += 32) {
     const uint32_t k = k0 + T.lane;
     uint32_t c = 0;
     bool isunk = false;
@@ -598,13 +589,12 @@ __device__ __forceinline__ void finish_tokens(const KModel &M, const KBatch &B, 
         }
       }
     }
-    base += T.shfl(incl, G - 1);
+    base += T.shfl(incl, 31);
   }
 }
 
 // Publishes the normalized text + alignment of one sentence (spans API).
-template <int G>
-__device__ __forceinline__ void publish_norm_tile(const KBatch &B, const Tile<G> &T, const TileMem &tm, uint32_t sent,
+__device__ __forceinline__ void publish_norm_tile(const KBatch &B, const Tile &T, const TileMem &tm, uint32_t sent,
                                                   uint32_t n, bool have_map) {
   unsigned long long pos = 0;
   if (T.lane == 0) {
@@ -615,26 +605,26 @@ __device__ __forceinline__ void publish_norm_tile(const KBatch &B, const Tile<G>
   }
   pos = T.shfl(pos, 0);
   if (pos + n + 1 > B.tmp_norm_cap) return;
-  for (uint32_t k = T.lane; k < n; k += G) B.tmp_norm[pos + k] = tm.text[k];
+  for (uint32_t k = T.lane; k < n; k += 32) B.tmp_norm[pos + k] = tm.text[k];
   if (have_map)
-    for (uint32_t k = T.lane; k <= n; k += G) B.tmp_n2o[pos + k] = tm.n2o[k];
+    for (uint32_t k = T.lane; k <= n; k += 32) B.tmp_n2o[pos + k] = tm.n2o[k];
 }
 
 // One sentence, unigram model: K1 -> K2 -> K4.  Returns false if the sentence does
 // not fit the tile's scratch (the caller defers it to the long-sentence kernel).
-template <int G, bool SPANS>
-__device__ __forceinline__ bool encode_unigram_sentence(const KModel &M, const KBatch &B, const Tile<G> &T,
+template <bool SPANS>
+__device__ __forceinline__ bool encode_unigram_sentence(const KModel &M, const KBatch &B, const Tile &T,
                                                         const HotTrie &H, const TileMem &tm, const uint8_t *in,
                                                         uint32_t len, uint32_t sent, uint32_t *need) {
-  const NormResult nr = normalize_tile<G, SPANS>(M, T, in, len, tm);
+  const NormResult nr = normalize_tile<SPANS>(M, T, in, len, tm);
   const uint32_t n = nr.n;
   if (n > tm.ncap) { *need = n; return false; }
-  if (SPANS) publish_norm_tile<G>(B, T, tm, sent, n, n > 0);
+  if (SPANS) publish_norm_tile(B, T, tm, sent, n, n > 0);
   if (n == 0) {
     if (T.lane == 0) { B.sent_start[sent] = 0; B.sent_count[sent] = 0; }
     return true;
   }
-  viterbi_tile<G>(M, T, H, tm, n);
+  viterbi_tile(M, T, H, tm, n);
   // back-trace by one lane; token records are packed in place at the top of the DP
   // arrays (slot n - t for the t-th token from the end: that slot is >= the current
   // position, whose entry has already been read).
@@ -656,14 +646,14 @@ __device__ __forceinline__ bool encode_unigram_sentence(const KModel &M, const K
   n_tok = T.shfl(n_tok, 0);
   T.sync();
   // resolve trie units to vocab ids (one L2 read per token)
-  for (uint32_t k = T.lane; k < n_tok; k += G) {
+  for (uint32_t k = T.lane; k < n_tok; k += 32) {
     const uint32_t slot = n - n_tok + 1 + k;
     const uint32_t ix = tm.bidx[slot];
     tm.bidx[slot] = static_cast<uint32_t>(ix == kIdxUnk ? M.unk_id : __ldg(M.trie_id + ix));
   }
   T.sync();
-  finish_tokens<G, SPANS>(M, B, T, tm.text, reinterpret_cast<const uint32_t *>(tm.score) + (n - n_tok + 1),
-                          reinterpret_cast<const int32_t *>(tm.bidx) + (n - n_tok + 1), sent, n_tok);
+  finish_tokens<SPANS>(M, B, T, tm.text, reinterpret_cast<const uint32_t *>(tm.score) + (n - n_tok + 1),
+                       reinterpret_cast<const int32_t *>(tm.bidx) + (n - n_tok + 1), sent, n_tok);
   return true;
 }
 
@@ -711,10 +701,9 @@ __device__ __forceinline__ void stage_hot_trie(const KModel &M, uint64_t *mbar, 
 
 // ------------------------------------------------------------- kernels ----
 
-// Persistent kernel: CTAs loop over batches of 32/G consecutive sentences per warp
-// claimed from a global counter; inputs are staged into shared memory with aligned
-// 16-byte loads.
-template <int G, bool SPANS>
+// Persistent kernel: every warp loops over sentences claimed one at a time from a
+// global counter; inputs are staged into shared memory with aligned 16-byte loads.
+template <bool SPANS>
 __global__ void __launch_bounds__(512, 1) encode_unigram_kernel(const KModel M, const KBatch B) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint64_t *mbar = reinterpret_cast<uint64_t *>(smem);
@@ -724,42 +713,36 @@ __global__ void __launch_bounds__(512, 1) encode_unigram_kernel(const KModel M, 
   stage_hot_trie(M, mbar, s_link, s_val);
   HotTrie H{s_link, s_val, M.trie_link, M.trie_val, M.hot_link, M.hot_val};
 
-  constexpr int TPW = 32 / G;
-  const Tile<G> T;
-  const int tile_in_warp = (threadIdx.x & 31) / G;
-  const int tile_in_cta = (threadIdx.x >> 5) * TPW + tile_in_warp;
-  const TileMem tm = carve_tile(tiles + static_cast<size_t>(tile_in_cta) * B.tile_bytes, B.ncap, G, M.match_slots, SPANS);
+  const Tile T;
+  const TileMem tm = carve_tile(tiles + static_cast<size_t>(threadIdx.x >> 5) * B.tile_bytes, B.ncap, M.match_slots, SPANS);
 
   for (;;) {
-    uint32_t first = 0;
-    if ((threadIdx.x & 31) == 0) first = atomicAdd(B.work_counter, static_cast<uint32_t>(TPW));
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
+    uint32_t widx = 0;
+    if (T.lane == 0) widx = atomicAdd(B.work_counter, 1u);
+    widx = __shfl_sync(0xFFFFFFFFu, widx, 0);
     const uint32_t work_n = B.sub_list ? B.sub_n : B.n;
-    if (first >= work_n) break;
-    const uint32_t widx = first + tile_in_warp;
-    if (widx < work_n) {
-      const uint32_t sent = B.sub_list ? B.sub_list[2 * widx] : widx;
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      bool fits = len64 + 32ull <= tm.stage_cap;
-      uint32_t need = 0;
-      if (fits) {
-        const uint32_t len = static_cast<uint32_t>(len64);
-        // coalesced, vectorised staging of the input bytes (16-byte aligned loads)
-        const uint8_t *g = B.bytes + off;
-        const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(g) & 15u);
-        const uint4 *ga = reinterpret_cast<const uint4 *>(g - mis);
-        const uint32_t nvec = (mis + len + 15u) >> 4;
-        uint4 *sa = reinterpret_cast<uint4 *>(tm.stage);
-        for (uint32_t v = T.lane; v < nvec; v += G) sa[v] = __ldg(ga + v);
-        T.sync();
-        fits = encode_unigram_sentence<G, SPANS>(M, B, T, H, tm, tm.stage + mis, len, sent, &need);
-      }
-      if (!fits && T.lane == 0) {
-        const uint32_t slot = atomicAdd(B.status, 1u);
-        B.deferred[2 * slot] = sent;
-        B.deferred[2 * slot + 1] = need;  // exact normalized length if known, else 0
-      }
+    if (widx >= work_n) break;
+    const uint32_t sent = B.sub_list ? B.sub_list[2 * widx] : widx;
+    const unsigned long long off = B.offsets[sent];
+    const unsigned long long len64 = B.offsets[sent + 1] - off;
+    bool fits = len64 + 32ull <= tm.stage_cap;
+    uint32_t need = 0;
+    if (fits) {
+      const uint32_t len = static_cast<uint32_t>(len64);
+      // coalesced, vectorised staging of the input bytes (16-byte aligned loads)
+      const uint8_t *g = B.bytes + off;
+      const uint32_t mis = static_cast<uint32_t>(reinterpret_cast<uintptr_t>(g) & 15u);
+      const uint4 *ga = reinterpret_cast<const uint4 *>(g - mis);
+      const uint32_t nvec = (mis + len + 15u) >> 4;
+      uint4 *sa = reinterpret_cast<uint4 *>(tm.stage);
+      for (uint32_t v = T.lane; v < nvec; v += 32) sa[v] = __ldg(ga + v);
+      T.sync();
+      fits = encode_unigram_sentence<SPANS>(M, B, T, H, tm, tm.stage + mis, len, sent, &need);
+    }
+    if (!fits && T.lane == 0) {
+      const uint32_t slot = atomicAdd(B.status, 1u);
+      B.deferred[2 * slot] = sent;
+      B.deferred[2 * slot + 1] = need;  // exact normalized length if known, else 0
     }
     __syncwarp();
   }
@@ -775,7 +758,7 @@ __global__ void __launch_bounds__(256) encode_unigram_long_kernel(const KModel M
   uint32_t *s_val = s_link + M.hot_link;
   stage_hot_trie(M, mbar, s_link, s_val);
   HotTrie H{s_link, s_val, M.trie_link, M.trie_val, M.hot_link, M.hot_val};
-  const Tile<32> T;
+  const Tile T;
   const uint32_t warps_per_cta = blockDim.x >> 5;
   for (uint32_t w = blockIdx.x * warps_per_cta + (threadIdx.x >> 5); w < B.long_n; w += gridDim.x * warps_per_cta) {
     const uint32_t sent = B.long_list[2 * w];
@@ -784,11 +767,11 @@ __global__ void __launch_bounds__(256) encode_unigram_long_kernel(const KModel M
     // invert tile_bytes_for(): the host sized the slab for ncap
     const uint32_t ncap = B.long_list[2 * w + 1];
     (void)bytes;
-    const TileMem tm = carve_tile(B.long_scratch + so, ncap, 32, M.match_slots, SPANS);
+    const TileMem tm = carve_tile(B.long_scratch + so, ncap, M.match_slots, SPANS);
     const unsigned long long off = B.offsets[sent];
     const uint32_t len = static_cast<uint32_t>(B.offsets[sent + 1] - off);
     uint32_t need = 0;
-    const bool ok = encode_unigram_sentence<32, SPANS>(M, B, T, H, tm, B.bytes + off, len, sent, &need);
+    const bool ok = encode_unigram_sentence<SPANS>(M, B, T, H, tm, B.bytes + off, len, sent, &need);
     if (!ok && T.lane == 0) atomicOr(B.status + 1, 2u);  // slab was sized from an upper bound: cannot happen
     __syncwarp();
   }

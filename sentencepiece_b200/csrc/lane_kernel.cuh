@@ -115,14 +115,16 @@ struct LaneCtx {
 
 // The per-lane slabs (normalized text, back-pointer log) are written and read back within one group: ~12 KB per
 // resident warp, tens of MB per GPU, within H100's 50 MB L2 -- but only stays there if the batch's streamed input and ids do not
-// push it out.  Every slab access carries an L2 eviction-priority hint (evict_last); the once-read input and the
-// once-written ids use the streaming forms (__ldcs / __stcs).
-__device__ __forceinline__ unsigned long long slab_policy(uint32_t mode) {
+// push it out.  Every slab access carries an L2 cache policy (evict_normal); the once-read input and the once-written
+// ids use the streaming forms (__ldcs / __stcs), and the dead rows are discarded at the end of a group (slab_discard).
+// The hinted accesses read the policy from a uniform register.  The redux makes the value warp-uniform for the
+// compiler, so it stays in uniform registers instead of being copied into one (R2UR) at every access.
+__device__ __forceinline__ unsigned long long slab_policy() {
   unsigned long long pol;
-  if (mode == 1u) asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
-  else if (mode == 2u) asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  else asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
+  asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+  const uint32_t lo = __reduce_or_sync(0xFFFFFFFFu, static_cast<uint32_t>(pol));
+  const uint32_t hi = __reduce_or_sync(0xFFFFFFFFu, static_cast<uint32_t>(pol >> 32));
+  return (static_cast<unsigned long long>(hi) << 32) | lo;
 }
 __device__ __forceinline__ uint32_t slab_ld(const uint32_t *p, unsigned long long pol) {
   uint32_t v;
@@ -500,7 +502,7 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
       }
     }
   }
-  if (B.slab_discard) slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
+  slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
 }
 
 // shared memory per warp: ring of R slots, each {score f32, back-pointer u32, position tag u16} x 32 lanes
@@ -528,7 +530,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
   LaneCtx c;
-  c.pol = slab_policy(B.slab_l2);
+  c.pol = slab_policy();
   uint16_t *rp;  // ring position tags: a slot belongs to position p iff rp == p (no clearing, skipped positions
                  // of whole words leave stale slots behind that simply fail the test)
   {
@@ -801,7 +803,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
   LaneCtx c;
-  c.pol = slab_policy(B.slab_l2);
+  c.pol = slab_policy();
   {
     uint8_t *ring = rings + static_cast<size_t>(warp_in_cta) * (R * 32 * 8);
     c.rs = reinterpret_cast<float *>(ring) + lane;

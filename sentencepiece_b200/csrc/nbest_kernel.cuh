@@ -72,7 +72,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   LaneCtx c;
-  c.pol = slab_policy(B.slab_l2);
+  c.pol = slab_policy();
   {
     uint8_t *slab = text_slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(G.cap);
     c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;

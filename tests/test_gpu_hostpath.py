@@ -14,7 +14,7 @@ N = 420_000  # > pipeline_min_sentences (300k): spm_encode_ids takes the large-b
 
 
 def _engine(model, **env):
-    """engine created under the given SPM_B200_* experiment knobs (read at engine creation)"""
+    """engine created under the given SPM_B200_* environment settings (read at engine creation)"""
     from sentencepiece_b200 import Engine
     old = {k: os.environ.get(k) for k in env}
     os.environ.update({k: str(v) for k, v in env.items()})
@@ -108,7 +108,8 @@ def test_bpe_long_words_stay_in_the_lane_kernel(corpus_gen):
     eng = _engine("bpe32k")
     a, ao = eng.encode_packed(rb, ro)
     assert eng.info().last_deferred == 0
-    ref = _engine("bpe32k", SPM_B200_FUSED=0, SPM_B200_SORT=0, SPM_B200_BPE_LANE_V=1)
+    ref = _engine("bpe32k", SPM_B200_FUSED=0, SPM_B200_SORT=0)
+    ref.set_tuning(32, 0, 0)  # the general BPE kernel (bpe_kernel.cuh) as the reference
     b, bo = ref.encode_packed(rb, ro)
     assert np.array_equal(ao, bo) and np.array_equal(a, b)
     om = oracle_py.OracleModel(model_bytes("bpe32k"))

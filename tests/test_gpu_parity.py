@@ -215,16 +215,22 @@ def test_device_pointer_api(corpus_gen):
 
 
 def test_tuning_variants_agree(corpus_gen):
-    """every kernel variant (tile widths, CTA sizes, the general tile kernel) gives the same ids"""
+    """every tuning (the general kernel at several shared-memory caps and CTA sizes, the lane kernels at several CTA
+    sizes) gives the same ids; lanes_per_sentence other than 1 and 32 is rejected"""
     from sentencepiece_b200 import Engine
     buf, offs = corpus_gen.fill("mixed", 4007, 4000)
     mb = model_bytes("mix_bf8k")
     ref = oracle_py.OracleModel(mb).encode_batch(buf, offs)
-    for lanes, cap, thr in [(32, 256, 1024), (32, 128, 512), (8, 256, 256), (16, 192, 512), (4, 128, 128)]:
+    for lanes, cap, thr in [(32, 256, 512), (32, 128, 512), (32, 192, 256), (32, 128, 128), (1, 0, 512), (1, 0, 768)]:
         eng = Engine(mb)
         eng.set_tuning(lanes, cap, thr)
         assert_same(*eng.encode_packed(buf, offs), *ref, f"lanes={lanes} cap={cap} threads={thr}")
         eng.close()
+    eng = Engine(mb)
+    for lanes in (8, 64):
+        with pytest.raises(RuntimeError):
+            eng.set_tuning(lanes, 0, 0)
+    eng.close()
 
 
 @pytest.mark.parametrize("workload", [("uni32k", "en"), ("bpe32k", "en")])

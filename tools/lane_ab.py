@@ -1,11 +1,9 @@
 """A/B of the lane-kernel generations on an H100: ids must be identical, times are printed.
 
-usage: python tools/lane_ab.py [model:kind ...] [--n N] [--variants "FW=0;FW=1;BV=1;BV=2,T=704"]
+usage: python tools/lane_ab.py [model:kind ...] [--n N] [--variants "FW=0;FW=1;T=512"]
 Each variant is a ';'-separated item of ','-separated KEY=VALUE knobs:
-  FW whole-word shortcut (SPM_B200_FASTWORDS), S length ordering (SPM_B200_SORT),
-  T threads per CTA, BV BPE lane kernel version (SPM_B200_BPE_LANE_V), L2 eviction priority of the slab
-  CR=1 empties the BPE word cache before every launch, C log2 of its entries (SPM_B200_BPE_CACHE), D discard of dead slab
-  rows (SPM_B200_SLAB_DISCARD), G sort block of the device path (SPM_B200_SORT_SEG), accesses (SPM_B200_SLAB_L2: 0 normal, 1 evict_last, 2 evict_first), CAP slab capacity per lane (SPM_B200_LANE_CAP).
+  FW whole-word shortcut (SPM_B200_FASTWORDS), S length ordering (SPM_B200_SORT), T threads per CTA,
+  CR=1 empties the BPE word cache before every launch, C log2 of its entries (SPM_B200_BPE_CACHE).
 """
 import argparse
 import os
@@ -20,8 +18,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import corpus  # noqa: E402
 from sentencepiece_b200 import Engine  # noqa: E402
 
-ENV = {"FW": "SPM_B200_FASTWORDS", "L2": "SPM_B200_SLAB_L2", "D": "SPM_B200_SLAB_DISCARD", "C": "SPM_B200_BPE_CACHE", "G": "SPM_B200_SORT_SEG", "CAP": "SPM_B200_LANE_CAP",
-       "BV": "SPM_B200_BPE_LANE_V", "S": "SPM_B200_SORT"}
+ENV = {"FW": "SPM_B200_FASTWORDS", "C": "SPM_B200_BPE_CACHE", "S": "SPM_B200_SORT"}
 
 ap = argparse.ArgumentParser()
 ap.add_argument("workloads", nargs="*", default=["uni32k:en"])

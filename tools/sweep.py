@@ -1,5 +1,6 @@
-"""Tuning sweep on an H100: encode-kernel time for the device-resident workload under
-different tile widths / CTA sizes / shared-memory caps.  usage: python tools/sweep.py [workload] [n]"""
+"""Tuning sweep on an H100: encode-kernel time for the device-resident workload under different
+kernels (lanes per sentence 1 or 32), CTA sizes and shared-memory caps.
+usage: python tools/sweep.py [workload] [n] [lanes,threads,cap ...]"""
 import itertools
 import os
 import sys

@@ -1,5 +1,5 @@
 """Host-path traces of the fused path (SPM_B200_TRACE=1: timeline + per-phase cycles per warp) for the bench corpora.
-usage: python tools/trace_e2e.py [model:kind ...]   (env: SPM_B200_FUSED_X experiment bits, T threads per CTA)"""
+usage: python tools/trace_e2e.py [model:kind ...]   (env: T threads per CTA)"""
 import os, sys, time
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -21,10 +21,10 @@ for model, kind in todo:
         t0 = time.perf_counter()
         try:
             ids, ido = eng.encode_packed(pb, po, copy=False)
-        except Exception as e:  # noqa: BLE001 (timing experiments with invalid results)
+        except Exception as e:  # noqa: BLE001
             ids, ido = np.zeros(0), np.zeros(1)
             print("   (call failed:", str(e)[:80], ")")
         dt = time.perf_counter() - t0
-        print(f"{model}/{kind} rep {rep} [{os.environ.get('SPM_B200_FUSED_X','-')}]: {dt*1e3:.2f} ms, device kernel {eng.info().last_main_kernel_ms:.3f} ms, {len(offs)-1} sentences, {len(ids)} ids, bytes {int(offs[-1])}", flush=True)
+        print(f"{model}/{kind} rep {rep}: {dt*1e3:.2f} ms, device kernel {eng.info().last_main_kernel_ms:.3f} ms, {len(offs)-1} sentences, {len(ids)} ids, bytes {int(offs[-1])}", flush=True)
     os.environ.pop("SPM_B200_TRACE", None)
     eng.close()
