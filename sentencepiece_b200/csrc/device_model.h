@@ -36,8 +36,10 @@ struct KModel {
   const int32_t *trie_id;
   const uint2 *trie_node2;  // {link, child mask} interleaved (one 8-byte load per transition)
   // {link, child mask, score bits, word_safe} (unigram lane kernel: one 16-byte load per transition brings the piece
-  // score and the whole-word limit along, so neither costs a second dependent lookup)
+  // score and the whole-word limit along, so neither costs a second dependent lookup).  A double array of its own:
+  // the same keys with U+2581 spelled as the one byte kWsByte (lane_kernel.cuh), units numbered independently.
   const uint4 *trie_node4;
+  const int32_t *trie_id_ws;  // vocab id of the piece ending at a trie_node4 unit, -1 otherwise
   uint32_t trie_units;
   uint32_t hot_link;   // units of trie_link staged into shared memory by each CTA (multiple of 4)
   uint32_t hot_val;    // units of trie_val staged (multiple of 4)
@@ -58,8 +60,9 @@ struct KModel {
   const int32_t *byte_to_id;  // [256] PieceToId(ByteToPiece(b)), sentencepiece_processor.cc:587-588
   const float *scores;        // [vocab] (BPE: score of a piece id)
   const uint8_t *types;       // [vocab] live piece types
-  // [trie_units] whole-word shortcut (lane_kernel.cuh): a word that is exactly the piece at this unit and ends at a normalized
-  // byte position <= word_safe[unit] is certain to be encoded as that piece alone (0 = never); see engine.cu
+  // [trie_node4 units] whole-word shortcut (lane_kernel.cuh): a word that is exactly the piece at this unit and ends at a
+  // normalized byte position (U+2581 as one byte) <= word_safe[unit] is certain to be encoded as that piece alone
+  // (0 = never); see engine.cu
   const uint16_t *word_safe;
   // [trie_units] BPE lane2 kernel: vocab id of the piece at this unit when a word that is exactly the piece encodes
   // to that single id (its merge sequence reproduces it), else 0xFFFFFFFF

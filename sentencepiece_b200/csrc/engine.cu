@@ -116,6 +116,22 @@ bool valid_utf8(const char *s, size_t n) {
   return true;
 }
 
+// A piece as encode_unigram_lane_kernel spells it: every U+2581 (E2 96 81) becomes the one byte kWsByte.  Pieces are
+// valid UTF-8, so E2 96 81 is always that character and the respelling is one to one.
+std::string spell_ws_byte(const char *p, size_t n) {
+  std::string s;
+  s.reserve(n);
+  for (size_t i = 0; i < n; ++i) {
+    if (i + 2 < n && p[i] == '\xE2' && p[i + 1] == '\x96' && p[i + 2] == '\x81') {
+      s.push_back(static_cast<char>(kWsByte));
+      i += 2;
+    } else {
+      s.push_back(p[i]);
+    }
+  }
+  return s;
+}
+
 }  // namespace
 
 struct spm_engine {
@@ -129,6 +145,9 @@ struct spm_engine {
 
   ModelData model;
   DeviceTrie trie, user_trie;
+  // unigram: the piece trie with every U+2581 spelled as the one byte kWsByte (lane_kernel.cuh), the key set of
+  // encode_unigram_lane_kernel's normalized text; its own unit order, node4 table and unit -> id array
+  DeviceTrie trie_ws;
   float min_score = 0.f, max_score = 0.f;
   int32_t unk_id = -1;
   uint32_t max_expand_num = 3, max_expand_den = 1;  // worst-case normalized bytes per input byte
@@ -137,7 +156,7 @@ struct spm_engine {
 
   // device tables
   DevBuf<uint32_t> d_link, d_val, d_user_link, d_cm_units, d_cm_lead, d_cm_pair, d_node2;
-  DevBuf<int32_t> d_id, d_cm_solo, d_byte_to_id;
+  DevBuf<int32_t> d_id, d_id_ws, d_cm_solo, d_byte_to_id;
   DevBuf<uint8_t> d_cm_targets, d_types;
   DevBuf<float> d_scores;
   DevBuf<uint16_t> d_word_safe;
@@ -207,7 +226,7 @@ struct spm_engine {
   DevBuf<unsigned long long> d_seg_words;
   // Launch geometry of the lane kernels for an ids-only batch; ok == false: the model / tuning is outside the lane
   // kernels (the general warp-per-sentence kernels take the batch).  Shared memory per warp grows with the longest
-  // piece (ring of max piece length + 2 slots), so the warps per CTA shrink until the rings fit.
+  // piece (ring of max(max piece length, 4) + 2 slots), so the warps per CTA shrink until the rings fit.
   struct LaneGeom {
     bool ok = false;
     int version = 1;       // unigram: 2 = encode_unigram_lane_kernel (whole-word shortcut), 1 = the plain instantiation
@@ -239,8 +258,11 @@ struct spm_engine {
       return g;
     }
     if (trie.max_key_len > 62) return g;
-    g.R = trie.max_key_len + 2;
     g.version = ((km.flags & kFlagFastWords) && batch_fast_words) ? 2 : 1;  // 2: whole-word shortcut, 1: plain
+    // ring of the longest edge + 2 slots: an edge is a piece (version 2 walks the one-byte-U+2581 keys) or the UNK edge
+    // over one character, up to 4 bytes -- the kernels step the ring index by an edge length with a single wrap
+    const uint32_t longest = g.version == 2 ? trie_ws.max_key_len : trie.max_key_len;
+    g.R = std::max<uint32_t>(longest, 4) + 2;
     const size_t ring = g.version == 2 ? lane_ring_bytes(g.R) : static_cast<size_t>(g.R) * 32 * 8;
     const int warps = static_cast<int>(std::min<size_t>(threads / 32, avail / ring));
     if (warps < 4) return g;
@@ -400,6 +422,18 @@ int spm_engine::build_tables() {
   if (!BuildDeviceTrie(keys, V, &trie, &e)) { set_error(e); return SPM_ERR_MODEL; }
   if (trie.max_key_len > 255) { set_error("pieces longer than 255 bytes are not supported by the device path"); return SPM_ERR_UNSUPPORTED; }
   if (!user_keys.empty() && !BuildDeviceTrie(user_keys, V, &user_trie, &e)) { set_error(e); return SPM_ERR_MODEL; }
+  // the same key set, weights and kinds with U+2581 as one byte (encode_unigram_lane_kernel)
+  trie_ws = DeviceTrie();
+  if (m.model_type == SPM_UNIGRAM) {
+    std::vector<std::string> spelled(keys.size());
+    std::vector<TrieKey> ws_keys = keys;
+    for (size_t j = 0; j < keys.size(); ++j) {
+      spelled[j] = spell_ws_byte(keys[j].data, keys[j].len);
+      ws_keys[j].data = spelled[j].data();
+      ws_keys[j].len = static_cast<uint32_t>(spelled[j].size());
+    }
+    if (!BuildDeviceTrie(ws_keys, V, &trie_ws, &e)) { set_error(e); return SPM_ERR_MODEL; }
+  }
 
   // ---- byte fallback ids (sentencepiece_processor.cc:587-588) ----
   std::vector<int32_t> byte_to_id(256, unk_id);
@@ -546,8 +580,14 @@ int spm_engine::build_tables() {
 // each of magnitude <= maxabs).  So a later candidate into e is at most B + S_alt + c * ulp(Vmax) and cannot
 // exceed the stored value (>= B + S_P - ulp(Vmax)) when  S_P - S_alt > (c + 1) * ulp(Vmax).  The table stores the
 // largest e for which that holds with a further factor of two of slack on both the margin and Vmax.
+//
+// The kernel spells U+2581 as the one byte kWsByte, in its normalized text and in its trie (trie_ws), so positions,
+// e and the keys here are all in that spelling.  The segmentations of a word, their edges and their scores are the
+// same in either spelling, so S_P - S_alt and c do not change.  The bound on Vmax still holds: a path into e has at
+// most one edge per character, and every character, U+2581 included, still takes at least one byte, so there are at
+// most e edges of magnitude <= maxabs.
 int spm_engine::upload_word_safe() {
-  std::vector<uint16_t> safe(trie.link.size(), 0);
+  std::vector<uint16_t> safe(trie_ws.link.size(), 0);
   const bool eligible = fast_words && model.model_type == SPM_UNIGRAM && bpe_word_split && model.escape_whitespaces &&
                         !model.treat_whitespace_as_suffix && !any_user_defined && trie.max_key_len <= 62;
   km.flags &= ~kFlagFastWords;
@@ -562,31 +602,32 @@ int spm_engine::upload_word_safe() {
     std::vector<double> E;
     for (int i = 0; i < V; ++i) {
       if (model.types[i] != SPM_NORMAL) continue;
-      const uint32_t unit = trie.unit_of_id[i];
+      const uint32_t unit = trie_ws.unit_of_id[i];
       if (unit == 0xFFFFFFFFu) continue;
-      const unsigned char *p = reinterpret_cast<const unsigned char *>(model.piece(i));
-      const uint32_t L = static_cast<uint32_t>(model.piece_len(i));
+      const std::string key = spell_ws_byte(model.piece(i), model.piece_len(i));
+      const unsigned char *p = reinterpret_cast<const unsigned char *>(key.data());
+      const uint32_t L = static_cast<uint32_t>(key.size());
       E.assign(L + 1, kNegInf);
       E[0] = 0.0;
       uint32_t chars = 0;
       for (uint32_t st = 0; st < L;) {
         static const uint8_t kLen[16] = {1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 3, 4};  // OneCharLen, util.h:151-153
-        const uint32_t mb = std::min<uint32_t>(kLen[p[st] >> 4], L - st);
+        const uint32_t mb = p[st] == kWsByte ? 1u : std::min<uint32_t>(kLen[p[st] >> 4], L - st);
         ++chars;
         if (E[st] > kNegInf) {
           bool has_single = false;
-          uint32_t l = trie.link[0];
+          uint32_t l = trie_ws.link[0];
           for (uint32_t k = st; k < L; ++k) {
             const uint32_t v = (l >> kLinkBaseShift) ^ p[k];
-            if (v >= trie.link.size() || (trie.link[v] & kLinkLabelMask) != p[k]) break;
-            l = trie.link[v];
+            if (v >= trie_ws.link.size() || (trie_ws.link[v] & kLinkLabelMask) != p[k]) break;
+            l = trie_ws.link[v];
             const uint32_t kind = (l >> kLinkKindShift) & 3u;
             if (kind != kKindNormal && kind != kKindUserDefined) continue;
             const uint32_t len = k + 1 - st;
             if (len == mb) has_single = true;
             if (st == 0 && len == L) continue;  // the whole-word edge itself
             float sc;
-            memcpy(&sc, &trie.val[v], 4);
+            memcpy(&sc, &trie_ws.val[v], 4);
             E[st + len] = std::max(E[st + len], E[st] + static_cast<double>(sc));
           }
           if (!has_single) E[st + mb] = std::max(E[st + mb], E[st] + unk);
@@ -668,10 +709,13 @@ int spm_engine::upload_word_safe() {
     km.bpe_cache_mask = static_cast<uint32_t>(entries - 1);
   }
   {
-    std::vector<uint4> n4(trie.link.size());
-    for (size_t u = 0; u < trie.link.size(); ++u) n4[u] = make_uint4(trie.link[u], trie.cmask[u], trie.val[u], safe[u]);
+    std::vector<uint4> n4(trie_ws.link.size());
+    for (size_t u = 0; u < trie_ws.link.size(); ++u)
+      n4[u] = make_uint4(trie_ws.link[u], trie_ws.cmask[u], trie_ws.val[u], safe[u]);
     CUDA_TRY(d_node4.upload(n4));
+    CUDA_TRY(d_id_ws.upload(trie_ws.id));
     km.trie_node4 = d_node4.p;
+    km.trie_id_ws = d_id_ws.p;
   }
   return SPM_OK;
 }
@@ -693,6 +737,10 @@ int spm_engine::upload_types() {
     const uint8_t t = model.types[i];
     const uint32_t kind = t == SPM_NORMAL ? kKindNormal : (t == SPM_USER_DEFINED ? kKindUserDefined : kKindUnused);
     trie.link[u] = (trie.link[u] & ~(3u << kLinkKindShift)) | (kind << kLinkKindShift);
+    if (!trie_ws.link.empty()) {
+      const uint32_t uw = trie_ws.unit_of_id[i];
+      trie_ws.link[uw] = (trie_ws.link[uw] & ~(3u << kLinkKindShift)) | (kind << kLinkKindShift);
+    }
   }
   bool any_unused = false;
   any_user_defined = false;
@@ -930,7 +978,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       CUDA_TRY(cudaMemcpy(ks, d_kstats.p, sizeof ks, cudaMemcpyDeviceToHost));
       if (ks[12])
         fprintf(stderr, "[kstats] groups %llu: warp trips/group %.1f, lane trips/sentence %.1f (lane utilisation of K2 %.3f), starts/sentence "
-                "%.1f (whole words %.1f), normalized bytes/sentence %.1f\n", ks[12], double(ks[8]) / ks[12], double(ks[9]) / n,
+                "%.1f (whole words %.1f), normalized bytes/sentence %.1f (U+2581 as one byte)\n", ks[12], double(ks[8]) / ks[12], double(ks[9]) / n,
                 double(ks[9]) / (32.0 * ks[8]), double(ks[10]) / n, double(ks[11]) / n, double(ks[13]) / n);
       if (ks[4]) {
         const double w = 1e-6 / (static_cast<double>(grid) * geom.tiles);
@@ -2106,7 +2154,7 @@ void spm_engine_destroy(spm_engine *e) {
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
   e->d_link.release(); e->d_val.release(); e->d_user_link.release(); e->d_cm_units.release(); e->d_cm_lead.release();
-  e->d_cm_pair.release(); e->d_id.release(); e->d_cm_solo.release(); e->d_byte_to_id.release(); e->d_cm_targets.release();
+  e->d_cm_pair.release(); e->d_id.release(); e->d_id_ws.release(); e->d_cm_solo.release(); e->d_byte_to_id.release(); e->d_cm_targets.release();
   e->d_types.release(); e->d_scores.release(); e->d_word_safe.release(); e->d_node4.release(); e->d_word_fast.release(); e->d_bpe_cache.release(); e->d_kstats.release(); e->d_sample.release(); e->d_bytes.release(); e->d_tmp_norm.release(); e->d_norm.release();
   e->d_long_scratch.release(); e->d_offsets.release(); e->d_tmp_ids.release(); e->d_ids.release();
   e->d_tmp_tok_end.release(); e->d_tok_end.release(); e->d_tmp_n2o.release(); e->d_n2o.release();

@@ -32,6 +32,12 @@
 namespace spm_b200 {
 
 constexpr uint32_t kLaneUnk = 0x3FFFFFu;  // 22-bit trie-unit field: UNK piece
+// encode_unigram_lane_kernel spells U+2581 as this one byte, in its normalized text and in its trie (KModel::trie_node4):
+// a walk from a word start takes one transition on it instead of three, and the text is two bytes shorter per word.
+// 0xFF never occurs in the normalized text otherwise (it is valid UTF-8: malformed bytes become U+FFFD, pieces and
+// charsmap targets are checked at load), and both sides of every comparison change alike, so the lattice -- characters,
+// candidate pieces, scores, relaxation order -- is the same.
+constexpr uint32_t kWsByte = 0xFFu;
 
 // slab geometry: per warp [text words: cap/4 + 12][32] u32, then [log: cap + 4][32] u32
 constexpr uint32_t kLaneTextSlack = 12;  // window loads may run a few words past the text
@@ -200,6 +206,12 @@ struct ByteStream {
 
 // Sequential normalizer for one lane.  Returns the normalized length, or 0xFFFFFFFF if
 // it exceeds `cap` (the caller defers the sentence).
+// kWs1: every U+2581 -- escaped spaces, literal ones from the input or a charsmap target -- is written as kWsByte and
+// the returned length counts it as one byte.  The cap still applies to the length with U+2581 as three bytes (out +
+// saved), tested where the three-byte spelling tests it -- before the trailing strip, and again before the suffix --
+// so the same sentences are deferred in either spelling.  (Before the strip out and saved only grow, so the test on
+// their final sum sees the largest length, as the three-byte spelling's overflow flag does.)
+template <bool kWs1 = false>
 __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_t *in, uint32_t len, const LaneCtx &c,
                                                    uint32_t cap) {
   const bool rm = M.flags & kFlagRemoveExtraWs;
@@ -213,6 +225,7 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
   S.init(in, in + len);
   uint32_t out = 0;  // normalized bytes produced
   uint32_t acc = 0;  // partial word
+  uint32_t saved = 0;  // kWs1: 2 per U+2581 written (out + saved = the length with U+2581 as three bytes)
   bool overflow = false;
   auto put = [&](uint32_t ch) {
     acc |= ch << ((out & 3u) * 8u);
@@ -222,8 +235,11 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
     }
     ++out;
   };
+  auto put_u2581 = [&]() {
+    if (kWs1) { put(kWsByte); saved += 2; } else { put(0xE2); put(0x96); put(0x81); }
+  };
   auto put_ws = [&]() {
-    if (esc) { put(0xE2); put(0x96); put(0x81); } else { put(' '); }
+    if (esc) put_u2581(); else put(' ');
   };
   uint32_t pos = 0;
   bool is_prev_space = rm;  // normalizer.cc:130
@@ -250,10 +266,11 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
           const uint32_t ch = (w4 >> (8 * i)) & 0xFFu;
           const bool sp = ch == ' ';
           const bool emit = !(sp && prev);
-          const uint32_t bytes = (sp && esc) ? 0x8196E2u : ch;  // U+2581 = E2 96 81
-          const uint32_t blen = emit ? ((sp && esc) ? 3u : 1u) : 0u;
+          const uint32_t bytes = (sp && esc) ? (kWs1 ? kWsByte : 0x8196E2u) : ch;  // U+2581 = E2 96 81
+          const uint32_t blen = emit ? ((sp && esc && !kWs1) ? 3u : 1u) : 0u;
           chunk |= static_cast<unsigned long long>(emit ? bytes : 0u) << (8u * clen);
           clen += blen;
+          if (kWs1) saved += (emit && sp && esc) ? 2u : 0u;
           prev = sp && rm;
         }
         is_prev_space = prev;
@@ -337,9 +354,13 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
         }
         if (!started) { started = true; if (addp && !suffix) put_ws(); }
         if (l) {  // a valid multi-byte character: never a space
-          put(b); put(b1);
-          if (l > 2) put(b2);
-          if (l > 3) put(b3);
+          if (kWs1 && l == 3 && b == 0xE2u && b1 == 0x96u && b2 == 0x81u) {
+            put_u2581();  // a literal U+2581 (still not a space for remove_extra_whitespaces)
+          } else {
+            put(b); put(b1);
+            if (l > 2) put(b2);
+            if (l > 3) put(b3);
+          }
           consumed = l;
         } else {  // malformed: one byte -> U+FFFD (normalizer.cc:231-244)
           put(0xEF); put(0xBF); put(0xBD);
@@ -369,7 +390,15 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
         uint32_t last = 0;
         for (uint32_t i = i0; i < spl; ++i) {
           last = sp_byte(i);
-          if (last == ' ' && esc) { put(0xE2); put(0x96); put(0x81); } else put(last);
+          if (last == ' ' && esc) {
+            put_u2581();
+          } else if (kWs1 && last == 0xE2u && i + 2 < spl && sp_byte(i + 1) == 0x96u && sp_byte(i + 2) == 0x81u) {
+            put_u2581();  // a literal U+2581 in a rule target or user symbol
+            i += 2;
+            last = 0x81u;
+          } else {
+            put(last);
+          }
         }
         is_prev_space = last == ' ';
       }
@@ -379,21 +408,23 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
     if (consumed <= 4) S.consume(consumed); else S.init(in + pos, in + len);
   }
   if (!started) return 0;  // all chars are whitespace (:97-100)
-  if (overflow || out > cap) return 0xFFFFFFFFu;
+  if (overflow || out + saved > cap) return 0xFFFFFFFFu;
   // flush the partial word, then strip trailing spaces on the escaped output (:166-176)
   slab_st(c.text_w + static_cast<size_t>(out >> 2) * 32, acc, c.pol);
   if (rm) {
     auto byte_at = [&](uint32_t k) -> uint32_t {
       return (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
     };
-    if (esc) {
+    if (esc && kWs1) {
+      while (out >= 1 && byte_at(out - 1) == kWsByte) { out -= 1; saved -= 2; }
+    } else if (esc) {
       while (out >= 3 && byte_at(out - 3) == 0xE2 && byte_at(out - 2) == 0x96 && byte_at(out - 1) == 0x81) out -= 3;
     } else {
       while (out >= 1 && byte_at(out - 1) == ' ') out -= 1;
     }
   }
   if (suffix && addp) {  // :179
-    if (out + 3 > cap) return 0xFFFFFFFFu;
+    if (out + saved + 3 > cap) return 0xFFFFFFFFu;
     acc = (out & 3u) ? (slab_ld(c.text_w + static_cast<size_t>(out >> 2) * 32, c.pol) & ((1u << ((out & 3u) * 8u)) - 1u)) : 0u;
     put_ws();
     slab_st(c.text_w + static_cast<size_t>(out >> 2) * 32, acc, c.pol);
@@ -405,8 +436,14 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
 // back-pointer log: two coalesced backward scans (count, then write) around one warp-aggregated claim of output space.
 // entry t (t = 0..nlog-1) = plen (6 bits) << 24 | (previous char length - 1) << 22 | trie unit (kLaneUnk: UNK piece);
 // bit 31 (lane2 whole-word entries): the previous logged position is plen bytes back.
+// kWs1: the text and the units are those of lane_normalize<true> and trie_node4 (ids from trie_id_ws); an UNK character
+// that is kWsByte falls back to the three byte pieces of E2 96 81.
+template <bool kWs1 = false>
 __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, const LaneCtx &c, uint32_t n, uint32_t nlog,
                                             uint32_t lane, bool have, bool defer, uint32_t sent, bool bf) {
+  auto text_byte = [&](uint32_t k) -> uint32_t {
+    return (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+  };
   // ---------------- K4: coalesced backward scans of the log ----------------
   // entry t (t = 0..nlog-1) belongs to the (t+1)-th character boundary p_t; the character
   // before p_t has (entry>>22 & 3) + 1 bytes, so positions are recovered going backwards.
@@ -430,7 +467,7 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
           if (pos_b == want) {
             const uint32_t plen = (e >> 24) & 63u;
             const bool isunk = (e & 0x3FFFFFu) == kLaneUnk;
-            if (bf) count += isunk ? plen : 1u;
+            if (bf) count += !isunk ? 1u : (kWs1 && plen == 1u && text_byte(want - 1u) == kWsByte) ? 3u : plen;
             else count += !(isunk && prev_unk);
             prev_unk = isunk;
             want -= plen;
@@ -484,15 +521,20 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
           if (isunk) {
             if (bf) {
               for (uint32_t i = 0; i < plen; ++i) {
-                const uint32_t kk = want - 1 - i;
-                const uint32_t ch = (slab_ld(c.text_w + static_cast<size_t>(kk >> 2) * 32, c.pol) >> ((kk & 3u) * 8u)) & 0xFFu;
-                __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + ch));
+                const uint32_t ch = text_byte(want - 1 - i);
+                if (kWs1 && ch == kWsByte) {  // U+2581 = E2 96 81, written from the end
+                  __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + 0x81));
+                  __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + 0x96));
+                  __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + 0xE2));
+                } else {
+                  __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + ch));
+                }
               }
             } else if (!prev_unk) {
               __stcs(B.tmp_ids + pos + (--w), M.unk_id);
             }
           } else {
-            __stcs(B.tmp_ids + pos + (--w), __ldg(M.trie_id + idx));  // streaming store
+            __stcs(B.tmp_ids + pos + (--w), __ldg((kWs1 ? M.trie_id_ws : M.trie_id) + idx));  // streaming store
           }
           prev_unk = isunk;
           want -= plen;
@@ -510,6 +552,8 @@ __host__ __device__ inline uint32_t lane_ring_bytes(uint32_t R) { return R * 32u
 
 constexpr uint32_t kLogWordStep = 1u << 31;  // log entry: the previous logged position is plen bytes back (whole word)
 constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of a little-endian word
+// OneCharLen in the kWsByte spelling: U+2581 is one byte
+__device__ __forceinline__ uint32_t one_char_len_ws1(uint32_t lead) { return lead == kWsByte ? 1u : one_char_len(lead); }
 
 // Whole-word shortcut (kFlagFastWords; engine.cu upload_word_safe has the proof): when no piece contains U+2581
 // past its first byte, every segmentation has a token boundary in front of every U+2581, so the Viterbi problem of
@@ -519,6 +563,8 @@ constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of
 // the reference necessarily ends the word with P alone.  The walk from b reaches e on P's node, P has just been
 // relaxed into e exactly as the reference relaxes it (first candidate of e), and the starts inside the word are
 // skipped: 73 % of the words of the English corpus, half of all character starts.
+// The kernel works in the kWsByte spelling throughout (lane_normalize<true>, trie_node4, lane_finish<true>): a word
+// starts with one transition on U+2581 instead of three.
 __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KModel M, const KBatch B, uint8_t *slabs,
                                                                        uint32_t cap, uint32_t R) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -572,7 +618,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       const unsigned long long len64 = B.offsets[sent + 1] - off;
       if (len64 > 4ull * cap || len64 > 0xFFF0ull || off < B.off_lo || off + len64 > B.off_hi) defer = true;
       else {
-        n = lane_normalize(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
+        n = lane_normalize<true>(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
         if (n == 0xFFFFFFFFu || n >= 0xFFF0u) { defer = true; n = 0; }  // (positions are 16-bit ring tags)
       }
       if (defer) {
@@ -589,7 +635,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     // from the walk position k (low byte first).  ss = ring slot of s, times 32.
     uint32_t s = 0, ss = 0, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0;
     bool has_single = false, done = n == 0;
-    bool wstart = true;  // s is the first character of a word (text start or U+2581)
+    bool wstart = true;  // s is the first character of a word (text start or kWsByte)
     float base = 0.f;
     bool base_regular = regular;  // base == 0
     uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
@@ -608,7 +654,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       for (uint32_t r = 0; r < R; ++r) rp[r * 32] = 0xFFFFu;  // no slot belongs to a position of this sentence
       c.rs[0] = 0.f;
       w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
-      mblen = one_char_len(w0 & 0xFFu);
+      mblen = one_char_len_ws1(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
     }
@@ -687,20 +733,10 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
           if (fastwords && wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal) {
             // the walk covered [s, k) and ended on a NORMAL piece: is k the end of the word, early enough to be safe?
             bool wend = k >= n;
-            if (!wend && k + 3u <= n) {
-              const uint32_t o = k - ((s >> 2) << 2);
-              uint32_t b3;
-              if (o <= 13u) {
-                const uint32_t wi = o >> 2;
-                const uint32_t lo = wi == 0u ? w0 : (wi == 1u ? w1 : (wi == 2u ? w2 : w3));
-                const uint32_t hi = wi == 0u ? w1 : (wi == 1u ? w2 : (wi == 2u ? w3 : 0u));
-                b3 = __funnelshift_r(lo, hi, (o & 3u) * 8u) & 0xFFFFFFu;
-              } else {
-                b3 = 0;
-                for (uint32_t i = 0; i < 3u; ++i)
-                  b3 |= ((slab_ld(c.text_w + static_cast<size_t>((k + i) >> 2) * 32, c.pol) >> (((k + i) & 3u) * 8u)) & 0xFFu) << (8u * i);
-              }
-              wend = b3 == kWsWord;
+            if (!wend) {
+              const uint32_t wi = (k >> 2) - (s >> 2);  // word of the window that holds byte k
+              const uint32_t wd = wi == 0u ? w0 : (wi == 1u ? w1 : (wi == 2u ? w2 : (wi == 3u ? w3 : slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol))));
+              wend = ((wd >> ((k & 3u) * 8u)) & 0xFFu) == kWsByte;
             }
             fast = wend && k <= lsafe;
           }
@@ -750,8 +786,8 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
               w0 = slab_ld(tw + 0, c.pol); w1 = slab_ld(tw + 32, c.pol); w2 = slab_ld(tw + 64, c.pol); w3 = slab_ld(tw + 96, c.pol);
             }
             cur = window_low();
-            wstart = (static_cast<uint32_t>(cur) & 0xFFFFFFu) == kWsWord;
-            mblen = one_char_len(static_cast<uint32_t>(cur) & 0xFFu);
+            wstart = (static_cast<uint32_t>(cur) & 0xFFu) == kWsByte;
+            mblen = one_char_len_ws1(static_cast<uint32_t>(cur) & 0xFFu);
             if (mblen > n - s) mblen = n - s;
             k = s;
             l = root;
@@ -775,7 +811,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       }
     }
     const uint32_t t_g2 = tst ? static_cast<uint32_t>(clock64()) : 0u;
-    lane_finish(M, B, c, n, nlog, lane, have, defer, sent, bf);  // K4
+    lane_finish<true>(M, B, c, n, nlog, lane, have, defer, sent, bf);  // K4
     const uint32_t t_g3 = tst ? static_cast<uint32_t>(clock64()) : 0u;
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();
