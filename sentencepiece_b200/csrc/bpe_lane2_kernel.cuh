@@ -236,59 +236,35 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  LaneCtx c;
-  c.pol = slab_policy();
+  const LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  uint32_t *const text_all = c.text_w - lane;  // the warp's slab without the lane offset (phase B reads other lanes' columns)
+  uint32_t *const log_all = c.log - lane;
   uint32_t *sym, *pn, *list;
   float *ps;
-  uint32_t *text_all, *log_all;  // the warp's slab without the lane offset (phase B reads other lanes' columns)
   {
     uint8_t *a = arrays + static_cast<size_t>(warp_in_cta) * kBpeLane2WarpBytes;
     sym = reinterpret_cast<uint32_t *>(a) + lane;                             // node(22) | byte_len << 22
     pn = reinterpret_cast<uint32_t *>(a + kBpeWordSyms * 32 * 4) + lane;      // pair node(22) | offset_in_word << 22
     ps = reinterpret_cast<float *>(a + kBpeWordSyms * 32 * 8) + lane;         // pair score
     list = reinterpret_cast<uint32_t *>(a + kBpeSymArrayBytes);               // [kBpeListCap][2]
-    uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
-    text_all = reinterpret_cast<uint32_t *>(slab);
-    log_all = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32;
-    c.text_w = text_all + lane;
-    c.log = log_all + lane;
     long_scratch += static_cast<size_t>(warp_global) * bpe_long_bytes(cap);
-    c.rs = nullptr;
-    c.rb = nullptr;
-    c.s_lead = s_tab;
-    c.s_pair = s_tab + 8;
-    c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
-    c.s_plain = s_tab + 8 + 1024 + 128;
-    c.s_plainsp = c.s_plain + 4;
   }
   const uint32_t *tlink = M.trie_link;
   const uint32_t root = __ldg(&tlink[0]);
   const bool bf = M.flags & kFlagByteFallback;
 
-  for (;;) {
-    uint32_t first = 0;
-    if (lane == 0) first = atomicAdd(B.work_counter, 32u);
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
-    if (first >= B.n) break;
-    const bool tst = B.kstats != nullptr;  // trace / kstats mode: phase clocks (lane 0)
-    const uint32_t t_g0 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+  uint32_t first = 0;
+  while (lane_claim_group(B, lane, &first)) {
+    LanePhaseClock clk(B);
     lane_wait_input(B, first, lane);
     const bool have = first + lane < B.n;
     const uint32_t sent = have && B.order ? B.order[first + lane] : first + lane;
     // ---------------- K1 ----------------
     uint32_t n = 0;
     bool defer = false;
-    if (have) {
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      if (len64 > 4ull * cap || off < B.off_lo || off + len64 > B.off_hi) defer = true;
-      else {
-        n = lane_normalize(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
-        if (n == 0xFFFFFFFFu) { defer = true; n = 0; }
-      }
-    }
+    if (have) defer = !lane_k1(M, B, c, sent, cap, &n);  // recorded after phase B
     __syncwarp();  // the text of every lane is visible to the whole warp (phase B)
-    const uint32_t t_g1 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
 
     // ---------------- phase B: one listed word per lane ----------------
     uint32_t count = 0;  // words in the list (warp-uniform)
@@ -453,13 +429,10 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
     }
     if (count) drain();
     if (have && defer) {
-      const uint32_t slot = atomicAdd(B.status, 1u);
-      B.deferred[2 * slot] = sent;
-      B.deferred[2 * slot + 1] = 0;
-      B.sent_count[sent] = 0;  // until a later pass encodes it
+      lane_defer(B, sent);
       nlog = 0;
     }
-    const uint32_t t_g2 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     // ---------------- K4: id path of PopulateSentencePieceText over the symbol log ----------------
     const uint32_t unk = static_cast<uint32_t>(M.unk_id);
     const uint32_t max_log = __reduce_max_sync(0xFFFFFFFFu, nlog);
@@ -478,25 +451,8 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
         }
       }
     }
-    uint32_t incl = cnt;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-      if (lane >= static_cast<uint32_t>(d)) incl += t;
-    }
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    unsigned long long pos = 0;
-    if (lane == 0 && total) {
-      pos = atomicAdd(B.cursor, static_cast<unsigned long long>(total));
-      if (pos + total > B.tmp_cap) atomicOr(B.status + 2, 1u);
-    }
-    pos = __shfl_sync(0xFFFFFFFFu, pos, 0);
-    const bool room = pos + total <= B.tmp_cap;
-    pos += incl - cnt;
-    if (have && !defer) {
-      B.sent_start[sent] = pos;
-      B.sent_count[sent] = room ? cnt : 0u;
-    }
+    bool room;
+    const unsigned long long pos = lane_claim_output(B, lane, cnt, have, defer, sent, &room);
     if (room) {
       bool prev_unk = false;
       uint32_t w = 0, off = 0;
@@ -508,11 +464,8 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
             const bool isunk = (e & 0xFFFFFFu) == unk;
             if (isunk) {
               if (bf) {
-                for (uint32_t i = 0; i < plen; ++i) {
-                  const uint32_t kk = off + i;
-                  const uint32_t ch = (c.text_w[static_cast<size_t>(kk >> 2) * 32] >> ((kk & 3u) * 8u)) & 0xFFu;
-                  __stcs(B.tmp_ids + pos + (w++), __ldg(M.byte_to_id + ch));
-                }
+                for (uint32_t i = 0; i < plen; ++i)
+                  __stcs(B.tmp_ids + pos + (w++), __ldg(M.byte_to_id + lane_text_byte_plain(c, off + i)));
               } else if (!prev_unk) {
                 __stcs(B.tmp_ids + pos + (w++), M.unk_id);
               }
@@ -526,14 +479,10 @@ __global__ void __launch_bounds__(704, 1) encode_bpe_lane2_kernel(const KModel M
       }
     }
     slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
-    const uint32_t t_g3 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();
-    if (tst && lane == 0) {
-      typedef unsigned long long ull;
-      atomicAdd(B.kstats + 4, ull(static_cast<uint32_t>(clock64()) - t_g0)); atomicAdd(B.kstats + 5, ull(t_g1 - t_g0));
-      atomicAdd(B.kstats + 6, ull(t_g2 - t_g1)); atomicAdd(B.kstats + 7, ull(t_g3 - t_g2));
-    }
+    clk.flush(lane);
   }
 }
 

@@ -232,6 +232,7 @@ struct spm_engine {
     int version = 1;       // unigram: 2 = encode_unigram_lane_kernel (whole-word shortcut), 1 = the plain instantiation
     int threads = 0;
     uint32_t R = 0, smem = 0;
+    uint32_t warp_bytes = 0;  // shared memory per warp: the unigram ring or the BPE symbol arrays and word list
   };
   // unigram: which instantiation takes the next batch -- the whole-word shortcut pays on text made of space-separated
   // words and only costs on text without them (CJK, mixed script).  Decided per call from a sample of the batch's bytes
@@ -254,7 +255,8 @@ struct spm_engine {
       if (warps < 4) return g;
       g.ok = true;
       g.threads = warps * 32;
-      g.smem = static_cast<uint32_t>(kLaneTableBytes + static_cast<size_t>(warps) * kBpeLane2WarpBytes);
+      g.warp_bytes = kBpeLane2WarpBytes;
+      g.smem = static_cast<uint32_t>(kLaneTableBytes + static_cast<size_t>(warps) * g.warp_bytes);
       return g;
     }
     if (trie.max_key_len > 62) return g;
@@ -263,15 +265,28 @@ struct spm_engine {
     // over one character, up to 4 bytes -- the kernels step the ring index by an edge length with a single wrap
     const uint32_t longest = g.version == 2 ? trie_ws.max_key_len : trie.max_key_len;
     g.R = std::max<uint32_t>(longest, 4) + 2;
-    const size_t ring = g.version == 2 ? lane_ring_bytes(g.R) : static_cast<size_t>(g.R) * 32 * 8;
+    const uint32_t ring = g.version == 2 ? lane_ring_bytes(g.R) : lane_plain_ring_bytes(g.R);
     const int warps = static_cast<int>(std::min<size_t>(threads / 32, avail / ring));
     if (warps < 4) return g;
     g.ok = true;
     g.threads = warps * 32;
+    g.warp_bytes = ring;
     g.smem = static_cast<uint32_t>(kLaneTableBytes + static_cast<size_t>(warps) * ring);
     return g;
   }
   bool uses_lane_kernel() const { return lane_geometry().ok; }
+  // Per-warp slabs (normalized text + back-pointer log) of `warps` resident warps of a lane kernel.
+  cudaError_t ensure_lane_slabs(size_t warps, uint32_t cap) { return d_lane_slabs.ensure(warps * lane_slab_bytes(cap) + 256); }
+  // Launches the lane encode kernel that takes an ids-only batch under `lg` (lg.ok): BPE lane2, or the unigram
+  // whole-word (version 2) or plain instantiation.  The slabs (and the BPE long-word scratch) must be in place.
+  void launch_lane_encode(const LaneGeom &lg, int grid, const KModel &M, const KBatch &B, cudaStream_t st) {
+    if (model.model_type == SPM_BPE)
+      encode_bpe_lane2_kernel<<<grid, lg.threads, lg.smem, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
+    else if (lg.version == 2)
+      encode_unigram_lane_kernel<<<grid, lg.threads, lg.smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
+    else
+      encode_unigram_lane_plain_kernel<<<grid, lg.threads, lg.smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
+  }
   // Decode (K7): per-id decoded strings, built on first use
   DevBuf<uint32_t> d_dec_off, d_dec_info;
   DevBuf<uint8_t> d_dec_bytes, d_dec_tmp, d_dec_text;
@@ -873,16 +888,15 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
   const uint32_t K = km.match_slots;
   // fast path: sentence per lane (lane kernels); else the general kernels, a warp per sentence
   const LaneGeom lg = spans ? LaneGeom{} : lane_geometry();
-  const bool lane_path = !bpe && lg.ok;
-  const bool bpe_lane_path = bpe && lg.ok;
+  const bool lane_path = lg.ok;
   LaunchGeom geom = plan_geometry(*this, bpe ? bpe_tile_bytes(ncap, spans) : tile_bytes_for(ncap, K, spans), tile_threads / 32);
-  if (lane_path || bpe_lane_path) {
+  if (lane_path) {
     geom.tiles = lg.threads / 32;
-    geom.tile_bytes = bpe ? kBpeLane2WarpBytes : (lg.version == 2 ? lane_ring_bytes(lg.R) : lg.R * 32 * 8);
+    geom.tile_bytes = lg.warp_bytes;
     geom.hot_link = geom.hot_val = 0;  // the lane kernels read the trie through L1: rings / word arrays get the shared memory
     geom.smem_bytes = lg.smem;
     const size_t warps_total = static_cast<size_t>(sm_count) * ctas_per_sm * geom.tiles;
-    CUDA_TRY(d_lane_slabs.ensure(warps_total * lane_slab_bytes(lane_cap) + 256));
+    CUDA_TRY(ensure_lane_slabs(warps_total, lane_cap));
     if (bpe) CUDA_TRY(d_bpe_long.ensure(warps_total * bpe_long_bytes(lane_cap)));
   }
   if (geom.smem_bytes > smem_optin) { set_error("shared-memory geometry does not fit; lower smem_norm_cap"); return SPM_ERR_ARG; }
@@ -946,22 +960,16 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       CUDA_TRY(cudaMemsetAsync(d_kstats.p, 0, 16 * sizeof(unsigned long long), st));
       B.kstats = d_kstats.p;
     }
-    if (lane_path || bpe_lane_path) {
+    if (lane_path) {
       const int rc = build_order(d_offs, n, st, &B.order, cur_ready ? (1u << cur_piece_shift) : 0u);
       if (rc) return rc;
       B.ready = cur_ready;
       B.ready_base = cur_ready_base;
       B.piece_shift = cur_piece_shift;
-    }
-    if (bpe_lane_path) {
-      encode_bpe_lane2_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
+      launch_lane_encode(lg, grid, M, B, st);
     } else if (bpe) {
       if (spans) encode_bpe_kernel<true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
       else encode_bpe_kernel<false><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
-    } else if (lane_path && lg.version == 2) {
-      encode_unigram_lane_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
-    } else if (lane_path) {
-      encode_unigram_lane_plain_kernel<<<grid, lg.threads, geom.smem_bytes, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
     } else if (spans) {
       encode_unigram_kernel<true><<<grid, tile_threads, geom.smem_bytes, st>>>(M, B);
     } else {
@@ -988,7 +996,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     }
     uint32_t n_def = h_ctrl32.p[0];
     const uint32_t *def_list = d_deferred.p;
-    if (n_def && (lane_path || bpe_lane_path)) {
+    if (n_def && lane_path) {
       // ---- second chance: the sentences a lane kernel could not take (long words, long
       //      sentences) go through the shared-memory warp kernels before the HBM-scratch path ----
       last_deferred = n_def;
@@ -1417,11 +1425,10 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   // ---- launch geometry of the lane kernels (as in run_device) ----
   const LaneGeom lg = lane_geometry();
   if (!lg.ok) { set_error("fused path: the model is outside the lane kernels"); return SPM_ERR_ARG; }
-  const int lane_threads = lg.threads;
-  const uint32_t smem = lg.smem;
   const int grid = sm_count * ctas_per_sm;
-  CUDA_TRY(d_lane_slabs.ensure(static_cast<size_t>(grid) * (lane_threads / 32) * lane_slab_bytes(lane_cap) + 256));
-  if (bpe) CUDA_TRY(d_bpe_long.ensure(static_cast<size_t>(grid) * (lane_threads / 32) * bpe_long_bytes(lane_cap)));
+  const size_t warps_total = static_cast<size_t>(grid) * (lg.threads / 32);
+  CUDA_TRY(ensure_lane_slabs(warps_total, lane_cap));
+  if (bpe) CUDA_TRY(d_bpe_long.ensure(warps_total * bpe_long_bytes(lane_cap)));
   // ---- queue the whole input ----
   CUDA_TRY(cudaMemsetAsync(d_ready.p, 0, sizeof(uint32_t), s_h2d));
   CUDA_TRY(cudaMemcpyAsync(s_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s_h2d));
@@ -1484,9 +1491,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
     if (rc) return rc;
     if (!B.order) { set_error("fused path needs the segment order"); return SPM_ERR_ARG; }
   }
-  if (bpe) encode_bpe_lane2_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, d_bpe_long.p);
-  else if (lg.version == 2) encode_unigram_lane_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
-  else encode_unigram_lane_plain_kernel<<<grid, lane_threads, smem, st>>>(M, B, d_lane_slabs.p, lane_cap, lg.R);
+  launch_lane_encode(lg, grid, M, B, st);
   CUDA_TRY(cudaGetLastError());
   ++last_launches;
   CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -1516,12 +1521,12 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(cudaStreamSynchronize(st));
   feeder.join();
   if (trace) fprintf(stderr, "[trace] fused kernel done at %.3f ms; warp-cycles: input wait %.1f M, compaction %.1f M (look-back %.1f M), "
-                     "%llu groups on %d warps\n", now_ms(), h_ctrl64.p[4] * 1e-6, h_ctrl64.p[5] * 1e-6, h_ctrl64.p[6] * 1e-6,
-                     static_cast<unsigned long long>(h_ctrl64.p[7]), grid * (lane_threads / 32));
+                     "%llu groups on %zu warps\n", now_ms(), h_ctrl64.p[4] * 1e-6, h_ctrl64.p[5] * 1e-6, h_ctrl64.p[6] * 1e-6,
+                     static_cast<unsigned long long>(h_ctrl64.p[7]), warps_total);
   if (trace) {
     float km = 0.f;
     cudaEventElapsedTime(&km, ev[0], ev[1]);
-    const double w = 1e-6 / (grid * (lane_threads / 32));  // M cycles per warp
+    const double w = 1e-6 / warps_total;  // M cycles per warp
     fprintf(stderr, "[trace] kernel %.3f ms on the device; M cycles per warp (lane 0): group loop %.2f = K1 + input wait %.2f, K2 %.2f, "
                     "K4 %.2f, drain %.2f\n", km, h_ctrl64.p[8] * w, h_ctrl64.p[9] * w, h_ctrl64.p[10] * w, h_ctrl64.p[11] * w,
             (h_ctrl64.p[8] - h_ctrl64.p[9] - h_ctrl64.p[10] - h_ctrl64.p[11]) * w);
@@ -1809,7 +1814,7 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
   int ctas = static_cast<int>(std::min<size_t>(sm_count, groups));
   int warps_per_cta = static_cast<int>(std::min<size_t>(32, (groups + ctas - 1) / ctas));
   size_t warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-  CUDA_TRY(d_lane_slabs.ensure(warps_total * lane_slab_bytes(lane_cap) + 256));
+  CUDA_TRY(ensure_lane_slabs(warps_total, lane_cap));
   CUDA_TRY(d_nb_scratch.ensure(warps_total * 32 * nbest_lane_bytes(G) + 256));
   bool grown = false;
   const size_t nc = n * static_cast<size_t>(nbest);
@@ -1863,7 +1868,7 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
       warps_per_cta = G.hyp_cap > (1u << 17) ? 1 : 2;
       ctas = sm_count;
       warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-      CUDA_TRY(d_lane_slabs.ensure(warps_total * lane_slab_bytes(G.cap) + 256));
+      CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
       CUDA_TRY(d_nb_scratch.ensure(warps_total * 32 * nbest_lane_bytes(G) + 256));
       continue;
     }
@@ -1917,7 +1922,7 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
     const size_t groups = (m + 31) / 32;
     int ctas = static_cast<int>(std::min<size_t>(sm_count, (groups + warps_per_cta - 1) / warps_per_cta));
     size_t warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-    CUDA_TRY(d_lane_slabs.ensure(warps_total * lane_slab_bytes(G.cap) + 256));
+    CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
     CUDA_TRY(d_lat_scratch.ensure(warps_total * 32 * lattice_lane_bytes(G) + 256));
     CUDA_TRY(d_lat_node_start.ensure(m));
     CUDA_TRY(d_lat_pos_start.ensure(m));
@@ -1968,7 +1973,7 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
         warps_per_cta = 2;
         ctas = static_cast<int>(std::min<size_t>(sm_count, (groups + warps_per_cta - 1) / warps_per_cta));
         warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-        CUDA_TRY(d_lane_slabs.ensure(warps_total * lane_slab_bytes(G.cap) + 256));
+        CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
         CUDA_TRY(d_lat_scratch.ensure(warps_total * 32 * lattice_lane_bytes(G) + 256));
         --attempt;
         continue;

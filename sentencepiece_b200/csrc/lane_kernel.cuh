@@ -156,6 +156,69 @@ __device__ __forceinline__ void slab_discard(const LaneCtx &c, uint32_t lane, ui
   __syncwarp();
 }
 
+// The lane's view of its warp's slab and of the normalizer's tables (s_tab, filled by fill_lane_tables).  The rings
+// (rs / rb) belong to the kernels that have them and are left null here.
+__device__ __forceinline__ LaneCtx lane_ctx(const uint32_t *s_tab, uint8_t *slabs, uint32_t cap, uint32_t warp_global,
+                                            uint32_t lane) {
+  LaneCtx c;
+  c.pol = slab_policy();
+  uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
+  c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
+  c.log = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32 + lane;
+  c.rs = nullptr;
+  c.rb = nullptr;
+  c.s_lead = s_tab;
+  c.s_pair = s_tab + 8;
+  c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
+  c.s_plain = s_tab + 8 + 1024 + 128;
+  c.s_plainsp = c.s_plain + 4;
+  return c;
+}
+
+// Claims the warp's next group of 32 sentences, [*first, *first + 32) of the processing order; false once the batch
+// is done.
+__device__ __forceinline__ bool lane_claim_group(const KBatch &B, uint32_t lane, uint32_t *first) {
+  uint32_t f = 0;
+  if (lane == 0) f = atomicAdd(B.work_counter, 32u);
+  *first = __shfl_sync(0xFFFFFFFFu, f, 0);
+  return *first < B.n;
+}
+
+// Byte k of the lane's normalized text: L2-hinted slab load (the encode kernels) or plain load (n-best, lattice, and
+// the BPE kernel's byte fallback).
+__device__ __forceinline__ uint32_t lane_text_byte(const LaneCtx &c, uint32_t k) {
+  return (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+}
+__device__ __forceinline__ uint32_t lane_text_byte_plain(const LaneCtx &c, uint32_t k) {
+  return (c.text_w[static_cast<size_t>(k >> 2) * 32] >> ((k & 3u) * 8u)) & 0xFFu;
+}
+
+// A sentence the lane kernel leaves to a later pass (the general warp-per-sentence kernels).
+__device__ __forceinline__ void lane_defer(const KBatch &B, uint32_t sent) {
+  const uint32_t slot = atomicAdd(B.status, 1u);
+  B.deferred[2 * slot] = sent;
+  B.deferred[2 * slot + 1] = 0;
+  B.sent_count[sent] = 0;  // until a later pass encodes it
+}
+
+// Phase clocks of the encode lane kernels when B.kstats is set, summed by lane 0 of each warp: kstats[4] the whole
+// group, [5] K1, [6] K2 (BPE: phases A and B), [7] K4.  Construct at the top of a group, mark() after K1, K2 and K4,
+// flush() at the end of the group.
+struct LanePhaseClock {
+  unsigned long long *ks;
+  uint32_t t[4];
+  uint32_t i;
+  __device__ __forceinline__ explicit LanePhaseClock(const KBatch &B) : ks(B.kstats), i(0) { mark(); }
+  __device__ __forceinline__ void mark() { t[i++] = ks ? static_cast<uint32_t>(clock64()) : 0u; }
+  __device__ __forceinline__ void flush(uint32_t lane) const {
+    if (ks && lane == 0) {
+      typedef unsigned long long ull;
+      atomicAdd(ks + 4, ull(static_cast<uint32_t>(clock64()) - t[0])); atomicAdd(ks + 5, ull(t[1] - t[0]));
+      atomicAdd(ks + 6, ull(t[2] - t[1])); atomicAdd(ks + 7, ull(t[3] - t[2]));
+    }
+  }
+};
+
 // Sequential byte stream over a lane's input: 16-byte aligned chunks (next chunk prefetched)
 // feed a 64-bit shift register that always exposes the next >= 4 bytes.  The aligned chunks
 // over-read into the neighbouring sentences by up to 15 bytes; a streamed host batch (engine.cu)
@@ -412,15 +475,14 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
   // flush the partial word, then strip trailing spaces on the escaped output (:166-176)
   slab_st(c.text_w + static_cast<size_t>(out >> 2) * 32, acc, c.pol);
   if (rm) {
-    auto byte_at = [&](uint32_t k) -> uint32_t {
-      return (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
-    };
     if (esc && kWs1) {
-      while (out >= 1 && byte_at(out - 1) == kWsByte) { out -= 1; saved -= 2; }
+      while (out >= 1 && lane_text_byte(c, out - 1) == kWsByte) { out -= 1; saved -= 2; }
     } else if (esc) {
-      while (out >= 3 && byte_at(out - 3) == 0xE2 && byte_at(out - 2) == 0x96 && byte_at(out - 1) == 0x81) out -= 3;
+      while (out >= 3 && lane_text_byte(c, out - 3) == 0xE2 && lane_text_byte(c, out - 2) == 0x96 &&
+             lane_text_byte(c, out - 1) == 0x81)
+        out -= 3;
     } else {
-      while (out >= 1 && byte_at(out - 1) == ' ') out -= 1;
+      while (out >= 1 && lane_text_byte(c, out - 1) == ' ') out -= 1;
     }
   }
   if (suffix && addp) {  // :179
@@ -432,6 +494,78 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
   return out;
 }
 
+// K1 of a lane kernel: normalizes sentence `sent` into the lane's slab, *n = the normalized length.  Returns false
+// (*n = 0) when the kernel does not take the sentence: more than 4 * cap input bytes or cap normalized bytes, input
+// outside the batch's valid range [B.off_lo, B.off_hi], or beyond `lim` (input lengths above it, normalized lengths
+// from it up; for a kernel whose positions have fewer than 32 bits).
+template <bool kWs1 = false>
+__device__ __forceinline__ bool lane_k1(const KModel &M, const KBatch &B, const LaneCtx &c, uint32_t sent, uint32_t cap,
+                                        uint32_t *n, unsigned long long lim = ~0ull) {
+  const unsigned long long off = B.offsets[sent];
+  const unsigned long long len64 = B.offsets[sent + 1] - off;
+  *n = 0;
+  if (len64 > 4ull * cap || len64 > lim || off < B.off_lo || off + len64 > B.off_hi) return false;
+  *n = lane_normalize<kWs1>(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
+  if (*n == 0xFFFFFFFFu || *n >= lim) { *n = 0; return false; }
+  return true;
+}
+
+// One claim of output space per warp (a scan of the lanes' id counts, one atomicAdd on B.cursor).  Returns the lane's
+// first slot in B.tmp_ids and records the sentence's start and count.  *room is false on every lane when the warp's
+// ids do not fit in B.tmp_cap: status[2] then tells the host to rerun the batch with a larger buffer.
+__device__ __forceinline__ unsigned long long lane_claim_output(const KBatch &B, uint32_t lane, uint32_t count, bool have,
+                                                                bool defer, uint32_t sent, bool *room) {
+  uint32_t incl = count;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+    if (lane >= static_cast<uint32_t>(d)) incl += t;
+  }
+  const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+  unsigned long long pos = 0;
+  if (lane == 0 && total) {
+    pos = atomicAdd(B.cursor, static_cast<unsigned long long>(total));
+    if (pos + total > B.tmp_cap) atomicOr(B.status + 2, 1u);
+  }
+  pos = __shfl_sync(0xFFFFFFFFu, pos, 0);
+  *room = pos + total <= B.tmp_cap;
+  pos += incl - count;
+  if (have && !defer) {
+    B.sent_start[sent] = pos;
+    B.sent_count[sent] = *room ? count : 0u;
+  }
+  return pos;
+}
+
+// Model::PopulateNodes (unigram_model.cc:547-596) from begin character bp, whose byte offset is surf[bp] (surf[L] = n):
+// walks the trie (trie_node2, root link word `root`) along the text and calls piece(length, v, score) for every
+// NORMAL or USER_DEFINED piece that begins there, shortest first -- length in characters (get_chars_length, :548-552),
+// trie unit, score (USER_DEFINED: float(double(length * max_score) - 0.1)).  piece returns false when the lattice is
+// full, which ends the walk.  Returns whether a one-character piece was found (if not, the caller adds the UNK node).
+template <typename F>
+__device__ __forceinline__ bool lane_populate_from(const KModel &M, const LaneCtx &c, uint32_t root, const uint16_t *surf,
+                                                   uint32_t bp, uint32_t n, F &&piece) {
+  bool has_single = false;
+  uint32_t l = root;
+  uint32_t clen = 0;  // characters completed so far
+  for (uint32_t kpos = surf[bp]; kpos < n; ++kpos) {
+    const uint32_t ch = lane_text_byte_plain(c, kpos);
+    const uint32_t v = (l >> kLinkBaseShift) ^ ch;
+    l = __ldg(&M.trie_node2[v]).x;
+    if ((l & kLinkLabelMask) != ch) break;
+    if (kpos + 1 == surf[bp + clen + 1]) ++clen;
+    const uint32_t kind = (l >> kLinkKindShift) & 3u;
+    if (kind == kKindNone || kind == kKindUnused) continue;
+    const uint32_t length = (kpos + 1 == surf[bp + clen]) ? clen : clen + 1;
+    const float sc = kind == kKindUserDefined
+                         ? static_cast<float>(static_cast<double>(__fmul_rn(static_cast<float>(length), M.max_score)) - 0.1)
+                         : __uint_as_float(__ldg(M.trie_val + v));
+    if (!piece(length, v, sc)) break;
+    has_single |= length == 1;
+  }
+  return has_single;
+}
+
 // K4: back-trace + id path of PopulateSentencePieceText (sentencepiece_processor.cc:547-636) over a lane's
 // back-pointer log: two coalesced backward scans (count, then write) around one warp-aggregated claim of output space.
 // entry t (t = 0..nlog-1) = plen (6 bits) << 24 | (previous char length - 1) << 22 | trie unit (kLaneUnk: UNK piece);
@@ -441,9 +575,6 @@ __device__ __forceinline__ uint32_t lane_normalize(const KModel &M, const uint8_
 template <bool kWs1 = false>
 __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, const LaneCtx &c, uint32_t n, uint32_t nlog,
                                             uint32_t lane, bool have, bool defer, uint32_t sent, bool bf) {
-  auto text_byte = [&](uint32_t k) -> uint32_t {
-    return (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
-  };
   // ---------------- K4: coalesced backward scans of the log ----------------
   // entry t (t = 0..nlog-1) belongs to the (t+1)-th character boundary p_t; the character
   // before p_t has (entry>>22 & 3) + 1 bytes, so positions are recovered going backwards.
@@ -467,7 +598,7 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
           if (pos_b == want) {
             const uint32_t plen = (e >> 24) & 63u;
             const bool isunk = (e & 0x3FFFFFu) == kLaneUnk;
-            if (bf) count += !isunk ? 1u : (kWs1 && plen == 1u && text_byte(want - 1u) == kWsByte) ? 3u : plen;
+            if (bf) count += !isunk ? 1u : (kWs1 && plen == 1u && lane_text_byte(c, want - 1u) == kWsByte) ? 3u : plen;
             else count += !(isunk && prev_unk);
             prev_unk = isunk;
             want -= plen;
@@ -478,26 +609,8 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
     }
     if (n && want != 0) { atomicOr(B.status + 1, 1u); count = 0; }
   }
-  // one claim of output space per warp
-  uint32_t incl = count;
-#pragma unroll
-  for (int d = 1; d < 32; d <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, incl, d);
-    if (lane >= static_cast<uint32_t>(d)) incl += t;
-  }
-  const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-  unsigned long long pos = 0;
-  if (lane == 0 && total) {
-    pos = atomicAdd(B.cursor, static_cast<unsigned long long>(total));
-    if (pos + total > B.tmp_cap) atomicOr(B.status + 2, 1u);
-  }
-  pos = __shfl_sync(0xFFFFFFFFu, pos, 0);
-  const bool room = pos + total <= B.tmp_cap;
-  pos += incl - count;
-  if (have && !defer) {
-    B.sent_start[sent] = pos;
-    B.sent_count[sent] = room ? count : 0u;
-  }
+  bool room;
+  const unsigned long long pos = lane_claim_output(B, lane, count, have, defer, sent, &room);
   // second backward scan: write ids from the end
   if (room) {
     uint32_t pos_b = n, want = n, w = count;
@@ -521,7 +634,7 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
           if (isunk) {
             if (bf) {
               for (uint32_t i = 0; i < plen; ++i) {
-                const uint32_t ch = text_byte(want - 1 - i);
+                const uint32_t ch = lane_text_byte(c, want - 1 - i);
                 if (kWs1 && ch == kWsByte) {  // U+2581 = E2 96 81, written from the end
                   __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + 0x81));
                   __stcs(B.tmp_ids + pos + (--w), __ldg(M.byte_to_id + 0x96));
@@ -549,6 +662,8 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
 
 // shared memory per warp: ring of R slots, each {score f32, back-pointer u32, position tag u16} x 32 lanes
 __host__ __device__ inline uint32_t lane_ring_bytes(uint32_t R) { return R * 32u * (4u + 4u + 2u); }
+// the same for encode_unigram_lane_plain_kernel, whose slots have no position tag
+__host__ __device__ inline uint32_t lane_plain_ring_bytes(uint32_t R) { return R * 32u * (4u + 4u); }
 
 constexpr uint32_t kLogWordStep = 1u << 31;  // log entry: the previous logged position is plen bytes back (whole word)
 constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of a little-endian word
@@ -575,8 +690,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  LaneCtx c;
-  c.pol = slab_policy();
+  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
   uint16_t *rp;  // ring position tags: a slot belongs to position p iff rp == p (no clearing, skipped positions
                  // of whole words leave stale slots behind that simply fail the test)
   {
@@ -584,14 +698,6 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     c.rs = reinterpret_cast<float *>(ring) + lane;
     c.rb = reinterpret_cast<uint32_t *>(ring + R * 32 * 4) + lane;
     rp = reinterpret_cast<uint16_t *>(ring + R * 32 * 8) + lane;
-    uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
-    c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
-    c.log = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32 + lane;
-    c.s_lead = s_tab;
-    c.s_pair = s_tab + 8;
-    c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
-    c.s_plain = s_tab + 8 + 1024 + 128;
-    c.s_plainsp = c.s_plain + 4;
   }
   const uint4 *node4 = M.trie_node4;
   const uint32_t root = __ldg(&node4[0]).x;
@@ -600,13 +706,9 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
   const bool fastwords = M.flags & kFlagFastWords;
   const uint32_t r_wrap = R * 32;
 
-  for (;;) {
-    uint32_t first = 0;
-    if (lane == 0) first = atomicAdd(B.work_counter, 32u);
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
-    if (first >= B.n) break;
-    const bool tst = B.kstats != nullptr;  // trace / kstats mode: phase clocks (lane 0)
-    const uint32_t t_g0 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+  uint32_t first = 0;
+  while (lane_claim_group(B, lane, &first)) {
+    LanePhaseClock clk(B);
     lane_wait_input(B, first, lane);
     const bool have = first + lane < B.n;
     const uint32_t sent = have && B.order ? B.order[first + lane] : first + lane;
@@ -614,22 +716,11 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     uint32_t n = 0;
     bool defer = false;
     if (have) {
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      if (len64 > 4ull * cap || len64 > 0xFFF0ull || off < B.off_lo || off + len64 > B.off_hi) defer = true;
-      else {
-        n = lane_normalize<true>(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
-        if (n == 0xFFFFFFFFu || n >= 0xFFF0u) { defer = true; n = 0; }  // (positions are 16-bit ring tags)
-      }
-      if (defer) {
-        const uint32_t slot = atomicAdd(B.status, 1u);
-        B.deferred[2 * slot] = sent;
-        B.deferred[2 * slot + 1] = 0;
-        B.sent_count[sent] = 0;  // until a later pass encodes it
-      }
+      defer = !lane_k1<true>(M, B, c, sent, cap, &n, 0xFFF0u);  // (positions are 16-bit ring tags)
+      if (defer) lane_defer(B, sent);
     }
     __syncwarp();
-    const uint32_t t_g1 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     // ---------------- K2: flat state machine, one trie transition per trip ----------------
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
     // from the walk position k (low byte first).  ss = ring slot of s, times 32.
@@ -670,7 +761,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
           const uint32_t d = k - s;
           uint32_t ch;
           if (d >= 13u) {  // beyond the register window: long piece, rare
-            ch = (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+            ch = lane_text_byte(c, k);
           } else {
             if (d == 8u) cur = window_high();
             ch = static_cast<uint32_t>(cur) & 0xFFu;
@@ -721,7 +812,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
             if (k < n) {
               uint32_t nb;
               const uint32_t d2 = k - s;
-              if (d2 >= 13u) nb = (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+              if (d2 >= 13u) nb = lane_text_byte(c, k);
               else nb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
               end_walk = !((nd.y >> (nb & 31u)) & 1u);
             }
@@ -810,16 +901,12 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
         atomicAdd(B.kstats + 11, ull(st_fast)); atomicAdd(B.kstats + 12, ull(1)); atomicAdd(B.kstats + 13, ull(nb));
       }
     }
-    const uint32_t t_g2 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     lane_finish<true>(M, B, c, n, nlog, lane, have, defer, sent, bf);  // K4
-    const uint32_t t_g3 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();
-    if (tst && lane == 0) {
-      typedef unsigned long long ull;
-      atomicAdd(B.kstats + 4, ull(static_cast<uint32_t>(clock64()) - t_g0)); atomicAdd(B.kstats + 5, ull(t_g1 - t_g0));
-      atomicAdd(B.kstats + 6, ull(t_g2 - t_g1)); atomicAdd(B.kstats + 7, ull(t_g3 - t_g2));
-    }
+    clk.flush(lane);
   }
 }
 
@@ -827,7 +914,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
 // lookup on a match, cleared ring slots instead of position tags).  Text with few space-separated words -- CJK, the
 // byte-fallback / mixed-script configuration -- gains nothing from the shortcut and would only pay for its bookkeeping,
 // so the engine picks this instantiation for such batches (engine.cu,
-// `pick_fast_words`); ring geometry R * 32 * 8 bytes per warp.
+// `pick_fast_words`); ring geometry lane_plain_ring_bytes(R) per warp.
 __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(const KModel M, const KBatch B, uint8_t *slabs,
                                                                        uint32_t cap, uint32_t R) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -838,33 +925,20 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  LaneCtx c;
-  c.pol = slab_policy();
+  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
   {
-    uint8_t *ring = rings + static_cast<size_t>(warp_in_cta) * (R * 32 * 8);
+    uint8_t *ring = rings + static_cast<size_t>(warp_in_cta) * lane_plain_ring_bytes(R);
     c.rs = reinterpret_cast<float *>(ring) + lane;
     c.rb = reinterpret_cast<uint32_t *>(ring + R * 32 * 4) + lane;
-    uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
-    c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
-    c.log = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32 + lane;
-    c.s_lead = s_tab;
-    c.s_pair = s_tab + 8;
-    c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
-    c.s_plain = s_tab + 8 + 1024 + 128;
-    c.s_plainsp = c.s_plain + 4;
   }
   const uint2 *node2 = M.trie_node2;
   const uint32_t root = __ldg(&node2[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
   const bool regular = M.flags & kFlagRegularScores;
 
-  for (;;) {
-    uint32_t first = 0;
-    if (lane == 0) first = atomicAdd(B.work_counter, 32u);
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
-    if (first >= B.n) break;
-    const bool tst = B.kstats != nullptr;  // trace / kstats mode: phase clocks (lane 0)
-    const uint32_t t_g0 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+  uint32_t first = 0;
+  while (lane_claim_group(B, lane, &first)) {
+    LanePhaseClock clk(B);
     lane_wait_input(B, first, lane);
     const bool have = first + lane < B.n;
     const uint32_t sent = have && B.order ? B.order[first + lane] : first + lane;
@@ -872,22 +946,11 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
     uint32_t n = 0;
     bool defer = false;
     if (have) {
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      if (len64 > 4ull * cap || off < B.off_lo || off + len64 > B.off_hi) defer = true;
-      else {
-        n = lane_normalize(M, B.bytes + off, static_cast<uint32_t>(len64), c, cap);
-        if (n == 0xFFFFFFFFu) { defer = true; n = 0; }
-      }
-      if (defer) {
-        const uint32_t slot = atomicAdd(B.status, 1u);
-        B.deferred[2 * slot] = sent;
-        B.deferred[2 * slot + 1] = 0;
-        B.sent_count[sent] = 0;  // until a later pass encodes it
-      }
+      defer = !lane_k1(M, B, c, sent, cap, &n);
+      if (defer) lane_defer(B, sent);
     }
     __syncwarp();
-    const uint32_t t_g1 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     // ---------------- K2: flat state machine, one trie transition per trip ----------------
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
     // from the walk position k (low byte first).
@@ -922,7 +985,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
           const uint32_t d = k - s;
           uint32_t ch;
           if (d >= 13u) {  // beyond the register window: long piece, rare
-            ch = (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+            ch = lane_text_byte(c, k);
           } else {
             if (d == 8u) cur = window_high();
             ch = static_cast<uint32_t>(cur) & 0xFFu;
@@ -972,7 +1035,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
             if (k < n) {
               uint32_t nb;
               const uint32_t d2 = k - s;
-              if (d2 >= 13u) nb = (slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
+              if (d2 >= 13u) nb = lane_text_byte(c, k);
               else nb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
               end_walk = !((nd.y >> (nb & 31u)) & 1u);
             }
@@ -1017,16 +1080,12 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
         }
       }
     }
-    const uint32_t t_g2 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     lane_finish(M, B, c, n, nlog, lane, have, defer, sent, bf);  // K4
-    const uint32_t t_g3 = tst ? static_cast<uint32_t>(clock64()) : 0u;
+    clk.mark();
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();
-    if (tst && lane == 0) {
-      typedef unsigned long long ull;
-      atomicAdd(B.kstats + 4, ull(static_cast<uint32_t>(clock64()) - t_g0)); atomicAdd(B.kstats + 5, ull(t_g1 - t_g0));
-      atomicAdd(B.kstats + 6, ull(t_g2 - t_g1)); atomicAdd(B.kstats + 7, ull(t_g3 - t_g2));
-    }
+    clk.flush(lane);
   }
 }
 

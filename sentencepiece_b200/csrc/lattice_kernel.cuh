@@ -65,44 +65,21 @@ __global__ void __launch_bounds__(512, 1) lattice_lane_kernel(const KModel M, co
   __syncthreads();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  LaneCtx c;
-  c.pol = slab_policy();
-  {
-    uint8_t *slab = text_slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(G.cap);
-    c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
-    c.log = nullptr; c.rs = nullptr; c.rb = nullptr;
-    c.s_lead = s_tab; c.s_pair = s_tab + 8;
-    c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
-    c.s_plain = s_tab + 8 + 1024 + 128;
-    c.s_plainsp = c.s_plain + 4;
-  }
+  const LaneCtx c = lane_ctx(s_tab, text_slabs, G.cap, warp_global, lane);
   uint8_t *sp = scratch + (static_cast<size_t>(warp_global) * 32 + lane) * lattice_lane_bytes(G);
   uint4 *node = reinterpret_cast<uint4 *>(sp); sp += 16ull * G.node_cap;
   float *A = reinterpret_cast<float *>(sp); sp += 4ull * (G.cap + 4);
   float *H = reinterpret_cast<float *>(sp); sp += 4ull * (G.cap + 4);
   uint32_t *ecnt = reinterpret_cast<uint32_t *>(sp); sp += 4ull * (G.cap + 4);
   uint16_t *surf = reinterpret_cast<uint16_t *>(sp);
-  const uint2 *node2 = M.trie_node2;
-  const uint32_t root = __ldg(&node2[0]).x;
-  auto text_byte = [&](uint32_t k) -> uint32_t {
-    return (c.text_w[static_cast<size_t>(k >> 2) * 32] >> ((k & 3u) * 8u)) & 0xFFu;
-  };
+  const uint32_t root = __ldg(&M.trie_node2[0]).x;
 
-  for (;;) {
-    uint32_t first = 0;
-    if (lane == 0) first = atomicAdd(B.work_counter, 32u);
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
-    if (first >= B.n) break;
+  uint32_t first = 0;
+  while (lane_claim_group(B, lane, &first)) {
     if (first + lane < B.n) {
       const uint32_t sent = B.order ? B.order[first + lane] : first + lane;
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      uint32_t n = 0;
-      bool too_big = len64 > 4ull * G.cap;
-      if (!too_big) {
-        n = lane_normalize(M, B.bytes + off, static_cast<uint32_t>(len64), c, G.cap);
-        if (n == 0xFFFFFFFFu) { too_big = true; n = 0; }
-      }
+      uint32_t n;
+      const bool too_big = !lane_k1(M, B, c, sent, G.cap, &n);
       uint32_t L = 0;
       bool overflow = false;
       uint32_t nn = 0;
@@ -111,7 +88,7 @@ __global__ void __launch_bounds__(512, 1) lattice_lane_kernel(const KModel M, co
       } else if (n != 0) {
         // ---- Lattice::SetSentence ----
         for (uint32_t p = 0; p < n;) {
-          uint32_t mb = one_char_len(text_byte(p));
+          uint32_t mb = one_char_len(lane_text_byte_plain(c, p));
           if (mb > n - p) mb = n - p;
           surf[L] = static_cast<uint16_t>(p);
           A[L] = __uint_as_float(kLatticeUnset);
@@ -127,36 +104,21 @@ __global__ void __launch_bounds__(512, 1) lattice_lane_kernel(const KModel M, co
         // ---- Model::PopulateNodes with Lattice::ForwardAlgorithm folded in ----
         for (uint32_t bp = 0; bp < L && !overflow; ++bp) {
           const float a = A[bp];
-          bool has_single = false;
-          uint32_t l = root;
-          uint32_t clen = 0;  // characters completed so far
-          auto add_node = [&](uint32_t ep, int32_t id, float sc, uint32_t chbytes) {
-            if (nn >= G.node_cap) { overflow = true; return; }
+          auto add_node = [&](uint32_t ep, int32_t id, float sc, uint32_t chbytes) -> bool {
+            if (nn >= G.node_cap) { overflow = true; return false; }
             node[nn++] = make_uint4(static_cast<uint32_t>(id), __float_as_uint(sc), bp | (ep << 16), chbytes);
             ecnt[ep] += 1;
             const float y = __fadd_rn(__fmul_rn(inv_theta, sc), a);
             const float cur = A[ep];
             A[ep] = __float_as_uint(cur) == kLatticeUnset ? y : lattice_log_sum_exp(cur, y);
+            return true;
           };
-          for (uint32_t kpos = surf[bp]; kpos < n && !overflow; ++kpos) {
-            const uint32_t ch = text_byte(kpos);
-            const uint32_t v = (l >> kLinkBaseShift) ^ ch;
-            l = __ldg(&node2[v]).x;
-            if ((l & kLinkLabelMask) != ch) break;
-            if (kpos + 1 == surf[bp + clen + 1]) ++clen;
-            const uint32_t kind = (l >> kLinkKindShift) & 3u;
-            if (kind == kKindNone || kind == kKindUnused) continue;
-            // get_chars_length (:548-552): characters whose start lies before the piece's end
-            const uint32_t length = (kpos + 1 == surf[bp + clen]) ? clen : clen + 1;
-            const float sc = kind == kKindUserDefined
-                                 ? static_cast<float>(static_cast<double>(__fmul_rn(static_cast<float>(length), M.max_score)) - 0.1)
-                                 : __uint_as_float(__ldg(M.trie_val + v));
-            add_node(bp + length, __ldg(M.trie_id + v), sc, 0u);
-            has_single |= length == 1;
-          }
+          const bool has_single = lane_populate_from(M, c, root, surf, bp, n, [&](uint32_t length, uint32_t v, float sc) {
+            return add_node(bp + length, __ldg(M.trie_id + v), sc, 0u);
+          });
           if (!has_single && !overflow) {
             uint32_t chb = 0;
-            for (uint32_t k = surf[bp]; k < surf[bp + 1]; ++k) chb |= text_byte(k) << (8u * (k - surf[bp]));
+            for (uint32_t k = surf[bp]; k < surf[bp + 1]; ++k) chb |= lane_text_byte_plain(c, k) << (8u * (k - surf[bp]));
             add_node(bp + 1, M.unk_id, M.unk_score, chb);
           }
         }

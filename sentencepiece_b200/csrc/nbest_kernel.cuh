@@ -71,17 +71,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
   __syncthreads();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  LaneCtx c;
-  c.pol = slab_policy();
-  {
-    uint8_t *slab = text_slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(G.cap);
-    c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
-    c.log = nullptr; c.rs = nullptr; c.rb = nullptr;
-    c.s_lead = s_tab; c.s_pair = s_tab + 8;
-    c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
-    c.s_plain = s_tab + 8 + 1024 + 128;
-    c.s_plainsp = c.s_plain + 4;
-  }
+  const LaneCtx c = lane_ctx(s_tab, text_slabs, G.cap, warp_global, lane);
   // agenda top: [warp][entry][lane]
   uint2 *s_top = reinterpret_cast<uint2 *>(smem + kLaneTableBytes) + static_cast<size_t>(threadIdx.x >> 5) * (32 * TOP) + lane;
   // per-lane scratch
@@ -95,12 +85,8 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
   uint16_t *surf = reinterpret_cast<uint16_t *>(sp);
   uint32_t *sort_cur = reinterpret_cast<uint32_t *>(maxbt);  // maxbt is dead once the nodes exist
 
-  const uint2 *node2 = M.trie_node2;
-  const uint32_t root = __ldg(&node2[0]).x;
+  const uint32_t root = __ldg(&M.trie_node2[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
-  auto text_byte = [&](uint32_t k) -> uint32_t {
-    return (c.text_w[static_cast<size_t>(k >> 2) * 32] >> ((k & 3u) * 8u)) & 0xFFu;
-  };
   auto hget = [&](uint32_t i) -> uint2 { return i < TOP ? s_top[i * 32] : heap[i + 1]; };
   auto hset = [&](uint32_t i, uint2 e) {
     if (i < TOP) s_top[i * 32] = e;
@@ -157,21 +143,12 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
     return top;
   };
 
-  for (;;) {
-    uint32_t first = 0;
-    if (lane == 0) first = atomicAdd(B.work_counter, 32u);
-    first = __shfl_sync(0xFFFFFFFFu, first, 0);
-    if (first >= B.n) break;
+  uint32_t first = 0;
+  while (lane_claim_group(B, lane, &first)) {
     if (first + lane < B.n) {
       const uint32_t sent = B.order ? B.order[first + lane] : first + lane;
-      const unsigned long long off = B.offsets[sent];
-      const unsigned long long len64 = B.offsets[sent + 1] - off;
-      uint32_t n = 0;
-      bool too_big = len64 > 4ull * G.cap;
-      if (!too_big) {
-        n = lane_normalize(M, B.bytes + off, static_cast<uint32_t>(len64), c, G.cap);
-        if (n == 0xFFFFFFFFu) { too_big = true; n = 0; }
-      }
+      uint32_t n;
+      const bool too_big = !lane_k1(M, B, c, sent, G.cap, &n);
       const size_t cbase = static_cast<size_t>(sent) * nbest;
       uint32_t K = 0;
       if (too_big) {
@@ -184,7 +161,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
         // ---- Lattice::SetSentence ----
         uint32_t L = 0;
         for (uint32_t p = 0; p < n;) {
-          uint32_t mb = one_char_len(text_byte(p));
+          uint32_t mb = one_char_len(lane_text_byte_plain(c, p));
           if (mb > n - p) mb = n - p;
           surf[L] = static_cast<uint16_t>(p);
           maxbt[L] = -INFINITY;
@@ -203,30 +180,15 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
         // monotone in x, so it equals fl(max_q backtrace(q) + score(r)), and every q is complete before r is made.
         for (uint32_t bp = 0; bp < L && !overflow; ++bp) {
           const float in_bt = maxbt[bp];
-          bool has_single = false;
-          uint32_t l = root;
-          uint32_t clen = 0;  // characters completed so far
-          for (uint32_t kpos = surf[bp]; kpos < n; ++kpos) {
-            const uint32_t ch = text_byte(kpos);
-            const uint32_t v = (l >> kLinkBaseShift) ^ ch;
-            l = __ldg(&node2[v]).x;
-            if ((l & kLinkLabelMask) != ch) break;
-            if (kpos + 1 == surf[bp + clen + 1]) ++clen;
-            const uint32_t kind = (l >> kLinkKindShift) & 3u;
-            if (kind == kKindNone || kind == kKindUnused) continue;
-            // get_chars_length (:548-552): characters whose start lies before the piece's end
-            const uint32_t length = (kpos + 1 == surf[bp + clen]) ? clen : clen + 1;
-            if (nn >= G.node_cap) { overflow = true; break; }
-            const float sc = kind == kKindUserDefined
-                                 ? static_cast<float>(static_cast<double>(__fmul_rn(static_cast<float>(length), M.max_score)) - 0.1)
-                                 : __uint_as_float(__ldg(M.trie_val + v));
+          const bool has_single = lane_populate_from(M, c, root, surf, bp, n, [&](uint32_t length, uint32_t v, float sc) {
+            if (nn >= G.node_cap) { overflow = true; return false; }
             const float bt = __fadd_rn(in_bt, sc);
             node[nn] = make_uint4(static_cast<uint32_t>(__ldg(M.trie_id + v)), __float_as_uint(sc), __float_as_uint(bt),
                                   bp | ((bp + length) << 16));
             maxbt[bp + length] = fmaxf(maxbt[bp + length], bt);
             ++nn;
-            has_single |= length == 1;
-          }
+            return true;
+          });
           if (!has_single && !overflow) {
             if (nn >= G.node_cap) { overflow = true; break; }
             const float bt = __fadd_rn(in_bt, M.unk_score);
@@ -278,7 +240,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
                   if (isunk) {
                     if (bf) {
                       for (uint32_t k = surf[nd.w & 0xFFFFu]; k < surf[nd.w >> 16]; ++k)
-                        O.tmp_ids[pos + (w++)] = __ldg(M.byte_to_id + text_byte(k));
+                        O.tmp_ids[pos + (w++)] = __ldg(M.byte_to_id + lane_text_byte_plain(c, k));
                     } else if (!prev_unk) {
                       O.tmp_ids[pos + (w++)] = M.unk_id;
                     }
