@@ -996,12 +996,14 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     }
     uint32_t n_def = h_ctrl32.p[0];
     const uint32_t *def_list = d_deferred.p;
-    if (n_def && lane_path) {
-      // ---- second chance: the sentences a lane kernel could not take (long words, long
-      //      sentences) go through the shared-memory warp kernels before the HBM-scratch path ----
+    // ---- second chance: the sentences a lane kernel could not take (long words, long sentences) go through the
+    //      shared-memory warp kernels before the HBM-scratch path -- unless their tiles do not fit in shared memory
+    //      (a model with up to 62 piece matches per start), in which case the HBM-scratch path takes them all ----
+    const LaunchGeom g2 = n_def && lane_path ? plan_geometry(*this, bpe ? bpe_tile_bytes(ncap, false)
+                                                                       : tile_bytes_for(ncap, K, false), tile_threads / 32)
+                                             : LaunchGeom{};
+    if (n_def && lane_path && g2.smem_bytes <= smem_optin) {
       last_deferred = n_def;
-      const LaunchGeom g2 =
-          plan_geometry(*this, bpe ? bpe_tile_bytes(ncap, false) : tile_bytes_for(ncap, K, false), tile_threads / 32);
       KModel M2 = km;
       M2.hot_link = g2.hot_link;
       M2.hot_val = g2.hot_val;
