@@ -110,8 +110,6 @@ __device__ __forceinline__ void lane_wait_input(const KBatch &B, uint32_t first,
 struct LaneCtx {
   uint32_t *text_w;  // + word*32 (already offset by lane)
   uint32_t *log;     // + t*32    (already offset by lane)
-  float *rs;         // ring scores, + slot*32 (already offset by lane)
-  uint32_t *rb;      // ring back-pointers (plen<<24 | unit), 0 = unset
   const uint32_t *s_lead, *s_pair;
   const int32_t *s_solo;
   const uint32_t *s_plain;  // bit b: ASCII byte b is copied verbatim (no rule starts with it, not a space)
@@ -156,8 +154,7 @@ __device__ __forceinline__ void slab_discard(const LaneCtx &c, uint32_t lane, ui
   __syncwarp();
 }
 
-// The lane's view of its warp's slab and of the normalizer's tables (s_tab, filled by fill_lane_tables).  The rings
-// (rs / rb) belong to the kernels that have them and are left null here.
+// The lane's view of its warp's slab and of the normalizer's tables (s_tab, filled by fill_lane_tables).
 __device__ __forceinline__ LaneCtx lane_ctx(const uint32_t *s_tab, uint8_t *slabs, uint32_t cap, uint32_t warp_global,
                                             uint32_t lane) {
   LaneCtx c;
@@ -165,8 +162,6 @@ __device__ __forceinline__ LaneCtx lane_ctx(const uint32_t *s_tab, uint8_t *slab
   uint8_t *slab = slabs + static_cast<size_t>(warp_global) * lane_slab_bytes(cap);
   c.text_w = reinterpret_cast<uint32_t *>(slab) + lane;
   c.log = reinterpret_cast<uint32_t *>(slab) + static_cast<size_t>(cap / 4 + kLaneTextSlack) * 32 + lane;
-  c.rs = nullptr;
-  c.rb = nullptr;
   c.s_lead = s_tab;
   c.s_pair = s_tab + 8;
   c.s_solo = reinterpret_cast<const int32_t *>(s_tab + 8 + 1024);
@@ -660,10 +655,49 @@ __device__ __forceinline__ void lane_finish(const KModel &M, const KBatch &B, co
   slab_discard(c, lane, (__reduce_max_sync(0xFFFFFFFFu, n) >> 2) + 4u, max_log);
 }
 
-// shared memory per warp: ring of R slots, each {score f32, back-pointer u32, position tag u16} x 32 lanes
-__host__ __device__ inline uint32_t lane_ring_bytes(uint32_t R) { return R * 32u * (4u + 4u + 2u); }
+// Ring of the unigram lane kernels, R slots per warp.  A slot is a row of 32 scores (f32), then a row of 32 back-pointers
+// (u32) and, in encode_unigram_lane_kernel, a row of 32 position tags (u16).  K2 holds the 32-bit shared-memory offset
+// of the lane's score in a slot: the back-pointer is kRingBp bytes further, the tag tag_delta = kRingTag - 2 * lane
+// bytes further, and the next slot kRingSlot bytes further.  Stepping to a slot is one add and a wrap, and no pointer
+// has to be rebuilt inside the loop.
+constexpr uint32_t kRingBp = 32u * 4u, kRingTag = 32u * 8u;
+constexpr uint32_t kRingSlot = 32u * (4u + 4u + 2u), kPlainRingSlot = 32u * (4u + 4u);
+__host__ __device__ inline uint32_t lane_ring_bytes(uint32_t R) { return R * kRingSlot; }
 // the same for encode_unigram_lane_plain_kernel, whose slots have no position tag
-__host__ __device__ inline uint32_t lane_plain_ring_bytes(uint32_t R) { return R * 32u * (4u + 4u); }
+__host__ __device__ inline uint32_t lane_plain_ring_bytes(uint32_t R) { return R * kPlainRingSlot; }
+// Ring accesses by shared-memory address (the kernels fold the CTA's shared-memory base into their ring offsets once).
+static_assert(kRingBp == 128, "ring_ld_bp / ring_st_bp spell the back-pointer displacement as +128");
+__device__ __forceinline__ float ring_ld_score(uint32_t a) {
+  float v;
+  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ uint32_t ring_ld_bp(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.u32 %0, [%1+128];" : "=r"(v) : "r"(a) : "memory");  // + kRingBp
+  return v;
+}
+__device__ __forceinline__ uint32_t ring_ld_tag(uint32_t a) {
+  uint16_t v;
+  asm volatile("ld.shared.u16 %0, [%1];" : "=h"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void ring_st_score(uint32_t a, float v) {
+  asm volatile("st.shared.f32 [%0], %1;" :: "r"(a), "f"(v) : "memory");
+}
+__device__ __forceinline__ void ring_st_bp(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.u32 [%0+128], %1;" :: "r"(a), "r"(v) : "memory");  // + kRingBp
+}
+__device__ __forceinline__ void ring_st_tag(uint32_t a, uint32_t v) {
+  asm volatile("st.shared.u16 [%0], %1;" :: "r"(a), "h"(static_cast<uint16_t>(v)) : "memory");
+}
+
+// base_regular of the K2 loops: |x| in {0} U [2^-10, 2^18), the range in which the float two-sum decides the reference's
+// double comparison exactly (Q1), tested on the bits.  NaN, infinities and denormals fail; -0.0 passes.
+__device__ __forceinline__ bool score_regular(float x) {
+  const uint32_t a = __float_as_uint(x) << 1;  // the bits of |x|, shifted left by one
+  return a == 0u || a - (0x3A800000u << 1) < ((0x48800000u - 0x3A800000u) << 1);  // 2^-10 = 0x3A800000, 2^18 = 0x48800000
+}
 
 constexpr uint32_t kLogWordStep = 1u << 31;  // log entry: the previous logged position is plen bytes back (whole word)
 constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of a little-endian word
@@ -684,27 +718,25 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
                                                                        uint32_t cap, uint32_t R) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem);
-  uint8_t *rings = smem + kLaneTableBytes;
   fill_lane_tables(M, s_tab);
   __syncthreads();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
-  uint16_t *rp;  // ring position tags: a slot belongs to position p iff rp == p (no clearing, skipped positions
-                 // of whole words leave stale slots behind that simply fail the test)
-  {
-    uint8_t *ring = rings + static_cast<size_t>(warp_in_cta) * lane_ring_bytes(R);
-    c.rs = reinterpret_cast<float *>(ring) + lane;
-    c.rb = reinterpret_cast<uint32_t *>(ring + R * 32 * 4) + lane;
-    rp = reinterpret_cast<uint16_t *>(ring + R * 32 * 8) + lane;
-  }
+  const LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  // ring offsets (see kRingSlot): the lane's score in slot 0, one past the last slot.  Position tags: a slot belongs to
+  // position p iff its tag == p (no clearing: skipped positions of whole words leave stale slots behind that simply
+  // fail the test).
+  const uint32_t ring_lo = static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + kLaneTableBytes +
+                           warp_in_cta * lane_ring_bytes(R) + lane * 4u;
+  const uint32_t ring_span = lane_ring_bytes(R);
+  const uint32_t ring_hi = ring_lo + ring_span;
+  const uint32_t tag_delta = kRingTag - 2u * lane;
   const uint4 *node4 = M.trie_node4;
   const uint32_t root = __ldg(&node4[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
   const bool regular = M.flags & kFlagRegularScores;
   const bool fastwords = M.flags & kFlagFastWords;
-  const uint32_t r_wrap = R * 32;
 
   uint32_t first = 0;
   while (lane_claim_group(B, lane, &first)) {
@@ -723,10 +755,11 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     clk.mark();
     // ---------------- K2: flat state machine, one trie transition per trip ----------------
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
-    // from the walk position k (low byte first).  ss = ring slot of s, times 32.
-    uint32_t s = 0, ss = 0, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0;
+    // from the walk position k (low byte first).  ss = ring offset of s's slot.  kb = the byte at k once the walk
+    // has read it (the byte that failed the label test or the child mask), for the word-end test of the start block.
+    uint32_t s = 0, ss = ring_lo, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0, kb = 0;
     bool has_single = false, done = n == 0;
-    bool wstart = true;  // s is the first character of a word (text start or kWsByte)
+    bool wstart = fastwords;  // the shortcut is on and s is the first character of a word (text start or kWsByte)
     float base = 0.f;
     bool base_regular = regular;  // base == 0
     uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
@@ -742,20 +775,22 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
              (static_cast<unsigned long long>(w3 >> sh) << 32);
     };
     if (!done) {
-      for (uint32_t r = 0; r < R; ++r) rp[r * 32] = 0xFFFFu;  // no slot belongs to a position of this sentence
-      c.rs[0] = 0.f;
+      for (uint32_t r = 0; r < R; ++r) ring_st_tag(ring_lo + r * kRingSlot + tag_delta, 0xFFFFu);  // no slot belongs to a position of this sentence
+      ring_st_score(ring_lo, 0.f);
       w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len_ws1(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
     }
     // optional counters (engine: SPM_B200_KSTATS; device-resident path only): [8] warp trips, [9] lane trips,
-    // [10] starts retired, [11] whole words, [12] groups, [13] normalized bytes
+    // [10] starts retired, [11] whole words, [12] groups, [13] normalized bytes.  The loop counts only the lane's
+    // trips (always: a test would cost more than the add): the warp's trips are their maximum, the starts are the log entries and the whole words the entries with
+    // kLogWordStep.
     const bool kst = B.kstats != nullptr && B.seg_done == nullptr;
-    uint32_t st_trips = 0, st_lane = 0, st_starts = 0, st_fast = 0;
+    uint32_t st_lane = 0;
     while (__any_sync(0xFFFFFFFFu, !done)) {
-      if (kst) { ++st_trips; st_lane += !done; }
       if (!done) {
+        ++st_lane;
         bool end_walk = true;
         if (k < n) {
           const uint32_t d = k - s;
@@ -767,6 +802,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
             ch = static_cast<uint32_t>(cur) & 0xFFu;
             cur >>= 8;
           }
+          kb = ch;
           const uint32_t v = (l >> kLinkBaseShift) ^ ch;
           const uint4 nd = __ldg(&node4[v]);  // {link, child mask, score, word_safe}: one 16-byte load (L1/L2)
           if ((nd.x & kLinkLabelMask) == ch) {
@@ -776,10 +812,10 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
             const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
             if (kind == kKindNormal || kind == kKindUserDefined) {
               const uint32_t plen = k - s;
-              uint32_t sl = ss + plen * 32u;
-              if (sl >= r_wrap) sl -= r_wrap;
-              const float curs = c.rs[sl];
-              const bool unset = rp[sl] != k;
+              uint32_t sl = ss + plen * kRingSlot;
+              if (sl >= ring_hi) sl -= ring_span;
+              const float curs = ring_ld_score(sl);
+              const bool unset = ring_ld_tag(sl + tag_delta) != k;
               float ns;
               bool better;
               if (kind == kKindNormal && base_regular) {
@@ -801,68 +837,58 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
                 ns = static_cast<float>(cand);
               }
               if (better) {
-                c.rs[sl] = ns;
-                c.rb[sl] = (plen << 24) | v;
-                rp[sl] = static_cast<uint16_t>(k);
+                ring_st_score(sl, ns);
+                ring_st_bp(sl, (plen << 24) | v);
+                ring_st_tag(sl + tag_delta, k);
               }
               has_single |= plen == mblen;
             }
             // early termination: if the node has no child on the next byte the failing
             // probe (and its cold miss) is skipped and the start transition happens now
             if (k < n) {
-              uint32_t nb;
               const uint32_t d2 = k - s;
-              if (d2 >= 13u) nb = lane_text_byte(c, k);
-              else nb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
-              end_walk = !((nd.y >> (nb & 31u)) & 1u);
+              if (d2 >= 13u) kb = lane_text_byte(c, k);
+              else kb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
+              end_walk = !((nd.y >> (kb & 31u)) & 1u);
             }
           }
         }
         if (end_walk) {
-          // the walk from s is over (traverse() == -2, or end of text)
-          bool fast = false;
-          if (fastwords && wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal) {
-            // the walk covered [s, k) and ended on a NORMAL piece: is k the end of the word, early enough to be safe?
-            bool wend = k >= n;
-            if (!wend) {
-              const uint32_t wi = (k >> 2) - (s >> 2);  // word of the window that holds byte k
-              const uint32_t wd = wi == 0u ? w0 : (wi == 1u ? w1 : (wi == 2u ? w2 : (wi == 3u ? w3 : slab_ld(c.text_w + static_cast<size_t>(k >> 2) * 32, c.pol))));
-              wend = ((wd >> ((k & 3u) * 8u)) & 0xFFu) == kWsByte;
-            }
-            fast = wend && k <= lsafe;
-          }
+          // the walk from s is over (traverse() == -2, or end of text).  Whole word: the walk covered [s, k) from a
+          // word start and ended on a NORMAL piece at the end of the word, early enough to be safe.
+          const bool fast = wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal && (k >= n || kb == kWsByte) &&
+                            k <= lsafe;
           const uint32_t s_old = s;
           uint32_t steplog;
-          if (kst) { ++st_starts; st_fast += fast; }
           if (fast) {
             // the piece was relaxed into k when the walk stepped onto its node; nothing else can win there
-            ss += (k - s) * 32u;
+            ss += (k - s) * kRingSlot;
+            if (ss >= ring_hi) ss -= ring_span;
             s = k;
             steplog = kLogWordStep;
           } else {
-            uint32_t sl = ss + mblen * 32u;
-            if (sl >= r_wrap) sl -= r_wrap;
+            uint32_t sl = ss + mblen * kRingSlot;
+            if (sl >= ring_hi) sl -= ring_span;
             if (!has_single) {  // UNK edge, unigram_model.cc:995-1005
               const float cand = __fadd_rn(M.unk_score, base);
-              if (rp[sl] != s + mblen || cand > c.rs[sl]) {
-                c.rs[sl] = cand;
-                c.rb[sl] = (mblen << 24) | kLaneUnk;
-                rp[sl] = static_cast<uint16_t>(s + mblen);
+              if (ring_ld_tag(sl + tag_delta) != s + mblen || cand > ring_ld_score(sl)) {
+                ring_st_score(sl, cand);
+                ring_st_bp(sl, (mblen << 24) | kLaneUnk);
+                ring_st_tag(sl + tag_delta, s + mblen);
               }
             }
             ss = sl;
             s += mblen;
             steplog = (mblen - 1u) << 22;
           }
-          if (ss >= r_wrap) ss -= r_wrap;
           // position s is final: append (plen | previous char length or whole-word step | unit) to the log
-          slab_st(c.log + static_cast<size_t>(nlog) * 32, c.rb[ss] | steplog, c.pol);
+          slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | steplog, c.pol);
           ++nlog;
           if (s >= n) {
             done = true;
           } else {
-            base = c.rs[ss];
-            base_regular = regular && (base == 0.f || (fabsf(base) >= 0.0009765625f && fabsf(base) < 262144.f));
+            base = ring_ld_score(ss);
+            base_regular = regular && score_regular(base);
             // slide the text window so that it is anchored at s; prefetch the new tail word
             const uint32_t jw = (s >> 2) - (s_old >> 2);
             if (jw == 1u) {
@@ -877,8 +903,9 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
               w0 = slab_ld(tw + 0, c.pol); w1 = slab_ld(tw + 32, c.pol); w2 = slab_ld(tw + 64, c.pol); w3 = slab_ld(tw + 96, c.pol);
             }
             cur = window_low();
-            wstart = (static_cast<uint32_t>(cur) & 0xFFu) == kWsByte;
-            mblen = one_char_len_ws1(static_cast<uint32_t>(cur) & 0xFFu);
+            const uint32_t b0 = static_cast<uint32_t>(cur) & 0xFFu;
+            wstart = fastwords && b0 == kWsByte;
+            mblen = one_char_len_ws1(b0);
             if (mblen > n - s) mblen = n - s;
             k = s;
             l = root;
@@ -889,13 +916,13 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     }
     if (kst) {
       typedef unsigned long long ull;
-      uint32_t nb = n;
-      for (int d = 16; d > 0; d >>= 1) {
-        st_lane += __shfl_xor_sync(0xFFFFFFFFu, st_lane, d);
-        st_starts += __shfl_xor_sync(0xFFFFFFFFu, st_starts, d);
-        st_fast += __shfl_xor_sync(0xFFFFFFFFu, st_fast, d);
-        nb += __shfl_xor_sync(0xFFFFFFFFu, nb, d);
-      }
+      uint32_t st_fast = 0;
+      for (uint32_t t = 0; t < nlog; ++t) st_fast += slab_ld(c.log + static_cast<size_t>(t) * 32, c.pol) >> 31;
+      const uint32_t st_trips = __reduce_max_sync(0xFFFFFFFFu, st_lane);
+      st_lane = __reduce_add_sync(0xFFFFFFFFu, st_lane);
+      const uint32_t st_starts = __reduce_add_sync(0xFFFFFFFFu, nlog);
+      st_fast = __reduce_add_sync(0xFFFFFFFFu, st_fast);
+      const uint32_t nb = __reduce_add_sync(0xFFFFFFFFu, n);
       if (lane == 0) {
         atomicAdd(B.kstats + 8, ull(st_trips)); atomicAdd(B.kstats + 9, ull(st_lane)); atomicAdd(B.kstats + 10, ull(st_starts));
         atomicAdd(B.kstats + 11, ull(st_fast)); atomicAdd(B.kstats + 12, ull(1)); atomicAdd(B.kstats + 13, ull(nb));
@@ -919,18 +946,17 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
                                                                        uint32_t cap, uint32_t R) {
   extern __shared__ __align__(128) uint8_t smem[];
   uint32_t *s_tab = reinterpret_cast<uint32_t *>(smem);
-  uint8_t *rings = smem + kLaneTableBytes;
   fill_lane_tables(M, s_tab);
   __syncthreads();
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
-  {
-    uint8_t *ring = rings + static_cast<size_t>(warp_in_cta) * lane_plain_ring_bytes(R);
-    c.rs = reinterpret_cast<float *>(ring) + lane;
-    c.rb = reinterpret_cast<uint32_t *>(ring + R * 32 * 4) + lane;
-  }
+  const LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  // ring offsets (see kRingSlot): the lane's score in slot 0, one past the last slot
+  const uint32_t ring_lo = static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + kLaneTableBytes +
+                           warp_in_cta * lane_plain_ring_bytes(R) + lane * 4u;
+  const uint32_t ring_span = lane_plain_ring_bytes(R);
+  const uint32_t ring_hi = ring_lo + ring_span;
   const uint2 *node2 = M.trie_node2;
   const uint32_t root = __ldg(&node2[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
@@ -954,7 +980,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
     // ---------------- K2: flat state machine, one trie transition per trip ----------------
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
     // from the walk position k (low byte first).
-    uint32_t s = 0, ss = 0 /* ring slot of s */, k = 0, l = root, mblen = 1, nlog = 0;
+    uint32_t s = 0, ss = ring_lo /* ring offset of s's slot */, k = 0, l = root, mblen = 1, nlog = 0;
     bool has_single = false, done = n == 0;
     float base = 0.f;
     bool base_regular = regular;  // base == 0
@@ -971,8 +997,8 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
              (static_cast<unsigned long long>(w3 >> sh) << 32);
     };
     if (!done) {
-      for (uint32_t r = 0; r < R; ++r) c.rb[r * 32] = 0u;  // all positions unset
-      c.rs[0] = 0.f;
+      for (uint32_t r = 0; r < R; ++r) ring_st_bp(ring_lo + r * kPlainRingSlot, 0u);  // all positions unset
+      ring_st_score(ring_lo, 0.f);
       w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len(w0 & 0xFFu);
       if (mblen > n) mblen = n;
@@ -999,11 +1025,10 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
             const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
             if (kind == kKindNormal || kind == kKindUserDefined) {
               const uint32_t plen = k - s;
-              uint32_t sl = ss + plen;
-              if (sl >= R) sl -= R;
-              sl *= 32;
-              const float curs = c.rs[sl];
-              const bool unset = c.rb[sl] == 0u;
+              uint32_t sl = ss + plen * kPlainRingSlot;
+              if (sl >= ring_hi) sl -= ring_span;
+              const float curs = ring_ld_score(sl);
+              const bool unset = ring_ld_bp(sl) == 0u;
               float ns;
               bool better;
               if (kind == kKindNormal && base_regular) {
@@ -1025,8 +1050,8 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
                 ns = static_cast<float>(cand);
               }
               if (better) {
-                c.rs[sl] = ns;
-                c.rb[sl] = (plen << 24) | v;
+                ring_st_score(sl, ns);
+                ring_st_bp(sl, (plen << 24) | v);
               }
               has_single |= plen == mblen;
             }
@@ -1043,28 +1068,28 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
         }
         if (end_walk) {
           // the walk from s is over (traverse() == -2, or end of text)
-          uint32_t sl = ss + mblen;
-          if (sl >= R) sl -= R;
+          uint32_t sl = ss + mblen * kPlainRingSlot;
+          if (sl >= ring_hi) sl -= ring_span;
           if (!has_single) {  // UNK edge, unigram_model.cc:995-1005
             const float cand = __fadd_rn(M.unk_score, base);
-            if (c.rb[sl * 32] == 0u || cand > c.rs[sl * 32]) {
-              c.rs[sl * 32] = cand;
-              c.rb[sl * 32] = (mblen << 24) | kLaneUnk;
+            if (ring_ld_bp(sl) == 0u || cand > ring_ld_score(sl)) {
+              ring_st_score(sl, cand);
+              ring_st_bp(sl, (mblen << 24) | kLaneUnk);
             }
           }
           // position s leaves the window; only character starts are ever targets, so its
           // slot is the only one that has to be cleared for position s + R
-          c.rb[ss * 32] = 0u;
+          ring_st_bp(ss, 0u);
           s += mblen;
           ss = sl;
           // position s is final: append (plen | previous char length | unit) to the log
-          slab_st(c.log + static_cast<size_t>(nlog) * 32, c.rb[ss * 32] | ((mblen - 1u) << 22), c.pol);
+          slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | ((mblen - 1u) << 22), c.pol);
           ++nlog;
           if (s >= n) {
             done = true;
           } else {
-            base = c.rs[ss * 32];
-            base_regular = regular && (base == 0.f || (fabsf(base) >= 0.0009765625f && fabsf(base) < 262144.f));
+            base = ring_ld_score(ss);
+            base_regular = regular && score_regular(base);
             // slide the text window so that it is anchored at s; prefetch the new tail word
             if ((s >> 2) != ((s - mblen) >> 2)) {
               w0 = w1; w1 = w2; w2 = w3;
