@@ -392,7 +392,7 @@ __global__ void __launch_bounds__(256) encode_bpe_long_kernel(const KModel M, co
     const uint32_t len = static_cast<uint32_t>(B.offsets[sent + 1] - off);
     uint32_t need = 0;
     const bool ok = encode_bpe_sentence<SPANS>(M, B, T, H, bm, B.bytes + off, len, sent, &need);
-    if (!ok && T.lane == 0) atomicOr(B.status + 1, 2u);
+    if (!ok && T.lane == 0) atomicOr(B.status + 1, 8u);  // the slab was too small: its own bit and message
     __syncwarp();
   }
 }

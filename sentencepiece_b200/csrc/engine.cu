@@ -478,14 +478,18 @@ int spm_engine::build_tables() {
     auto off = [](uint32_t u) { return (u >> 10) << ((u & (1u << 9)) >> 6); };
     auto label = [](uint32_t u) { return u & ((1u << 31) | 0xFFu); };
     if (NU == 0) { set_error("Blob for normalization rule is broken."); return SPM_ERR_MODEL; }
-    // enumerate all keys by DFS over the double array: (node after the step, depth)
+    // enumerate all keys breadth-first over the double array: (node after the step, depth).  Keys of any length
+    // count: a rule set may have keys of hundreds of bytes, and their expansion sizes the long-sentence scratch.  The
+    // double array is a DAWG (darts-clone shares common suffixes), so a node can have several parents; breadth-first,
+    // a node is first reached at its least depth, where its keys have their highest ratio, and is walked on from there
+    // only.  Every edge still sets the lead / pair tables.  At most NU frames, also for a malformed blob.
     struct Fr { uint32_t node; uint32_t depth; uint32_t first; };
-    std::vector<Fr> stack;
+    std::vector<Fr> queue;
+    std::vector<uint8_t> queued(NU, 0);
     const uint32_t root_next = 0 ^ off(cm_units[0]);
-    stack.push_back({root_next, 0, 256});
-    while (!stack.empty()) {
-      const Fr f = stack.back();
-      stack.pop_back();
+    queue.push_back({root_next, 0, 256});
+    for (size_t head = 0; head < queue.size(); ++head) {
+      const Fr f = queue[head];
       for (uint32_t c = 0; c < 256; ++c) {
         const uint32_t node = f.node ^ c;
         if (node >= NU) continue;
@@ -515,7 +519,9 @@ int spm_engine::build_tables() {
             max_expand_den = static_cast<uint32_t>(klen);
           }
         }
-        if (f.depth < 64) stack.push_back({nxt, f.depth + 1, first});
+        if (queued[node]) continue;
+        queued[node] = 1;
+        queue.push_back({nxt, f.depth + 1, first});
       }
     }
   }
@@ -1082,7 +1088,8 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       h_ctrl32.p[2] |= h_ctrl32.p[10];
     }
     if (h_ctrl32.p[1]) {
-      if (h_ctrl32.p[1] & 2u) set_error("encode failed: the host-to-device copy of a streamed batch made no progress for 3 s");
+      if (h_ctrl32.p[1] & 8u) set_error("encode failed: a long sentence normalized to more bytes than the scratch sized for it");
+      else if (h_ctrl32.p[1] & 2u) set_error("encode failed: the host-to-device copy of a streamed batch made no progress for 3 s");
       else set_error("encode failed: internal consistency check (status " + std::to_string(h_ctrl32.p[1]) + ")");
       return SPM_ERR_ENCODE;
     }

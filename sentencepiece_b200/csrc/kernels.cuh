@@ -772,7 +772,7 @@ __global__ void __launch_bounds__(256) encode_unigram_long_kernel(const KModel M
     const uint32_t len = static_cast<uint32_t>(B.offsets[sent + 1] - off);
     uint32_t need = 0;
     const bool ok = encode_unigram_sentence<SPANS>(M, B, T, H, tm, B.bytes + off, len, sent, &need);
-    if (!ok && T.lane == 0) atomicOr(B.status + 1, 2u);  // slab was sized from an upper bound: cannot happen
+    if (!ok && T.lane == 0) atomicOr(B.status + 1, 8u);  // slab sized from an upper bound too small: its own bit and message
     __syncwarp();
   }
 }

@@ -72,6 +72,9 @@ __device__ __forceinline__ void fill_lane_tables(const KModel &M, uint32_t *s_ta
       simple = M.cm_solo[ch] < 0;
       for (uint32_t q = 0; q < 4; ++q) simple = simple && M.cm_pair[((ch * 256u) >> 5) + q] == 0u;
     }
+    // The 4-byte step emits at most 8 bytes.  An escaped space is 3 bytes, so four bytes hold at most two of them: true
+    // only when remove_extra_whitespaces drops the second of two adjacent spaces.  Otherwise the space is not simple.
+    if (ch == ' ' && (M.flags & kFlagEscapeWs) && !(M.flags & kFlagRemoveExtraWs)) simple = false;
     const uint32_t word = __ballot_sync(0xFFFFFFFFu, simple);
     if ((threadIdx.x & 31) == 0) s_tab[8 + 1024 + 128 + 4 + wq] = word;
   }

@@ -7,6 +7,9 @@ reference compiled under oracle/_ref (needs /root/reference for that build).
   tests/golden/charsmap_space_rules.bin     the space-containing rule set of
                                             src/normalizer_test.cc:149-164 compiled with the
                                             reference's own Builder::CompileCharsMap
+  tests/golden/charsmaps/<name>.bin         the rule sets of tests/charsmap_rules.py: the real ones
+                                            from Builder::GetPrecompiledCharsMap, the synthetic ones
+                                            compiled by Builder::CompileCharsMap
 """
 import base64
 import json
@@ -19,6 +22,8 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import charsmap_rules  # noqa: E402
 import corpus  # noqa: E402
 from oracle import oracle_py  # noqa: E402
 
@@ -35,30 +40,45 @@ EDGE = [b"", b" ", b"   ", b"\t", b"a", b"hello world", b"  hello   world  ", b"
         b"\xf0\x9f\x98", "a　　b  c\t\td".encode(), "Ａｐｐｌｅ　ｐｉｅ".encode()]
 
 
-def build_space_charsmap():
+def build_charsmap_tool():
+    """a small program linked against the reference's Builder: `mk_charsmap OUT --rules FILE` compiles the rules of
+    FILE (one "<hex key> <hex target>" line each) with CompileCharsMap, `mk_charsmap OUT --real NAME` writes the
+    precompiled rule set NAME"""
     src = os.path.join("/tmp", "mk_charsmap.cc")
     with open(src, "w") as f:
-        f.write(r'''
+        f.write(r"""
 #include <cstdio>
+#include <fstream>
 #include <string>
 #include "builder.h"
 #include "util.h"
 using namespace sentencepiece;
+static std::string unhex(const std::string &h) {
+  std::string s;
+  for (size_t i = 0; i + 1 < h.size(); i += 2) s += static_cast<char>(std::stoi(h.substr(i, 2), nullptr, 16));
+  return s;
+}
 int main(int argc, char **argv) {
-  normalizer::Builder::CharsMap cm;
-  auto add = [&](const std::string &s, const std::string &t) {
-    normalizer::Builder::Chars a, b;
-    for (const char32 c : string_util::UTF8ToUnicodeText(s)) a.push_back(c);
-    for (const char32 c : string_util::UTF8ToUnicodeText(t)) b.push_back(c);
-    cm[a] = b;
-  };
-  add("a", " A"); add("b", "B"); add("c", "D E"); add("d", " F G ");
-  std::string out;
-  if (!normalizer::Builder::CompileCharsMap(cm, &out).ok()) return 1;
+  if (argc != 4) return 2;
+  std::string out, mode = argv[2];
+  if (mode == "--real") {
+    if (!normalizer::Builder::GetPrecompiledCharsMap(argv[3], &out).ok()) return 1;
+  } else {
+    normalizer::Builder::CharsMap cm;
+    std::ifstream in(argv[3]);
+    std::string hk, ht;
+    while (in >> hk >> ht) {
+      normalizer::Builder::Chars a, b;
+      for (const char32 c : string_util::UTF8ToUnicodeText(unhex(hk))) a.push_back(c);
+      for (const char32 c : string_util::UTF8ToUnicodeText(unhex(ht == "-" ? "" : ht))) b.push_back(c);
+      cm[a] = b;
+    }
+    if (!normalizer::Builder::CompileCharsMap(cm, &out).ok()) return 1;
+  }
   FILE *f = fopen(argv[1], "wb"); fwrite(out.data(), 1, out.size(), f); fclose(f);
   return 0;
 }
-''')
+""")
     ref = "/root/reference"
     out = os.path.join("/tmp", "mk_charsmap")
     subprocess.check_call(["g++", "-std=c++17", "-O1", "-w", "-D_USE_INTERNAL_STRING_VIEW", "-DHAVE_PTHREAD=1", "-pthread",
@@ -66,7 +86,27 @@ int main(int argc, char **argv) {
                            f"-I{ref}/third_party/protobuf-lite", f"-I{ref}/third_party", src,
                            f"{ROOT}/oracle/_ref/libsentencepiece_train.a", f"{ROOT}/oracle/_ref/libsentencepiece.a",
                            "-o", out])
-    subprocess.check_call([out, os.path.join(GOLD, "charsmap_space_rules.bin")])
+    return out
+
+
+def compile_rules(tool, rules, path):
+    txt = os.path.join("/tmp", "mk_charsmap_rules.txt")
+    with open(txt, "w") as f:
+        for k, t in rules:
+            f.write(f"{k.encode().hex()} {t.encode().hex() or '-'}\n")
+    subprocess.check_call([tool, path, "--rules", txt])
+
+
+def build_charsmaps():
+    tool = build_charsmap_tool()
+    # src/normalizer_test.cc:149-164
+    compile_rules(tool, [("a", " A"), ("b", "B"), ("c", "D E"), ("d", " F G ")],
+                  os.path.join(GOLD, "charsmap_space_rules.bin"))
+    os.makedirs(charsmap_rules.DIR, exist_ok=True)
+    for name in charsmap_rules.REAL:
+        subprocess.check_call([tool, os.path.join(charsmap_rules.DIR, name + ".bin"), "--real", name])
+    for name, rules in charsmap_rules.RULES.items():
+        compile_rules(tool, rules, os.path.join(charsmap_rules.DIR, name + ".bin"))
 
 
 def main():
@@ -90,9 +130,12 @@ def main():
         }
     with open(os.path.join(GOLD, "edge_cases.json"), "w") as f:
         json.dump(edge, f)
-    build_space_charsmap()
+    build_charsmaps()
     print("golden fixtures regenerated")
 
 
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["charsmaps"]:
+        build_charsmaps()
+    else:
+        main()
