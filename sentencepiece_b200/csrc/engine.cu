@@ -994,6 +994,9 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
         fprintf(stderr, "[kstats] groups %llu: warp trips/group %.1f, lane trips/sentence %.1f (lane utilisation of K2 %.3f), starts/sentence "
                 "%.1f (whole words %.1f), normalized bytes/sentence %.1f (U+2581 as one byte)\n", ks[12], double(ks[8]) / ks[12], double(ks[9]) / n,
                 double(ks[9]) / (32.0 * ks[8]), double(ks[10]) / n, double(ks[11]) / n, double(ks[13]) / n);
+      if (ks[14])  // K2 runs the end-of-walk block of the parked lanes in warp-uniform start steps
+        fprintf(stderr, "[kstats] start steps/group %.1f, lanes per start step %.1f\n", double(ks[14]) / ks[12],
+                double(ks[10]) / ks[14]);
       if (ks[4]) {
         const double w = 1e-6 / (static_cast<double>(grid) * geom.tiles);
         fprintf(stderr, "[kstats] M cycles per warp (lane 0): group loop %.2f = K1 %.2f, K2 %.2f, K4 %.2f, rest %.2f\n", ks[4] * w,

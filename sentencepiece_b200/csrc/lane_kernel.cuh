@@ -702,6 +702,13 @@ __device__ __forceinline__ bool score_regular(float x) {
   return a == 0u || a - (0x3A800000u << 1) < ((0x48800000u - 0x3A800000u) << 1);  // 2^-10 = 0x3A800000, 2^18 = 0x48800000
 }
 
+// Start steps of the unigram lane kernels' K2: the parked lanes (walk over, end-of-walk block pending) run that block
+// together once at least kParkNum / kParkDen of the warp's live lanes are parked.  park_need(live) is that count,
+// rounded up: 1 <= park_need(live) <= live for live >= 1, and 0 when no lane is live.
+constexpr uint32_t kParkNum = 1, kParkDen = 2;
+static_assert(0 < kParkNum && kParkNum <= kParkDen, "the start step must run at the latest when every live lane is parked");
+__device__ __forceinline__ uint32_t park_need(uint32_t live) { return (live * kParkNum + kParkDen - 1u) / kParkDen; }
+
 constexpr uint32_t kLogWordStep = 1u << 31;  // log entry: the previous logged position is plen bytes back (whole word)
 constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of a little-endian word
 // OneCharLen in the kWsByte spelling: U+2581 is one byte
@@ -756,12 +763,12 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     }
     __syncwarp();
     clk.mark();
-    // ---------------- K2: flat state machine, one trie transition per trip ----------------
-    // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
-    // from the walk position k (low byte first).  ss = ring offset of s's slot.  kb = the byte at k once the walk
-    // has read it (the byte that failed the label test or the child mask), for the word-end test of the start block.
-    uint32_t s = 0, ss = ring_lo, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0, kb = 0;
-    bool has_single = false, done = n == 0;
+    // ---------------- K2: flat state machine, one trie transition per trip (parked-lane schedule, see below) ----------------
+    // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; ch = the byte at the walk position k and `cur`
+    // streams the bytes after it (low byte first).  ss = ring offset of s's slot.  When the walk ends, ch is the byte
+    // that failed the label test or the child mask, for the word-end test of the start step.
+    uint32_t s = 0, ss = ring_lo, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0, ch = 0;
+    bool has_single = false, parked = false;  // the lane is done once s reaches n
     bool wstart = fastwords;  // the shortcut is on and s is the first character of a word (text start or kWsByte)
     float base = 0.f;
     bool base_regular = regular;  // base == 0
@@ -777,89 +784,35 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       return static_cast<unsigned long long>(__funnelshift_r(w2, w3, sh)) |
              (static_cast<unsigned long long>(w3 >> sh) << 32);
     };
-    if (!done) {
+    if (n != 0) {
       for (uint32_t r = 0; r < R; ++r) ring_st_tag(ring_lo + r * kRingSlot + tag_delta, 0xFFFFu);  // no slot belongs to a position of this sentence
       ring_st_score(ring_lo, 0.f);
       w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len_ws1(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
+      ch = static_cast<uint32_t>(cur) & 0xFFu;
+      cur >>= 8;
     }
     // optional counters (engine: SPM_B200_KSTATS; device-resident path only): [8] warp trips, [9] lane trips,
-    // [10] starts retired, [11] whole words, [12] groups, [13] normalized bytes.  The loop counts only the lane's
-    // trips (always: a test would cost more than the add): the warp's trips are their maximum, the starts are the log entries and the whole words the entries with
-    // kLogWordStep.
+    // [10] starts retired, [11] whole words, [12] groups, [13] normalized bytes, [14] start steps.  The loop counts the
+    // lane's trips and the warp's trips and start steps (always: a test would cost more than the add); the starts are the
+    // log entries and the whole words the entries with kLogWordStep.
     const bool kst = B.kstats != nullptr && B.seg_done == nullptr;
-    uint32_t st_lane = 0;
-    while (__any_sync(0xFFFFFFFFu, !done)) {
-      if (!done) {
-        ++st_lane;
-        bool end_walk = true;
-        if (k < n) {
-          const uint32_t d = k - s;
-          uint32_t ch;
-          if (d >= 13u) {  // beyond the register window: long piece, rare
-            ch = lane_text_byte(c, k);
-          } else {
-            if (d == 8u) cur = window_high();
-            ch = static_cast<uint32_t>(cur) & 0xFFu;
-            cur >>= 8;
-          }
-          kb = ch;
-          const uint32_t v = (l >> kLinkBaseShift) ^ ch;
-          const uint4 nd = __ldg(&node4[v]);  // {link, child mask, score, word_safe}: one 16-byte load (L1/L2)
-          if ((nd.x & kLinkLabelMask) == ch) {
-            ++k;
-            l = nd.x;
-            lsafe = nd.w;
-            const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
-            if (kind == kKindNormal || kind == kKindUserDefined) {
-              const uint32_t plen = k - s;
-              uint32_t sl = ss + plen * kRingSlot;
-              if (sl >= ring_hi) sl -= ring_span;
-              const float curs = ring_ld_score(sl);
-              const bool unset = ring_ld_tag(sl + tag_delta) != k;
-              float ns;
-              bool better;
-              if (kind == kKindNormal && base_regular) {
-                // Exact float formulation of the reference's double comparison (Q1).  With
-                // |score|, |base| in {0} U [2^-10, 2^18) the double sum a + b is exact, so
-                // (float)cand == fl(a + b) and cand > cur <=> ns > cur || (ns == cur && err > 0),
-                // err being the exact rounding error of the float add (Knuth two-sum).
-                const float a = __uint_as_float(nd.z);
-                ns = __fadd_rn(a, base);
-                const float bb = __fsub_rn(ns, a);
-                const float err = __fadd_rn(__fsub_rn(a, __fsub_rn(ns, bb)), __fsub_rn(base, bb));
-                better = unset || ns > curs || (ns == curs && err > 0.f);
-              } else {
-                const double sc = kind == kKindNormal
-                                      ? static_cast<double>(__uint_as_float(nd.z))
-                                      : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
-                const double cand = sc + static_cast<double>(base);
-                better = unset || cand > static_cast<double>(curs);
-                ns = static_cast<float>(cand);
-              }
-              if (better) {
-                ring_st_score(sl, ns);
-                ring_st_bp(sl, (plen << 24) | v);
-                ring_st_tag(sl + tag_delta, k);
-              }
-              has_single |= plen == mblen;
-            }
-            // early termination: if the node has no child on the next byte the failing
-            // probe (and its cold miss) is skipped and the start transition happens now
-            if (k < n) {
-              const uint32_t d2 = k - s;
-              if (d2 >= 13u) kb = lane_text_byte(c, k);
-              else kb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
-              end_walk = !((nd.y >> (kb & 31u)) & 1u);
-            }
-          }
-        }
-        if (end_walk) {
+    uint32_t st_lane = 0, st_trips = 0, st_steps = 0;
+    // Schedule: a lane whose walk ends parks (the end-of-walk block is pending), and the parked lanes run that block
+    // together in a warp-uniform start step once there are park_need(live lanes) of them; every live, unparked lane
+    // then takes one trie transition.  Each lane's own sequence of relaxations and log entries is the same as with an
+    // end-of-walk block on every trip, only the trip on which it is issued moves.  need == 0: every lane is done.
+    uint32_t need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
+    while (need != 0) {
+      ++st_trips;
+      if (__popc(__ballot_sync(0xFFFFFFFFu, parked)) >= need) {
+        ++st_steps;
+        if (parked) {
           // the walk from s is over (traverse() == -2, or end of text).  Whole word: the walk covered [s, k) from a
           // word start and ended on a NORMAL piece at the end of the word, early enough to be safe.
-          const bool fast = wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal && (k >= n || kb == kWsByte) &&
+          const bool fast = wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal && (k >= n || ch == kWsByte) &&
                             k <= lsafe;
           const uint32_t s_old = s;
           uint32_t steplog;
@@ -887,9 +840,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
           // position s is final: append (plen | previous char length or whole-word step | unit) to the log
           slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | steplog, c.pol);
           ++nlog;
-          if (s >= n) {
-            done = true;
-          } else {
+          if (s < n) {
             base = ring_ld_score(ss);
             base_regular = regular && score_regular(base);
             // slide the text window so that it is anchored at s; prefetch the new tail word
@@ -906,13 +857,75 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
               w0 = slab_ld(tw + 0, c.pol); w1 = slab_ld(tw + 32, c.pol); w2 = slab_ld(tw + 64, c.pol); w3 = slab_ld(tw + 96, c.pol);
             }
             cur = window_low();
-            const uint32_t b0 = static_cast<uint32_t>(cur) & 0xFFu;
-            wstart = fastwords && b0 == kWsByte;
-            mblen = one_char_len_ws1(b0);
+            ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
+            cur >>= 8;
+            wstart = fastwords && ch == kWsByte;
+            mblen = one_char_len_ws1(ch);
             if (mblen > n - s) mblen = n - s;
             k = s;
             l = root;
             has_single = false;
+          }
+          parked = false;
+        }
+        need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
+      }
+      // walk step: one transition on ch (k < n holds for every live lane here: a walk that reaches n parks)
+      if (s < n && !parked) {
+        ++st_lane;
+        const uint32_t v = (l >> kLinkBaseShift) ^ ch;
+        const uint4 nd = __ldg(&node4[v]);  // {link, child mask, score, word_safe}: one 16-byte load (L1/L2)
+        parked = true;
+        if ((nd.x & kLinkLabelMask) == ch) {
+          ++k;
+          l = nd.x;
+          lsafe = nd.w;
+          const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
+          if (kind == kKindNormal || kind == kKindUserDefined) {
+            const uint32_t plen = k - s;
+            uint32_t sl = ss + plen * kRingSlot;
+            if (sl >= ring_hi) sl -= ring_span;
+            const float curs = ring_ld_score(sl);
+            const bool unset = ring_ld_tag(sl + tag_delta) != k;
+            float ns;
+            bool better;
+            if (kind == kKindNormal && base_regular) {
+              // Exact float formulation of the reference's double comparison (Q1).  With
+              // |score|, |base| in {0} U [2^-10, 2^18) the double sum a + b is exact, so
+              // (float)cand == fl(a + b) and cand > cur <=> ns > cur || (ns == cur && err > 0),
+              // err being the exact rounding error of the float add (Knuth two-sum).
+              const float a = __uint_as_float(nd.z);
+              ns = __fadd_rn(a, base);
+              const float bb = __fsub_rn(ns, a);
+              const float err = __fadd_rn(__fsub_rn(a, __fsub_rn(ns, bb)), __fsub_rn(base, bb));
+              better = unset || ns > curs || (ns == curs && err > 0.f);
+            } else {
+              const double sc = kind == kKindNormal
+                                    ? static_cast<double>(__uint_as_float(nd.z))
+                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
+              const double cand = sc + static_cast<double>(base);
+              better = unset || cand > static_cast<double>(curs);
+              ns = static_cast<float>(cand);
+            }
+            if (better) {
+              ring_st_score(sl, ns);
+              ring_st_bp(sl, (plen << 24) | v);
+              ring_st_tag(sl + tag_delta, k);
+            }
+            has_single |= plen == mblen;
+          }
+          // read the next byte; early termination: if the node has no child on it, the failing
+          // probe (and its cold miss) is skipped and the lane parks now
+          if (k < n) {
+            const uint32_t d = k - s;
+            if (d >= 13u) {  // beyond the register window: long piece, rare
+              ch = lane_text_byte(c, k);
+            } else {
+              if (d == 8u) cur = window_high();
+              ch = static_cast<uint32_t>(cur) & 0xFFu;
+              cur >>= 8;
+            }
+            parked = !((nd.y >> (ch & 31u)) & 1u);
           }
         }
       }
@@ -921,7 +934,6 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       typedef unsigned long long ull;
       uint32_t st_fast = 0;
       for (uint32_t t = 0; t < nlog; ++t) st_fast += slab_ld(c.log + static_cast<size_t>(t) * 32, c.pol) >> 31;
-      const uint32_t st_trips = __reduce_max_sync(0xFFFFFFFFu, st_lane);
       st_lane = __reduce_add_sync(0xFFFFFFFFu, st_lane);
       const uint32_t st_starts = __reduce_add_sync(0xFFFFFFFFu, nlog);
       st_fast = __reduce_add_sync(0xFFFFFFFFu, st_fast);
@@ -929,6 +941,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
       if (lane == 0) {
         atomicAdd(B.kstats + 8, ull(st_trips)); atomicAdd(B.kstats + 9, ull(st_lane)); atomicAdd(B.kstats + 10, ull(st_starts));
         atomicAdd(B.kstats + 11, ull(st_fast)); atomicAdd(B.kstats + 12, ull(1)); atomicAdd(B.kstats + 13, ull(nb));
+        atomicAdd(B.kstats + 14, ull(st_steps));
       }
     }
     clk.mark();
@@ -980,11 +993,11 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
     }
     __syncwarp();
     clk.mark();
-    // ---------------- K2: flat state machine, one trie transition per trip ----------------
-    // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; `cur` streams the bytes
-    // from the walk position k (low byte first).
-    uint32_t s = 0, ss = ring_lo /* ring offset of s's slot */, k = 0, l = root, mblen = 1, nlog = 0;
-    bool has_single = false, done = n == 0;
+    // ---------------- K2: flat state machine, one trie transition per trip (parked-lane schedule) ----------------
+    // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; ch = the byte at the walk position k and `cur`
+    // streams the bytes after it (low byte first).
+    uint32_t s = 0, ss = ring_lo /* ring offset of s's slot */, k = 0, l = root, mblen = 1, nlog = 0, ch = 0;
+    bool has_single = false, parked = false;  // the lane is done once s reaches n
     float base = 0.f;
     bool base_regular = regular;  // base == 0
     uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
@@ -999,77 +1012,21 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
       return static_cast<unsigned long long>(__funnelshift_r(w2, w3, sh)) |
              (static_cast<unsigned long long>(w3 >> sh) << 32);
     };
-    if (!done) {
+    if (n != 0) {
       for (uint32_t r = 0; r < R; ++r) ring_st_bp(ring_lo + r * kPlainRingSlot, 0u);  // all positions unset
       ring_st_score(ring_lo, 0.f);
       w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
+      ch = static_cast<uint32_t>(cur) & 0xFFu;
+      cur >>= 8;
     }
-    while (__any_sync(0xFFFFFFFFu, !done)) {
-      if (!done) {
-        bool end_walk = true;
-        if (k < n) {
-          const uint32_t d = k - s;
-          uint32_t ch;
-          if (d >= 13u) {  // beyond the register window: long piece, rare
-            ch = lane_text_byte(c, k);
-          } else {
-            if (d == 8u) cur = window_high();
-            ch = static_cast<uint32_t>(cur) & 0xFFu;
-            cur >>= 8;
-          }
-          const uint32_t v = (l >> kLinkBaseShift) ^ ch;
-          const uint2 nd = __ldg(&node2[v]);  // {link, child mask}: one 8-byte load (L1/L2)
-          if ((nd.x & kLinkLabelMask) == ch) {
-            ++k;
-            l = nd.x;
-            const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
-            if (kind == kKindNormal || kind == kKindUserDefined) {
-              const uint32_t plen = k - s;
-              uint32_t sl = ss + plen * kPlainRingSlot;
-              if (sl >= ring_hi) sl -= ring_span;
-              const float curs = ring_ld_score(sl);
-              const bool unset = ring_ld_bp(sl) == 0u;
-              float ns;
-              bool better;
-              if (kind == kKindNormal && base_regular) {
-                // Exact float formulation of the reference's double comparison (Q1).  With
-                // |score|, |base| in {0} U [2^-10, 2^18) the double sum a + b is exact, so
-                // (float)cand == fl(a + b) and cand > cur <=> ns > cur || (ns == cur && err > 0),
-                // err being the exact rounding error of the float add (Knuth two-sum).
-                const float a = __uint_as_float(__ldg(M.trie_val + v));
-                ns = __fadd_rn(a, base);
-                const float bb = __fsub_rn(ns, a);
-                const float err = __fadd_rn(__fsub_rn(a, __fsub_rn(ns, bb)), __fsub_rn(base, bb));
-                better = unset || ns > curs || (ns == curs && err > 0.f);
-              } else {
-                const double sc = kind == kKindNormal
-                                      ? static_cast<double>(__uint_as_float(__ldg(M.trie_val + v)))
-                                      : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
-                const double cand = sc + static_cast<double>(base);
-                better = unset || cand > static_cast<double>(curs);
-                ns = static_cast<float>(cand);
-              }
-              if (better) {
-                ring_st_score(sl, ns);
-                ring_st_bp(sl, (plen << 24) | v);
-              }
-              has_single |= plen == mblen;
-            }
-            // early termination: if the node has no child on the next byte the failing
-            // probe (and its cold miss) is skipped and the start transition happens now
-            if (k < n) {
-              uint32_t nb;
-              const uint32_t d2 = k - s;
-              if (d2 >= 13u) nb = lane_text_byte(c, k);
-              else nb = d2 == 8u ? static_cast<uint32_t>(window_high()) & 0xFFu : static_cast<uint32_t>(cur) & 0xFFu;
-              end_walk = !((nd.y >> (nb & 31u)) & 1u);
-            }
-          }
-        }
-        if (end_walk) {
+    // the schedule of encode_unigram_lane_kernel: parked lanes, warp-uniform start steps (park_need)
+    uint32_t need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
+    while (need != 0) {
+      if (__popc(__ballot_sync(0xFFFFFFFFu, parked)) >= need) {
+        if (parked) {
           // the walk from s is over (traverse() == -2, or end of text)
           uint32_t sl = ss + mblen * kPlainRingSlot;
           if (sl >= ring_hi) sl -= ring_span;
@@ -1088,9 +1045,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
           // position s is final: append (plen | previous char length | unit) to the log
           slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | ((mblen - 1u) << 22), c.pol);
           ++nlog;
-          if (s >= n) {
-            done = true;
-          } else {
+          if (s < n) {
             base = ring_ld_score(ss);
             base_regular = regular && score_regular(base);
             // slide the text window so that it is anchored at s; prefetch the new tail word
@@ -1099,11 +1054,71 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
               w3 = slab_ld(c.text_w + static_cast<size_t>((s >> 2) + 3) * 32, c.pol);
             }
             cur = window_low();
-            mblen = one_char_len(static_cast<uint32_t>(cur) & 0xFFu);
+            ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
+            cur >>= 8;
+            mblen = one_char_len(ch);
             if (mblen > n - s) mblen = n - s;
             k = s;
             l = root;
             has_single = false;
+          }
+          parked = false;
+        }
+        need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
+      }
+      // walk step: one transition on ch (k < n holds for every live lane here: a walk that reaches n parks)
+      if (s < n && !parked) {
+        const uint32_t v = (l >> kLinkBaseShift) ^ ch;
+        const uint2 nd = __ldg(&node2[v]);  // {link, child mask}: one 8-byte load (L1/L2)
+        parked = true;
+        if ((nd.x & kLinkLabelMask) == ch) {
+          ++k;
+          l = nd.x;
+          const uint32_t kind = (nd.x >> kLinkKindShift) & 3u;
+          if (kind == kKindNormal || kind == kKindUserDefined) {
+            const uint32_t plen = k - s;
+            uint32_t sl = ss + plen * kPlainRingSlot;
+            if (sl >= ring_hi) sl -= ring_span;
+            const float curs = ring_ld_score(sl);
+            const bool unset = ring_ld_bp(sl) == 0u;
+            float ns;
+            bool better;
+            if (kind == kKindNormal && base_regular) {
+              // Exact float formulation of the reference's double comparison (Q1).  With
+              // |score|, |base| in {0} U [2^-10, 2^18) the double sum a + b is exact, so
+              // (float)cand == fl(a + b) and cand > cur <=> ns > cur || (ns == cur && err > 0),
+              // err being the exact rounding error of the float add (Knuth two-sum).
+              const float a = __uint_as_float(__ldg(M.trie_val + v));
+              ns = __fadd_rn(a, base);
+              const float bb = __fsub_rn(ns, a);
+              const float err = __fadd_rn(__fsub_rn(a, __fsub_rn(ns, bb)), __fsub_rn(base, bb));
+              better = unset || ns > curs || (ns == curs && err > 0.f);
+            } else {
+              const double sc = kind == kKindNormal
+                                    ? static_cast<double>(__uint_as_float(__ldg(M.trie_val + v)))
+                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
+              const double cand = sc + static_cast<double>(base);
+              better = unset || cand > static_cast<double>(curs);
+              ns = static_cast<float>(cand);
+            }
+            if (better) {
+              ring_st_score(sl, ns);
+              ring_st_bp(sl, (plen << 24) | v);
+            }
+            has_single |= plen == mblen;
+          }
+          // read the next byte; early termination: if the node has no child on it, the failing
+          // probe (and its cold miss) is skipped and the lane parks now
+          if (k < n) {
+            const uint32_t d = k - s;
+            if (d >= 13u) {  // beyond the register window: long piece, rare
+              ch = lane_text_byte(c, k);
+            } else {
+              if (d == 8u) cur = window_high();
+              ch = static_cast<uint32_t>(cur) & 0xFFu;
+              cur >>= 8;
+            }
+            parked = !((nd.y >> (ch & 31u)) & 1u);
           }
         }
       }
