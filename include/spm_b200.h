@@ -141,7 +141,11 @@ int spm_encode_ids_device(spm_engine *e, const char *d_bytes, const uint64_t *d_
  * nbest_size is clamped to [1, 1024] like the reference; nbest_size <= 1 gives the Viterbi
  * segmentation with score 0.  Candidate c of sentence i is
  * ids[cand_offsets[i*K + c] .. cand_offsets[i*K + c + 1]) with K = the clamped nbest_size;
- * n_cands[i] tells how many of the K slots are real. */
+ * n_cands[i] tells how many of the K slots are real.
+ * Sentences of any length the encode path takes: sentences the per-lane kernel cannot hold (over
+ * 512 normalized bytes, a lattice over 2112 nodes, a full hypothesis pool or agenda) are computed by
+ * one warp each with 32-bit positions and a pool that grows on demand (counted in
+ * spm_engine_info.last_deferred); device memory is then the only limit. */
 int spm_nbest_encode(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int nbest_size,
                      const int32_t **ids, const uint64_t **cand_offsets, const float **scores,
                      const uint32_t **n_cands);
@@ -169,7 +173,10 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
 /* Replaces SentencePieceProcessor::CalculateEntropy(input, alpha, &entropy)
  * (src/sentencepiece_processor.cc:747-760 -> src/unigram_model.cc:266-291,857-864) for n sentences:
  * entropy[i] of the segmentation lattice of sentence i at inverse temperature alpha (unigram models).
- * Float results agree with the reference to rounding (the device's expf is not glibc's). */
+ * Float results agree with the reference to rounding (the device's expf is not glibc's).
+ * This and the lattice sampling of spm_sample_encode_ids / spm_sample_encode_and_score take
+ * sentences of any length the encode path takes: those over 512 normalized bytes are computed by one
+ * warp each with 32-bit positions (counted in spm_engine_info.last_deferred). */
 int spm_calculate_entropy(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, float alpha,
                           const float **entropy);
 

@@ -331,6 +331,67 @@ struct spm_engine {
   // mode 0: samples >= 1 draws per sentence from the lattice (ids, offsets[n*samples+1], scores); mode 1: entropy
   int run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples);
   int run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total);
+  // Long-sentence path of the lattice and n-best calls: one job per sentence their lane kernels deferred.
+  struct LongJob {
+    uint32_t sent;     // index in the launch
+    uint32_t cap;      // normalized-byte capacity of its slab
+    uint32_t hyp_cap;  // n-best: hypothesis pool
+  };
+  DevBuf<uint32_t> d_long_hyp, d_long_need;
+  static constexpr unsigned long long kLongWaveBytes = 1ull << 30;  // scratch of the long jobs of one launch
+  int read_deferred(uint32_t n_def, const uint64_t *offs, std::vector<LongJob> *jobs);
+  // Runs `jobs` in waves of at most kLongWaveBytes of scratch (a single larger job gets a wave of its own):
+  // slab_bytes(job) sizes a job's slab; launch(LB, m) runs the kernel over the m jobs of the wave in LB.long_list /
+  // long_scratch_off, their pools in d_long_hyp.  A job whose kernel leaves d_long_need[k] != 0 runs again in a later
+  // wave with that pool.  Stops early when the kernel reports an error (h_ctrl32[1]); h_ctrl32 / h_ctrl64 hold the
+  // control words after the last wave.
+  template <typename SlabBytes, typename Launch>
+  int run_long_jobs(std::vector<LongJob> jobs, const KBatch &B, SlabBytes &&slab_bytes, Launch &&launch) {
+    cudaStream_t st = stream;
+    std::vector<uint32_t> list, hyp, need;
+    std::vector<unsigned long long> offs;
+    for (size_t lo = 0; lo < jobs.size();) {
+      size_t hi = lo;
+      offs.assign(1, 0);
+      list.clear();
+      hyp.clear();
+      while (hi < jobs.size() && (hi == lo || offs.back() + slab_bytes(jobs[hi]) <= kLongWaveBytes)) {
+        offs.push_back(offs.back() + slab_bytes(jobs[hi]));
+        list.push_back(jobs[hi].sent);
+        list.push_back(jobs[hi].cap);
+        hyp.push_back(jobs[hi].hyp_cap);
+        ++hi;
+      }
+      const uint32_t m = static_cast<uint32_t>(hi - lo);
+      CUDA_TRY(d_long_scratch.ensure(offs.back() + 256));
+      CUDA_TRY(d_long_list.ensure(2 * static_cast<size_t>(m)));
+      CUDA_TRY(d_long_off.ensure(m + 1));
+      CUDA_TRY(d_long_hyp.ensure(m));
+      CUDA_TRY(d_long_need.ensure(m));
+      CUDA_TRY(cudaMemcpyAsync(d_long_list.p, list.data(), 2ull * m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(d_long_off.p, offs.data(), (m + 1) * sizeof(unsigned long long), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemcpyAsync(d_long_hyp.p, hyp.data(), m * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+      CUDA_TRY(cudaMemsetAsync(d_long_need.p, 0, m * sizeof(uint32_t), st));
+      KBatch LB = B;
+      LB.long_list = d_long_list.p;
+      LB.long_n = m;
+      LB.long_scratch = d_long_scratch.p;
+      LB.long_scratch_off = d_long_off.p;
+      launch(LB, m);
+      CUDA_TRY(cudaGetLastError());
+      ++last_launches;
+      need.resize(m);
+      CUDA_TRY(cudaMemcpyAsync(need.data(), d_long_need.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      if (h_ctrl32.p[1]) return SPM_OK;
+      for (uint32_t k = 0; k < m; ++k)
+        if (need[k]) jobs.push_back(LongJob{jobs[lo + k].sent, jobs[lo + k].cap, need[k]});
+      lo = hi;
+    }
+    return SPM_OK;
+  }
 
   // stats of the last call
   uint64_t last_launches = 0, last_h2d = 0, last_d2h = 0, last_deferred = 0;
@@ -1805,6 +1866,25 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
   return SPM_OK;
 }
 
+// The deferred list of a lattice / n-best lane kernel (n_def {sentence, normalized length or 0} pairs in d_deferred) as
+// long-sentence jobs: the slab holds the exact normalized length when the lane kernel measured it, else the bound from
+// the input length (offs: the launch's host offsets).
+int spm_engine::read_deferred(uint32_t n_def, const uint64_t *offs, std::vector<LongJob> *jobs) {
+  cudaStream_t st = stream;
+  CUDA_TRY(h_deferred.ensure(2 * static_cast<size_t>(n_def)));
+  CUDA_TRY(cudaMemcpyAsync(h_deferred.p, d_deferred.p, 2ull * n_def * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  jobs->clear();
+  for (uint32_t k = 0; k < n_def; ++k) {
+    const uint32_t s = h_deferred.p[2 * k];
+    uint64_t need = h_deferred.p[2 * k + 1];
+    if (need == 0) need = ((offs[s + 1] - offs[s]) * max_expand_num + max_expand_den - 1) / max_expand_den + 8;
+    if (need > 0x7FFFFF00ull) { set_error("sentence too long for the device path"); return SPM_ERR_UNSUPPORTED; }
+    jobs->push_back(LongJob{s, static_cast<uint32_t>(need + 8), 0u});
+  }
+  return SPM_OK;
+}
+
 // ---- n-best (K5): lattice + A* per sentence on the GPU; leaves candidates in the temporary buffers ----
 int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total) {
   cudaStream_t st = stream;
@@ -1828,7 +1908,7 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
   size_t warps_total = static_cast<size_t>(ctas) * warps_per_cta;
   CUDA_TRY(ensure_lane_slabs(warps_total, lane_cap));
   CUDA_TRY(d_nb_scratch.ensure(warps_total * 32 * nbest_lane_bytes(G) + 256));
-  bool grown = false;
+  CUDA_TRY(d_deferred.ensure(2 * n + 2));
   const size_t nc = n * static_cast<size_t>(nbest);
   CUDA_TRY(d_cand_start.ensure(nc));
   CUDA_TRY(d_cand_count.ensure(nc));
@@ -1852,6 +1932,7 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     B.off_hi = ~0ull;
     B.work_counter = d_ctrl32.p + 4;
     B.status = d_ctrl32.p;
+    B.deferred = d_deferred.p;
     NbestOut O{};
     O.tmp_ids = d_tmp_ids.p;
     O.tmp_cap = tmp_cap;
@@ -1871,24 +1952,26 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    if (h_ctrl32.p[3] && !grown) {
-      // some sentence needs a larger lattice / hypothesis pool: rerun the batch with roomy slabs on fewer warps
-      grown = true;
-      G.hyp_cap = std::min<uint32_t>(1u << 20, 8 * G.hyp_cap);
-      G.node_cap = 65535u;
-      G.cap = std::max<uint32_t>(G.cap, 8192u);  // long sentences: text and per-position arrays in roomy slabs
-      warps_per_cta = G.hyp_cap > (1u << 17) ? 1 : 2;
-      ctas = sm_count;
-      warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-      CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
-      CUDA_TRY(d_nb_scratch.ensure(warps_total * 32 * nbest_lane_bytes(G) + 256));
-      continue;
+    last_deferred = h_ctrl32.p[0];
+    if (h_ctrl32.p[0] && !h_ctrl32.p[1]) {
+      // ---- sentences the lane kernel deferred (long, large lattice, pool or agenda full): warp per sentence ----
+      std::vector<LongJob> jobs;
+      { const int rc = read_deferred(h_ctrl32.p[0], offsets, &jobs); if (rc) return rc; }
+      const uint32_t mm1 = trie.max_matches_per_start + 1;
+      for (LongJob &j : jobs) {
+        if (nbest_long_nodes(j.cap, mm1) > 0xFFFFFF00ull) { set_error("sentence too long for the device path"); return SPM_ERR_UNSUPPORTED; }
+        j.hyp_cap = static_cast<uint32_t>(std::min<unsigned long long>(4ull * j.cap + 16384ull + 64ull * nbest, 0xFFFFFF00ull));
+      }
+      const int rc = run_long_jobs(
+          jobs, B, [&](const LongJob &j) { return nbest_long_bytes(j.cap, mm1, j.hyp_cap, G.heap_cap); },
+          [&](const KBatch &LB, uint32_t m) {
+            const int lgrid = static_cast<int>(std::min<uint32_t>((m + 7) / 8, static_cast<uint32_t>(sm_count) * 4));
+            nbest_long_kernel<<<lgrid, 256, 0, st>>>(km, LB, O, d_long_hyp.p, d_long_need.p, mm1, G.heap_cap, nbest);
+          });
+      if (rc) return rc;
     }
-    if (h_ctrl32.p[3]) {
-      set_error("n-best: a sentence exceeds the device path's capacity (normalized length > " + std::to_string(G.cap) +
-                " bytes, lattice or hypothesis pool too large)");
-      return SPM_ERR_UNSUPPORTED;
-    }
+    if (h_ctrl32.p[1] & 8u) { set_error("n-best: a long sentence normalized to more bytes than the scratch sized for it"); return SPM_ERR_ENCODE; }
+    if (h_ctrl32.p[1] & 16u) { set_error("n-best: a lattice exceeds the sizes the model's trie implies"); return SPM_ERR_ENCODE; }
     if (h_ctrl32.p[1]) { set_error("n-best: internal consistency check failed"); return SPM_ERR_ENCODE; }
     if (h_ctrl32.p[2]) { tmp_cap = h_ctrl64.p[0] + 1024; continue; }
     *tmp_total = h_ctrl64.p[0];
@@ -1915,7 +1998,10 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
   G.cap = lane_cap;
   G.node_cap = lane_cap * (trie.max_matches_per_start + 1) + 64;
   constexpr size_t kChunk = 32768;
-  int warps_per_cta = 8;
+  const int warps_per_cta = 8;
+  const uint32_t mm1 = trie.max_matches_per_start + 1;
+  uint64_t deferred = 0;
+  CUDA_TRY(d_deferred.ensure(2 * std::min(n, kChunk) + 2));
   last_launches = 0;
   last_h2d = last_d2h = 0;
   float main_ms = 0.f;
@@ -1932,8 +2018,8 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
     CUDA_TRY(cudaMemcpyAsync(d_offsets.p, offsets + lo, (m + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
     last_h2d += chunk_bytes + (m + 1) * sizeof(uint64_t);
     const size_t groups = (m + 31) / 32;
-    int ctas = static_cast<int>(std::min<size_t>(sm_count, (groups + warps_per_cta - 1) / warps_per_cta));
-    size_t warps_total = static_cast<size_t>(ctas) * warps_per_cta;
+    const int ctas = static_cast<int>(std::min<size_t>(sm_count, (groups + warps_per_cta - 1) / warps_per_cta));
+    const size_t warps_total = static_cast<size_t>(ctas) * warps_per_cta;
     CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
     CUDA_TRY(d_lat_scratch.ensure(warps_total * 32 * lattice_lane_bytes(G) + 256));
     CUDA_TRY(d_lat_node_start.ensure(m));
@@ -1956,6 +2042,7 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
       B.off_hi = ~0ull;
       B.work_counter = d_ctrl32.p + 4;
       B.status = d_ctrl32.p;
+      B.deferred = d_deferred.p;
       LatticeOut O{};
       O.nodes = d_lat_nodes.p;
       O.pos = d_lat_pos.p;
@@ -1978,23 +2065,23 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
       CUDA_TRY(cudaStreamSynchronize(st));
       float a = 0.f;
       if (cudaEventElapsedTime(&a, ev[0], ev[1]) == cudaSuccess) main_ms += a;
-      if (h_ctrl32.p[3] && G.cap < 8192u) {
-        // a long sentence: this and the later chunks run with roomy per-lane slabs on fewer warps
-        G.cap = 8192u;
-        G.node_cap = G.cap * (trie.max_matches_per_start + 1) + 64;
-        warps_per_cta = 2;
-        ctas = static_cast<int>(std::min<size_t>(sm_count, (groups + warps_per_cta - 1) / warps_per_cta));
-        warps_total = static_cast<size_t>(ctas) * warps_per_cta;
-        CUDA_TRY(ensure_lane_slabs(warps_total, G.cap));
-        CUDA_TRY(d_lat_scratch.ensure(warps_total * 32 * lattice_lane_bytes(G) + 256));
-        --attempt;
-        continue;
+      const uint32_t n_def = h_ctrl32.p[0];
+      if (n_def && !h_ctrl32.p[1]) {
+        // ---- sentences the lane kernel deferred (long, large lattice): warp per sentence ----
+        std::vector<LongJob> jobs;
+        { const int rc = read_deferred(n_def, offsets + lo, &jobs); if (rc) return rc; }
+        const int rc = run_long_jobs(
+            jobs, B, [&](const LongJob &j) { return lattice_long_bytes(j.cap, mm1); },
+            [&](const KBatch &LB, uint32_t nj) {
+              const int lgrid = static_cast<int>(std::min<uint32_t>((nj + 7) / 8, static_cast<uint32_t>(sm_count) * 4));
+              lattice_long_kernel<<<lgrid, 256, 0, st>>>(km, LB, O, mm1, inv_theta, mode);
+            });
+        if (rc) return rc;
       }
-      if (h_ctrl32.p[3]) {
-        set_error("lattice: a sentence exceeds the device path's capacity (normalized length > " + std::to_string(G.cap) + " bytes)");
-        return SPM_ERR_UNSUPPORTED;
-      }
+      if (h_ctrl32.p[1] & 8u) { set_error("lattice: a long sentence normalized to more bytes than the scratch sized for it"); return SPM_ERR_ENCODE; }
+      if (h_ctrl32.p[1]) { set_error("lattice: a lattice exceeds the sizes the model's trie implies"); return SPM_ERR_ENCODE; }
       if (h_ctrl32.p[2] && attempt == 0) { node_cap = h_ctrl64.p[0] + 1024; continue; }
+      deferred += n_def;
       if (h_ctrl32.p[2]) { set_error("lattice: output buffer overflow persisted"); return SPM_ERR_CAPACITY; }
       break;
     }
@@ -2035,13 +2122,13 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
             probs.clear();
             for (uint32_t q = q0; q < q1; ++q) {
               float sc; memcpy(&sc, &nodes[q].y, 4);
-              const float arg = A(nodes[q].z & 0xFFFFu) + inv_theta * sc - Z;   // float expression (:528-529)
+              const float arg = A(nodes[q].z) + inv_theta * sc - Z;   // float expression (:528-529)
               probs.push_back(static_cast<float>(std::exp(static_cast<double>(arg))));
             }
             std::discrete_distribution<int> dist(probs.begin(), probs.end());
             const uint32_t q = q0 + static_cast<uint32_t>(dist(rng));
             path.push_back(q);
-            p = nodes[q].z & 0xFFFFu;
+            p = nodes[q].z;
             Z = A(p);
           }
           // id path of PopulateSentencePieceText over the sampled nodes, left to right
@@ -2078,6 +2165,7 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
   }
   last_main_ms = main_ms;
   last_ms = main_ms;
+  last_deferred = deferred;
   return SPM_OK;
 }
 

@@ -540,14 +540,16 @@ __device__ __forceinline__ unsigned long long lane_claim_output(const KBatch &B,
 // NORMAL or USER_DEFINED piece that begins there, shortest first -- length in characters (get_chars_length, :548-552),
 // trie unit, score (USER_DEFINED: float(double(length * max_score) - 0.1)).  piece returns false when the lattice is
 // full, which ends the walk.  Returns whether a one-character piece was found (if not, the caller adds the UNK node).
-template <typename F>
-__device__ __forceinline__ bool lane_populate_from(const KModel &M, const LaneCtx &c, uint32_t root, const uint16_t *surf,
-                                                   uint32_t bp, uint32_t n, F &&piece) {
+// populate_from reads byte k of the normalized text as text_byte(k) and character offsets from surf (16-bit in the
+// lane kernels' slabs, 32-bit on the long-sentence path).
+template <typename TextByte, typename SurfT, typename F>
+__device__ __forceinline__ bool populate_from(const KModel &M, TextByte &&text_byte, uint32_t root, const SurfT *surf,
+                                              uint32_t bp, uint32_t n, F &&piece) {
   bool has_single = false;
   uint32_t l = root;
   uint32_t clen = 0;  // characters completed so far
   for (uint32_t kpos = surf[bp]; kpos < n; ++kpos) {
-    const uint32_t ch = lane_text_byte_plain(c, kpos);
+    const uint32_t ch = text_byte(kpos);
     const uint32_t v = (l >> kLinkBaseShift) ^ ch;
     l = __ldg(&M.trie_node2[v]).x;
     if ((l & kLinkLabelMask) != ch) break;
@@ -562,6 +564,42 @@ __device__ __forceinline__ bool lane_populate_from(const KModel &M, const LaneCt
     has_single |= length == 1;
   }
   return has_single;
+}
+template <typename F>
+__device__ __forceinline__ bool lane_populate_from(const KModel &M, const LaneCtx &c, uint32_t root, const uint16_t *surf,
+                                                   uint32_t bp, uint32_t n, F &&piece) {
+  return populate_from(M, [&](uint32_t k) { return lane_text_byte_plain(c, k); }, root, surf, bp, n, piece);
+}
+
+// A sentence a lattice / n-best lane kernel leaves to the long-sentence path: (sentence, exact normalized length or 0
+// when unknown) in B.deferred, counted in B.status[0].
+__device__ __forceinline__ void lane_defer_long(const KBatch &B, uint32_t sent, uint32_t need) {
+  const uint32_t slot = atomicAdd(B.status, 1u);
+  B.deferred[2 * slot] = sent;
+  B.deferred[2 * slot + 1] = need;
+}
+
+// Character starts of a normalized text on the long-sentence path: surf[c] = byte offset of character c (the
+// sequential walk of Lattice::SetSentence, p += one_char_len(text[p]) clipped at n), surf[L] = n.  Warp-collective, 32
+// bytes per step: the lanes' character lengths go into two ballots and every lane follows the same jumps.  Returns L.
+__device__ __forceinline__ uint32_t long_char_starts(const uint8_t *text, uint32_t n, uint32_t *surf, uint32_t lane) {
+  uint32_t L = 0, carry = 0;  // carry: first character start of the window, relative to it
+  for (uint32_t w0 = 0; w0 < n; w0 += 32) {
+    const uint32_t q = w0 + lane;
+    const uint32_t len1 = q < n ? one_char_len(text[q]) - 1u : 0u;
+    const uint32_t b0 = __ballot_sync(0xFFFFFFFFu, len1 & 1u), b1 = __ballot_sync(0xFFFFFFFFu, len1 & 2u);
+    uint32_t starts = 0, p = carry;
+    while (p < 32u && w0 + p < n) {
+      starts |= 1u << p;
+      p += 1u + ((b0 >> p) & 1u) + (((b1 >> p) & 1u) << 1);
+    }
+    carry = p - 32u;  // the sentence ends inside the window when w0 + p >= n: no later window
+    if ((starts >> lane) & 1u) surf[L + __popc(starts & ((1u << lane) - 1u))] = q;
+    L += __popc(starts);
+  }
+  if (lane == 0) surf[L] = n;
+  __syncwarp();
+  return L;
 }
 
 // K4: back-trace + id path of PopulateSentencePieceText (sentencepiece_processor.cc:547-636) over a lane's
