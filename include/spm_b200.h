@@ -87,6 +87,24 @@ int spm_engine_set_types(spm_engine *e, const uint8_t *types);
  * from earlier batches; spm_engine_set_types empties the tables as well. */
 int spm_engine_cache_reset(spm_engine *e);
 
+/* The id effect of the encode extra options: SentencePieceProcessor::ApplyExtraOptions
+ * (src/sentencepiece_processor.cc:1019-1064) after SetEncodeExtraOptions, and the Python binding's
+ * encode(add_bos=, add_eos=, reverse=) (python/src/sentencepiece/sentencepiece.i:138-145).  Any list of
+ * REVERSE / BOS / EOS options applied in order turns a sentence's ids r into
+ *   prefix ++ (reverse ? reversed(r) : r) ++ suffix
+ * with constant id lists: BOS prepends to the prefix, EOS appends to the suffix, REVERSE swaps the two, reverses
+ * both and flips `reverse`.  UNK_PIECE changes piece strings only.  Parsing option strings and looking up the
+ * bos / eos pieces stay with the caller.
+ * The frame is engine state, like the live types: every later call that returns encode ids writes it, until it is
+ * set again; all zeros / NULL restores the plain output.  It applies to spm_encode_ids, spm_encode_ids_device
+ * (total_ids and the SPM_ERR_CAPACITY answer include it), every candidate of spm_nbest_encode, spm_sample_encode_ids
+ * and every sample of spm_sample_encode_and_score.  Empty sentences are framed too, as the reference frames the empty
+ * encode; the exception is spm_sample_encode_and_score, where the reference returns no sample for an empty sentence
+ * and its slots stay empty.  spm_encode_spans keeps returning the raw segmentation, on which tok_end is defined.
+ * Every id must lie in [0, vocab) and n_prefix, n_suffix <= 64, else SPM_ERR_ARG. */
+int spm_engine_set_encode_frame(spm_engine *e, const int32_t *prefix, uint32_t n_prefix, int reverse,
+                                const int32_t *suffix, uint32_t n_suffix);
+
 /* Text of the last failure on this engine (or of the last failed create when
  * e == NULL).  Never NULL. */
 const char *spm_last_error(const spm_engine *e);
@@ -113,7 +131,8 @@ int spm_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offsets, si
  * its exclusive end offset in the sentence's normalized text, the normalized
  * text itself and the normalized->original byte alignment (norm_to_orig,
  * src/normalizer.cc:181-183; norm_offsets[i+1]-norm_offsets[i]+1 entries per
- * sentence, stored at n2o[norm_offsets[i] + i ...]). */
+ * sentence, stored at n2o[norm_offsets[i] + i ...]).  The ids are the raw segmentation, on which tok_end is defined:
+ * the encode frame (spm_engine_set_encode_frame) is not applied here. */
 int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n,
                      const int32_t **ids, const uint32_t **tok_end, const uint64_t **id_offsets,
                      const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o);

@@ -15,7 +15,7 @@ EXPORTS = [
     "spm_last_error", "spm_encode_ids", "spm_encode_spans", "spm_encode_ids_device", "spm_host_alloc",
     "spm_host_free", "spm_engine_get_info", "spm_engine_set_tuning", "spm_nbest_encode", "spm_set_random_seed",
     "spm_sample_encode_ids", "spm_decode_ids", "spm_engine_set_unk_surface", "spm_calculate_entropy",
-    "spm_sample_encode_and_score", "spm_engine_cache_reset",
+    "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame",
 ]
 
 
@@ -59,6 +59,7 @@ def load():
     L.spm_engine_destroy.restype = None
     L.spm_engine_set_types.argtypes = [vp, vp]
     L.spm_engine_cache_reset.argtypes = [vp]
+    L.spm_engine_set_encode_frame.argtypes = [vp, vp, ctypes.c_uint32, ctypes.c_int, vp, ctypes.c_uint32]
     L.spm_last_error.argtypes = [vp]
     L.spm_last_error.restype = cp
     L.spm_encode_ids.argtypes = [vp, vp, vp, sz, P(vp), P(vp)]

@@ -53,3 +53,46 @@ def pieces_and_unk(data):
         else:
             raise ValueError("unsupported wire type in ModelProto")
     return pieces, unk
+
+
+def _fields(b, p, end):
+    """(field number, wire type, value) of a message: bytes for length-delimited fields, int for varints."""
+    while p < end:
+        key, p = _varint(b, p)
+        fno, wt = key >> 3, key & 7
+        if wt == 2:
+            ln, p = _varint(b, p)
+            yield fno, wt, b[p:p + ln]
+            p += ln
+        elif wt == 0:
+            v, p = _varint(b, p)
+            yield fno, wt, v
+        elif wt == 5:
+            p += 4
+        elif wt == 1:
+            p += 8
+        else:
+            raise ValueError("unsupported wire type in ModelProto")
+
+
+def special_pieces(data):
+    """TrainerSpec unk_piece / bos_piece / eos_piece (sentencepiece_model.proto:220-222, field 2 of ModelProto) and
+    their ids as the reference's bos_id() / eos_id() see them: PieceToId of the piece (the first definition wins,
+    model_interface.cc:51-61), -1 when that is the unknown id (the piece is not defined)."""
+    names = {45: "<unk>", 46: "<s>", 47: "</s>"}
+    for fno, wt, v in _fields(data, 0, len(data)):
+        if fno == 2 and wt == 2:
+            for f2, w2, v2 in _fields(v, 0, len(v)):
+                if f2 in names and w2 == 2:
+                    names[f2] = v2.decode("utf-8", errors="replace")
+    pieces, unk = pieces_and_unk(data)
+    first = {}
+    for i, p in enumerate(pieces):
+        first.setdefault(p, i)
+
+    def piece_id(p):
+        i = first.get(p, unk)
+        return -1 if i == unk else i
+
+    return dict(unk_piece=names[45], bos_piece=names[46], eos_piece=names[47],
+                bos_id=piece_id(names[46]), eos_id=piece_id(names[47]))

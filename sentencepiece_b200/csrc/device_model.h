@@ -78,6 +78,30 @@ struct KModel {
   int32_t model_type;
 };
 
+// The id effect of the encode extra options (spm_engine_set_encode_frame): every id list the final writers produce
+// becomes P ++ (body, or body reversed) ++ S.  np = ns = 0 is the plain output.
+struct KFrame {
+  const int32_t *ids;      // device memory: the np ids of P, then the ns ids of S
+  uint32_t np, ns;
+  uint32_t reverse;
+  // n-best compaction: item j is slot j % per of sentence j / per, and only the first n_real[j / per] slots hold
+  // candidates; the empty slots stay empty.  null = every item is framed.
+  const uint32_t *n_real;
+  uint32_t per;
+  __host__ __device__ __forceinline__ bool active() const { return np + ns + reverse != 0u; }
+  __device__ __forceinline__ uint32_t added(uint32_t j) const {
+    return (!n_real || j % per < n_real[j / per]) ? np + ns : 0u;
+  }
+  // id t (< np + body + ns) of a framed list whose `body` ids load(k) reads in their raw order
+  template <typename Load>
+  __device__ __forceinline__ int32_t at(uint32_t body, uint32_t t, Load load) const {
+    if (t < np) return ids[t];
+    t -= np;
+    if (t < body) return load(reverse ? body - 1u - t : t);
+    return ids[np + t - body];
+  }
+};
+
 // One batch.
 struct KBatch {
   const uint8_t *bytes;
@@ -107,6 +131,7 @@ struct KBatch {
   uint32_t *drained_upto;
   unsigned long long *host_progress;
   unsigned long long *kstats;         // [4] cycles (lane 0 of each warp): input wait, compaction, look-back wait, groups; or null
+  KFrame frame;                       // fused path: the frame the compaction writes around every sentence's ids
   // outputs of the encode kernel
   int32_t *tmp_ids;              // ids in completion order
   uint32_t *tmp_tok_end;         // (spans) token end offsets in normalized text, same positions

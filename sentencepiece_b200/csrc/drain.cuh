@@ -13,7 +13,8 @@
 //      segment's first output position.  An earlier segment that is not finished yet is waited for:
 //      one warp per finished-but-blocked segment (at most the segments of a piece or two) spins
 //      while the other resident warps keep taking groups, so the wait always ends;
-//   3. id_offsets (to pinned host memory) and the ids (to the device result buffer) are written;
+//   3. id_offsets (to pinned host memory) and the ids (to the device result buffer) are written; with an encode frame
+//      (KFrame) every sentence counts |P| + |S| more and its ids are written between P and S, reversed if asked;
 //   4. the run of finished segments is extended and its id count stored to a pinned host word: the
 //      host polls it and fetches the finished prefix with the copy engine while later segments are
 //      still being encoded (SM stores over PCIe reach only ~25 GB/s, the copy engine ~55 GB/s).
@@ -79,9 +80,10 @@ __device__ __forceinline__ void drain_publish(const KBatch &B, uint32_t seg, uin
   const uint32_t seg_n = min(B.n - seg_lo, 1u << B.seg_shift);
   // ---- 1. scan of the counts; relative offsets parked in sent_rel ----
   uint32_t run = 0;
+  const uint32_t framed = B.frame.np + B.frame.ns;  // ids the encode frame adds to every sentence
   for (uint32_t j = 0; j < seg_n; j += 32) {
     const uint32_t i = seg_lo + j + lane;
-    const uint32_t cnt = j + lane < seg_n ? __ldcg(B.sent_count + i) : 0u;
+    const uint32_t cnt = j + lane < seg_n ? __ldcg(B.sent_count + i) + framed : 0u;
     uint32_t incl = cnt;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) {
@@ -157,6 +159,18 @@ __device__ __forceinline__ void drain_finish(const KBatch &B, uint32_t seg, uint
       B.out_offsets[i] = B.out_off_base + dst;
     }
     if (!room) continue;
+    if (B.frame.active()) {
+      // framed: P, the sentence's ids (backwards under reverse), S -- one sentence per step
+      const uint32_t tot = have ? cnt + B.frame.np + B.frame.ns : 0u;
+#pragma unroll 1
+      for (uint32_t k = 0; k < 32; ++k) {
+        const unsigned long long s = __shfl_sync(0xFFFFFFFFu, src, k), d = __shfl_sync(0xFFFFFFFFu, dst, k);
+        const uint32_t c = __shfl_sync(0xFFFFFFFFu, cnt, k), m = __shfl_sync(0xFFFFFFFFu, tot, k);
+        for (uint32_t r = lane; r < m; r += 32)
+          B.out_ids[d + r] = B.frame.at(c, r, [&](uint32_t q) { return __ldcg(B.tmp_ids + s + q); });
+      }
+      continue;
+    }
     // one sentence per step: its ids are contiguous on both sides -> coalesced 128-byte loads and stores; four
     // sentences are in flight at a time so that the loads overlap
 #pragma unroll 1

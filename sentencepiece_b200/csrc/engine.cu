@@ -328,8 +328,11 @@ struct spm_engine {
   std::vector<int32_t> lat_ids;          // results of the last lattice sampling call
   std::vector<uint64_t> lat_offsets;
   std::vector<float> lat_scores;
-  // mode 0: samples >= 1 draws per sentence from the lattice (ids, offsets[n*samples+1], scores); mode 1: entropy
-  int run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples);
+  // mode 0: samples >= 1 draws per sentence from the lattice (ids, offsets[n*samples+1], scores), each with the encode
+  // frame -- also the draw of an empty sentence when frame_empty (SampleEncode frames its empty result; an empty
+  // sentence has no samples in SampleEncodeAndScore); mode 1: entropy
+  int run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples,
+                  bool frame_empty = false);
   int run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total);
   // Long-sentence path of the lattice and n-best calls: one job per sentence their lane kernels deferred.
   struct LongJob {
@@ -392,6 +395,17 @@ struct spm_engine {
     }
     return SPM_OK;
   }
+
+  // encode frame (spm_engine_set_encode_frame): the ids of P then S, on the host and where the writers read them
+  static constexpr uint32_t kMaxFrame = 64;
+  std::vector<int32_t> frame_ids;
+  uint32_t frame_np = 0, frame_ns = 0;
+  bool frame_rev = false;
+  DevBuf<int32_t> d_frame;
+  KFrame kframe(const uint32_t *n_real = nullptr, uint32_t per = 1) const {
+    return KFrame{d_frame.p, frame_np, frame_ns, frame_rev ? 1u : 0u, n_real, per};
+  }
+  bool framed() const { return frame_np + frame_ns != 0 || frame_rev; }
 
   // stats of the last call
   uint64_t last_launches = 0, last_h2d = 0, last_d2h = 0, last_deferred = 0;
@@ -1165,10 +1179,11 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     break;
   }
   if (h_ctrl32.p[2]) { set_error("temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
-  // ---- offsets (exclusive scan) + compaction into sentence order ----
+  // ---- offsets (exclusive scan) + compaction into sentence order; ids (not spans) get the encode frame ----
+  const bool framed_ids = !spans && framed();
   const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
   CUDA_TRY(d_block_sums.ensure(nb + 1));
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, 0);
+  scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, framed_ids ? frame_np + frame_ns : 0u);
   scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_ctrl64.p + 2);
   CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
@@ -1190,10 +1205,15 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     set_error("ids_capacity too small: need " + std::to_string(tot));
     return SPM_ERR_CAPACITY;
   }
-  scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, off_out, d_sent_start.p,
-                                                        d_tmp_ids.p, ids_out,
-                                                        spans ? d_tmp_tok_end.p : nullptr, spans ? d_tok_end.p : nullptr,
-                                                        user_ids_cap, 0, off_base);
+  if (framed_ids)
+    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, off_out, d_sent_start.p,
+                                                                d_tmp_ids.p, ids_out, nullptr, nullptr, user_ids_cap, 0,
+                                                                off_base, kframe());
+  else
+    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, off_out, d_sent_start.p,
+                                                          d_tmp_ids.p, ids_out,
+                                                          spans ? d_tmp_tok_end.p : nullptr, spans ? d_tok_end.p : nullptr,
+                                                          user_ids_cap, 0, off_base);
   last_launches += 3;
   if (spans) {
     const unsigned long long tn = h_ctrl64.p[1];  // sum(n_i + 1)
@@ -1293,7 +1313,7 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
   const uint64_t total_bytes = offsets[n] - offsets[0];
   CUDA_TRY(h_id_offsets.ensure(n + 1));
   // ids are not known in advance: start from the running average (or 1 id per 3 bytes) and grow
-  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 3 + 2 * n + 4096)));
+  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 3 + (2 + frame_np + frame_ns) * n + 4096)));
   uint64_t max_chunk_bytes = 0;
   for (size_t c = 0; c < C; ++c) {
     const size_t lo = c * chunk, hi = std::min(n, lo + chunk);
@@ -1388,7 +1408,7 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
   CUDA_TRY(d_ready.ensure(4));
   CUDA_TRY(h_marks.ensure(P + 1));
   CUDA_TRY(h_id_offsets.ensure(n + 1));
-  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 3 + 2 * n + 4096)));
+  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 3 + (2 + frame_np + frame_ns) * n + 4096)));
   // ---- queue the whole input ----
   CUDA_TRY(cudaMemsetAsync(d_ready.p, 0, sizeof(uint32_t), s_h2d));
   CUDA_TRY(cudaMemcpyAsync(s_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, s_h2d));
@@ -1479,7 +1499,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(d_ready.ensure(4));
   CUDA_TRY(h_marks.ensure(P + 1));
   CUDA_TRY(h_id_offsets.ensure(n + 1));
-  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 2 + 2 * n + 4096)));
+  CUDA_TRY(h_ids.ensure(std::max<size_t>(h_ids.cap, total_bytes / 2 + (2 + frame_np + frame_ns) * n + 4096)));
   const unsigned long long tmp_cap = total_bytes + 4ull * n + 1024;
   CUDA_TRY(d_tmp_ids.ensure(tmp_cap));
   CUDA_TRY(d_sent_start.ensure(n));
@@ -1555,6 +1575,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   B.out_cap = std::min<unsigned long long>(h_ids.cap, d_ids.cap);
   B.out_off_base = 0;
   B.kstats = trace ? d_ctrl64.p + 4 : nullptr;
+  B.frame = kframe();
   CUDA_TRY(cudaEventRecord(ev[0], st));
   // processing order: sorted within each drain segment.  Sorting whole input pieces instead makes all 32 segments of a
   // piece finish in the same last few groups, whose warps then compact them one after the other, which serializes the
@@ -1985,7 +2006,8 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
 //      chunks of sentences; mode 0 then draws on the host exactly as Lattice::Sample (unigram_model.cc:511-542) does
 //      -- std::exp in double, std::discrete_distribution<int> over float probabilities, this engine's std::mt19937 --
 //      for the sentences in order, which reproduces the reference's single-threaded stream under a seed ----
-int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples) {
+int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples,
+                            bool frame_empty) {
   cudaStream_t st = stream;
   lat_ids.clear();
   lat_scores.clear();
@@ -2110,8 +2132,11 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
       const uint32_t L = h_lat_nchars.p[i];
       const uint4 *nodes = h_lat_nodes.p + h_lat_node_start.p[i];
       const uint2 *pos = h_lat_pos.p + h_lat_pos_start.p[i];
+      const bool frame_it = framed() && (L || frame_empty);
       for (int sidx = 0; sidx < samples; ++sidx) {
         float score = 0.f;
+        if (frame_it) lat_ids.insert(lat_ids.end(), frame_ids.begin(), frame_ids.begin() + frame_np);
+        const size_t body = lat_ids.size();
         if (L) {
           auto A = [&](uint32_t p) { float f; memcpy(&f, &pos[p].x, 4); return f; };
           path.clear();
@@ -2157,6 +2182,10 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
             prev_unk = isunk;
           }
           score -= A(L);  // - marginal (:853)
+        }
+        if (frame_it) {  // the score stays the raw path's, as in the reference
+          if (frame_rev) std::reverse(lat_ids.begin() + body, lat_ids.end());
+          lat_ids.insert(lat_ids.end(), frame_ids.begin() + frame_np, frame_ids.end());
         }
         lat_offsets.push_back(lat_ids.size());
         lat_scores.push_back(score);
@@ -2286,6 +2315,7 @@ void spm_engine_destroy(spm_engine *e) {
   e->d_dec_off.release(); e->d_dec_info.release(); e->d_dec_bytes.release(); e->d_dec_tmp.release(); e->d_dec_text.release();
   e->d_dec_ids.release(); e->d_dec_text_offsets.release(); e->h_dec_text.release(); e->h_dec_text_offsets.release();
   for (int k = 0; k < 2; ++k) { e->p_dec_ids[k].release(); e->p_dec_text[k].release(); e->p_dec_toff[k].release(); e->h_stage[k].release(); }
+  e->d_frame.release();
   e->d_order.release(); e->d_order_hist.release(); e->d_seg_done.release(); e->d_sent_rel.release(); e->d_seg_words.release();
   if (e->ev_offs) cudaEventDestroy(e->ev_offs);
   if (e->s_h2d) cudaStreamDestroy(e->s_h2d);
@@ -2328,6 +2358,36 @@ int spm_engine_cache_reset(spm_engine *e) {
 }
 
 static void finish_timing(spm_engine *e);
+
+int spm_engine_set_encode_frame(spm_engine *e, const int32_t *prefix, uint32_t n_prefix, int reverse, const int32_t *suffix,
+                                uint32_t n_suffix) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (n_prefix > spm_engine::kMaxFrame || n_suffix > spm_engine::kMaxFrame) {
+    set_error("spm_engine_set_encode_frame: at most " + std::to_string(spm_engine::kMaxFrame) + " ids before and " +
+              std::to_string(spm_engine::kMaxFrame) + " after a sentence");
+    return SPM_ERR_ARG;
+  }
+  if ((n_prefix && !prefix) || (n_suffix && !suffix)) { set_error("spm_engine_set_encode_frame: null ids"); return SPM_ERR_ARG; }
+  std::vector<int32_t> ids;
+  if (n_prefix) ids.assign(prefix, prefix + n_prefix);
+  if (n_suffix) ids.insert(ids.end(), suffix, suffix + n_suffix);
+  const int32_t V = e->model.vocab_size();
+  for (const int32_t id : ids)
+    if (id < 0 || id >= V) {
+      set_error("spm_engine_set_encode_frame: id " + std::to_string(id) + " is outside [0, " + std::to_string(V) + ")");
+      return SPM_ERR_ARG;
+    }
+  CUDA_TRY(cudaSetDevice(e->device));
+  CUDA_TRY(e->d_frame.ensure(ids.size() + 1));
+  if (!ids.empty()) CUDA_TRY(cudaMemcpy(e->d_frame.p, ids.data(), ids.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+  e->frame_ids = std::move(ids);
+  e->frame_np = n_prefix;
+  e->frame_ns = n_suffix;
+  e->frame_rev = reverse != 0;
+  return SPM_OK;
+}
 
 int spm_engine_set_unk_surface(spm_engine *e, const char *surface, size_t bytes) {
   if (!e || (!surface && bytes)) return SPM_ERR_ARG;
@@ -2677,27 +2737,41 @@ int spm_nbest_encode(spm_engine *e, const char *bytes, const uint64_t *offsets, 
   }
   uint64_t tmp_total = 0;
   { const int rc = e->run_nbest(bytes, offsets, n, K, &tmp_total); if (rc) return rc; }
-  // candidate-major compaction: the shared scan + gather over n*K counts
+  // candidate-major compaction: the shared scan + gather over n*K counts; every candidate gets the encode frame
   const uint32_t nc32 = static_cast<uint32_t>(nc);
   const uint32_t nb = (nc32 + kScanChunk - 1) / kScanChunk;
+  const bool framed = e->framed();
+  const KFrame F = e->kframe(e->d_n_cands.p, K);
   CUDA_TRY(e->d_block_sums.ensure(nb + 1));
   CUDA_TRY(e->d_cand_offsets.ensure(nc + 1));
-  CUDA_TRY(e->d_ids.ensure(tmp_total + 1));
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, 0);
+  if (framed) scan_block_sums_kernel<true><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, 0, F);
+  else scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, 0);
   scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
-  scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, e->d_cand_offsets.p,
-                                                        e->d_cand_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
-                                                        e->d_ids.cap, 0, 0ull);
+  uint64_t total = tmp_total;
+  if (framed) {  // the frame's share depends on the candidate counts: read the total
+    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    total = e->h_ctrl64.p[2];
+  }
+  CUDA_TRY(e->d_ids.ensure(total + 1));
+  if (framed)
+    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p,
+                                                                e->d_cand_offsets.p, e->d_cand_start.p, e->d_tmp_ids.p,
+                                                                e->d_ids.p, nullptr, nullptr, e->d_ids.cap, 0, 0ull, F);
+  else
+    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, e->d_cand_offsets.p,
+                                                          e->d_cand_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
+                                                          e->d_ids.cap, 0, 0ull);
   CUDA_TRY(cudaGetLastError());
   e->last_launches += 3;
-  CUDA_TRY(e->h_ids.ensure(tmp_total + 1));
-  if (tmp_total) CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_ids.p, tmp_total * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(e->h_ids.ensure(total + 1));
+  if (total) CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_ids.p, total * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(e->h_cand_offsets.p, e->d_cand_offsets.p, (nc + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(e->h_cand_score.p, e->d_cand_score.p, nc * sizeof(float), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(e->h_n_cands.p, e->d_n_cands.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  e->last_d2h = tmp_total * 4 + (nc + 1) * 8 + nc * 4 + n * 4;
+  e->last_d2h = total * 4 + (nc + 1) * 8 + nc * 4 + n * 4;
   finish_timing(e);
   *ids = e->h_ids.p;
   return SPM_OK;
@@ -2721,7 +2795,7 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
     // forward-filtering / backward-sampling over the whole lattice (unigram_model.cc:511-542)
     { const int rc = nbest_args_ok(e, bytes, offsets, n); if (rc) return rc; }
     if (cudaSetDevice(e->device) != cudaSuccess) { e->set_error("cudaSetDevice failed"); return SPM_ERR_CUDA; }
-    const int rc = e->run_lattice(bytes, offsets, n, alpha, 0, 1);
+    const int rc = e->run_lattice(bytes, offsets, n, alpha, 0, 1, true);
     if (rc) return rc;
     if (e->lat_ids.empty()) e->lat_ids.reserve(1);
     *ids = e->lat_ids.data();
@@ -2800,15 +2874,21 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
                                                            e->d_sent_start.p, e->d_sent_count.p);
   const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
   CUDA_TRY(e->d_block_sums.ensure(nb + 1));
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, 0);
+  // every sentence's draw gets the encode frame
+  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->frame_np + e->frame_ns);
   scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
   CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaStreamSynchronize(st));
   const unsigned long long tot = e->h_ctrl64.p[2];
   CUDA_TRY(e->d_ids.ensure(tot + 1));
-  scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_id_offsets.p,
-                                                        e->d_sent_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
-                                                        e->d_ids.cap, 0, 0ull);
+  if (e->framed())
+    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_id_offsets.p,
+                                                                e->d_sent_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr,
+                                                                nullptr, e->d_ids.cap, 0, 0ull, e->kframe());
+  else
+    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_id_offsets.p,
+                                                          e->d_sent_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
+                                                          e->d_ids.cap, 0, 0ull);
   CUDA_TRY(cudaGetLastError());
   e->last_launches += 4;
   CUDA_TRY(e->h_ids.ensure(tot + 1));

@@ -73,6 +73,9 @@ util::Status SentencePieceProcessor::LoadFromSerializedProto(std::string_view se
   }
   impl_->loaded_types = m.types;
   extra_.clear();
+  frame_p_.clear();
+  frame_s_.clear();
+  frame_rev_ = false;
   seeded_ = false;
   return util::OkStatus();
 }
@@ -129,8 +132,42 @@ int SentencePieceProcessor::eos_id() const {
   return id == unk_id_ ? -1 : id;
 }
 
-// ParseExtraOptions, sentencepiece_processor.cc:1067-1101
+// ParseExtraOptions, sentencepiece_processor.cc:1067-1101; the engine then writes the options' id effect into every id
+// result (spm_engine_set_encode_frame), whatever the outcome of the parse left in extra_
 util::Status SentencePieceProcessor::SetEncodeExtraOptions(std::string_view extra_option) {
+  const util::Status st = ParseExtraOptions(extra_option);
+  if (!engine_) return st;
+  // the canonical form P ++ (r or reversed r) ++ S of the options applied in order
+  frame_p_.clear();
+  frame_s_.clear();
+  frame_rev_ = false;
+  for (const auto o : extra_) {
+    if (o == REVERSE) {
+      std::swap(frame_p_, frame_s_);
+      std::reverse(frame_p_.begin(), frame_p_.end());
+      std::reverse(frame_s_.begin(), frame_s_.end());
+      frame_rev_ = !frame_rev_;
+    } else if (o == BOS) {
+      frame_p_.insert(frame_p_.begin(), PieceToId(impl_->model.bos_piece));
+    } else if (o == EOS) {
+      frame_s_.push_back(PieceToId(impl_->model.eos_piece));
+    }
+  }
+  const int rc = spm_engine_set_encode_frame(engine_, frame_p_.data(), static_cast<uint32_t>(frame_p_.size()), frame_rev_,
+                                             frame_s_.data(), static_cast<uint32_t>(frame_s_.size()));
+  if (rc) {
+    const util::Status err = FromEngine(engine_, rc);
+    extra_.clear();
+    frame_p_.clear();
+    frame_s_.clear();
+    frame_rev_ = false;
+    spm_engine_set_encode_frame(engine_, nullptr, 0, 0, nullptr, 0);
+    return err;
+  }
+  return st;
+}
+
+util::Status SentencePieceProcessor::ParseExtraOptions(std::string_view extra_option) {
   extra_.clear();
   if (extra_option.empty()) return util::OkStatus();
   if (!engine_) return status();
@@ -271,22 +308,21 @@ util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> 
     for (size_t i = lo; i < hi; ++i) {
       auto &v = (*ids)[i];
       v.assign(out + oo[i], out + oo[i + 1]);
-      ApplyExtraIds(&v);
     }
   });
   return util::OkStatus();
 }
 
-// ApplyExtraOptions, sentencepiece_processor.cc:1019-1064
-void SentencePieceProcessor::ApplyExtraIds(std::vector<int> *v) const {
-  if (extra_.empty()) return;
-  const int bos = PieceToId(impl_->model.bos_piece), eos = PieceToId(impl_->model.eos_piece);
-  for (const auto o : extra_) {
-    if (o == REVERSE) std::reverse(v->begin(), v->end());
-    else if (o == EOS) v->push_back(eos);
-    else if (o == BOS) v->insert(v->begin(), bos);
-  }
+// The raw segmentation inside an id list the engine framed: the pieces forms lay it over the normalized text and then
+// apply the options to the piece strings.  A list shorter than the frame is an empty SampleEncodeAndScore slot.
+void SentencePieceProcessor::RawIds(const int32_t *ids, size_t n, std::vector<int> *raw) const {
+  const size_t f = frame_p_.size() + frame_s_.size();
+  if (n < f) { raw->clear(); return; }
+  raw->assign(ids + frame_p_.size(), ids + n - frame_s_.size());
+  if (frame_rev_) std::reverse(raw->begin(), raw->end());
 }
+
+// ApplyExtraOptions, sentencepiece_processor.cc:1019-1064, on piece strings
 void SentencePieceProcessor::ApplyExtraPieces(std::vector<std::string> *v, std::vector<int> *pid) const {
   if (extra_.empty()) return;
   const int bos = PieceToId(impl_->model.bos_piece), eos = PieceToId(impl_->model.eos_piece);
@@ -401,7 +437,6 @@ util::Status SentencePieceProcessor::NBestEncode(const std::vector<std::string_v
     cands.resize(nc[i]);
     for (uint32_t c = 0; c < nc[i]; ++c) {
       cands[c].assign(out + co[i * K + c], out + co[i * K + c + 1]);
-      ApplyExtraIds(&cands[c]);
     }
   }
   return util::OkStatus();
@@ -438,9 +473,9 @@ util::Status SentencePieceProcessor::NBestEncode(const std::vector<std::string_v
     cands.resize(nc[i]);
     for (uint32_t c = 0; c < nc[i]; ++c) {
       const uint64_t lo = co[i * K + c], hi = co[i * K + c + 1];
-      if (!PiecesFromIds(norms[i], out + lo, hi - lo, &cands[c]))
+      RawIds(out + lo, hi - lo, &pid);
+      if (!PiecesFromIds(norms[i], pid.data(), pid.size(), &cands[c]))
         return Internal("all normalized characters are not consumed.");  // sentencepiece_processor.cc:628-629
-      pid.assign(out + lo, out + hi);
       ApplyExtraPieces(&cands[c], &pid);
     }
   }
@@ -463,7 +498,6 @@ util::Status SentencePieceProcessor::SampleEncode(const std::vector<std::string_
   ids->resize(inputs.size());
   for (size_t i = 0; i < inputs.size(); ++i) {
     (*ids)[i].assign(out + oo[i], out + oo[i + 1]);
-    ApplyExtraIds(&(*ids)[i]);
   }
   return util::OkStatus();
 }
@@ -492,9 +526,9 @@ util::Status SentencePieceProcessor::SampleEncode(const std::vector<std::string_
   pieces->resize(inputs.size());
   std::vector<int> pid;
   for (size_t i = 0; i < inputs.size(); ++i) {
-    if (!PiecesFromIds(norms[i], out + oo[i], oo[i + 1] - oo[i], &(*pieces)[i]))
+    RawIds(out + oo[i], oo[i + 1] - oo[i], &pid);
+    if (!PiecesFromIds(norms[i], pid.data(), pid.size(), &(*pieces)[i]))
       return Internal("all normalized characters are not consumed.");
-    pid.assign(out + oo[i], out + oo[i + 1]);
     ApplyExtraPieces(&(*pieces)[i], &pid);
   }
   return util::OkStatus();
@@ -541,7 +575,6 @@ std::vector<std::pair<std::vector<int>, float>> SentencePieceProcessor::SampleEn
   if (spm_sample_encode_and_score(engine_, input.data(), offs, 1, num_samples, alpha, wor, include_best, &ids, &co, &sc)) return out;
   for (int c = 0; c < num_samples; ++c) {
     out.emplace_back(std::vector<int>(ids + co[c], ids + co[c + 1]), sc[c]);
-    ApplyExtraIds(&out.back().first);
   }
   return out;
 }
@@ -564,9 +597,9 @@ std::vector<std::pair<std::vector<std::string>, float>> SentencePieceProcessor::
   std::vector<int> pid;
   for (int c = 0; c < num_samples; ++c) {
     std::vector<std::string> pcs;
-    if (!PiecesFromIds(normalized, ids + co[c], co[c + 1] - co[c], &pcs)) return {};
-    pid.assign(ids + co[c], ids + co[c + 1]);
-    ApplyExtraPieces(&pcs, &pid);
+    RawIds(ids + co[c], co[c + 1] - co[c], &pid);
+    if (!PiecesFromIds(normalized, pid.data(), pid.size(), &pcs)) return {};
+    if (co[c + 1] > co[c]) ApplyExtraPieces(&pcs, &pid);  // an empty slot holds no sample to frame
     out.emplace_back(std::move(pcs), sc[c]);
   }
   return out;

@@ -139,7 +139,11 @@ class SentencePieceProcessor {
   std::vector<ExtraOption> extra_;
   mutable bool seeded_ = false;  // the engine's generator took the global seed (first sampling call)
   void SeedOnce() const;
-  void ApplyExtraIds(std::vector<int> *v) const;
+  // the id effect of extra_ as the engine writes it: frame_p_ ++ (r or reversed r) ++ frame_s_
+  std::vector<int> frame_p_, frame_s_;
+  bool frame_rev_ = false;
+  util::Status ParseExtraOptions(std::string_view extra_option);
+  void RawIds(const int32_t *ids, size_t n, std::vector<int> *raw) const;
   void ApplyExtraPieces(std::vector<std::string> *v, std::vector<int> *pid) const;
   // pieces of an id sequence over the sentence's normalized text (unknown tokens keep their surface)
   bool PiecesFromIds(std::string_view normalized, const int32_t *ids, size_t n, std::vector<std::string> *pieces) const;

@@ -783,14 +783,17 @@ __global__ void __launch_bounds__(256) encode_unigram_long_kernel(const KModel M
 // (block sums, scan of block sums, block scan) -- pure streaming over 4-byte counts.
 constexpr int kScanChunk = 2048;  // counts per block (256 threads x 8)
 
+// FRAMED: id lists that get the encode frame (KFrame) -- each framed item counts np + ns more.
+template <bool FRAMED = false>
 __global__ void __launch_bounds__(256) scan_block_sums_kernel(const uint32_t *counts, uint32_t n,
-                                                              unsigned long long *block_sums, uint32_t extra) {
+                                                              unsigned long long *block_sums, uint32_t extra,
+                                                              KFrame F = KFrame{}) {
   __shared__ unsigned long long warp_sums[8];
   const uint32_t base = blockIdx.x * kScanChunk;
   unsigned long long s = 0;
   for (uint32_t k = threadIdx.x; k < kScanChunk; k += 256) {
     const uint32_t i = base + k;
-    if (i < n) s += counts[i] + extra;
+    if (i < n) s += counts[i] + extra + (FRAMED ? F.added(i) : 0u);
   }
   for (int d = 16; d > 0; d >>= 1) s += __shfl_down_sync(0xFFFFFFFFu, s, d);
   if ((threadIdx.x & 31) == 0) warp_sums[threadIdx.x >> 5] = s;
@@ -830,7 +833,10 @@ __global__ void __launch_bounds__(1024) scan_block_prefix_kernel(unsigned long l
 // Block scan of counts -> offsets[i]; then every sentence's tokens are moved from
 // completion order (tmp) to sentence order (out): coalesced 4-byte copies, 8 lanes
 // per sentence.
-template <typename ElemT>
+// FRAMED (id lists only): the frame F is written around each framed item's ids, which are copied backwards when
+// F.reverse.  A template flag rather than a run-time test, so that the text and norm_to_orig instantiations and the
+// unframed id path keep their code as it was.
+template <typename ElemT, bool FRAMED = false>
 __global__ void __launch_bounds__(256) scan_write_gather_kernel(const uint32_t *counts, uint32_t n,
                                                                 const unsigned long long *block_prefix,
                                                                 unsigned long long *offsets,
@@ -838,7 +844,8 @@ __global__ void __launch_bounds__(256) scan_write_gather_kernel(const uint32_t *
                                                                 const ElemT *src, ElemT *dst,
                                                                 const uint32_t *src2, uint32_t *dst2,
                                                                 unsigned long long dst_cap, uint32_t extra,
-                                                                unsigned long long off_base) {
+                                                                unsigned long long off_base, KFrame F = KFrame{}) {
+  static_assert(!FRAMED || sizeof(ElemT) == 4, "the frame applies to id lists");
   __shared__ unsigned long long sh_off[kScanChunk + 1];
   __shared__ unsigned long long warp_sums[8];
   const uint32_t base = blockIdx.x * kScanChunk;
@@ -848,7 +855,7 @@ __global__ void __launch_bounds__(256) scan_write_gather_kernel(const uint32_t *
 #pragma unroll
   for (int k = 0; k < 8; ++k) {
     const uint32_t i = base + threadIdx.x * 8 + k;
-    c[k] = i < n ? counts[i] + extra : 0u;
+    c[k] = i < n ? counts[i] + extra + (FRAMED ? F.added(i) : 0u) : 0u;
     local += c[k];
   }
   unsigned long long incl = local;
@@ -873,6 +880,20 @@ __global__ void __launch_bounds__(256) scan_write_gather_kernel(const uint32_t *
   if (dst == nullptr) return;
   // gather: 8 lanes per sentence
   const uint32_t lane8 = threadIdx.x & 7;
+  if constexpr (FRAMED) {
+    for (uint32_t k = threadIdx.x >> 3; k < kScanChunk; k += 32) {
+      const uint32_t i = base + k;
+      if (i >= n) break;
+      const uint32_t body = counts[i];
+      const uint32_t cnt = body + F.added(i);  // (an empty n-best slot has body 0 and no frame: nothing to write)
+      const unsigned long long d0 = sh_off[k];
+      if (d0 + cnt > dst_cap) continue;
+      const ElemT *s = src + src_start[i];
+      for (uint32_t t = lane8; t < cnt; t += 8)
+        __stcs(dst + d0 + t, F.at(body, t, [&](uint32_t q) { return __ldcs(s + q); }));
+    }
+    return;
+  }
   for (uint32_t k = threadIdx.x >> 3; k < kScanChunk; k += 32) {
     const uint32_t i = base + k;
     if (i >= n) break;

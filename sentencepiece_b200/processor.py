@@ -6,6 +6,24 @@ import numpy as np
 from . import _capi
 
 
+# SetEncodeExtraOptions names (sentencepiece_processor.cc:1077-1082)
+_EXTRA_OPTIONS = {"bos": "bos", "eos": "eos", "reverse": "reverse", "unk": "unk", "unk_piece": "unk"}
+
+
+def extra_frame(options, bos_id, eos_id):
+    """The id effect of ApplyExtraOptions (sentencepiece_processor.cc:1019-1064) for options applied in order, in the
+    canonical form the engine writes: (prefix, reverse, suffix), ids -> prefix ++ (ids or reversed ids) ++ suffix."""
+    prefix, suffix, rev = [], [], False
+    for o in options:
+        if o == "reverse":
+            prefix, suffix, rev = suffix[::-1], prefix[::-1], not rev
+        elif o == "bos":
+            prefix.insert(0, bos_id)
+        elif o == "eos":
+            suffix.append(eos_id)
+    return prefix, rev, suffix
+
+
 def pack_sentences(sentences):
     """list[bytes|str] -> (uint8[total], uint64[n+1])"""
     bs = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in sentences]
@@ -57,6 +75,14 @@ class Engine:
     def cache_reset(self):
         """empties the engine's memo tables (the BPE word cache); results never depend on them"""
         self._check(self._lib.spm_engine_cache_reset(self._h))
+
+    def set_encode_frame(self, prefix=(), reverse=False, suffix=()):
+        """spm_engine_set_encode_frame: every later id result is prefix ++ (ids, reversed when `reverse`) ++ suffix;
+        no arguments restore the plain output."""
+        p = np.ascontiguousarray(prefix, dtype=np.int32)
+        q = np.ascontiguousarray(suffix, dtype=np.int32)
+        self._check(self._lib.spm_engine_set_encode_frame(self._h, p.ctypes.data if len(p) else None, len(p), int(bool(reverse)),
+                                                          q.ctypes.data if len(q) else None, len(q)))
 
     def encode_packed(self, buf, offs, copy=True):
         """Batch encode of a packed host buffer -> (ids int32[], id_offsets uint64[n+1])."""
@@ -198,7 +224,46 @@ class SentencePieceProcessor:
         self._engine = Engine(self._model_bytes, device=device)
         self._pieces = None
         self._unk_id = -1
+        self._special = None
+        self._extra = []
         return True
+
+    def _specials(self):
+        if self._special is None:
+            from . import _modelinfo
+            self._special = _modelinfo.special_pieces(self._model_bytes)
+        return self._special
+
+    def _check_defined(self, option):
+        sp = self._specials()
+        if option in ("bos", "eos") and sp[option + "_id"] < 0:
+            raise RuntimeError(f"id for `{sp[option + '_piece']}` is not defined.")  # sentencepiece_processor.cc:1088-1097
+
+    # sentencepiece_processor.h:267, parse of sentencepiece_processor.cc:1067-1101; on an error no option is kept
+    def SetEncodeExtraOptions(self, extra_option):
+        self._require()
+        self._extra = []
+        opts = []
+        for s in extra_option.split(":") if extra_option else []:
+            if s not in _EXTRA_OPTIONS:
+                raise RuntimeError(f'option "{s}" is not available.')
+            opts.append(_EXTRA_OPTIONS[s])
+            self._check_defined(opts[-1])
+        self._extra = opts
+        return True
+
+    def _options(self, add_bos, add_eos, reverse):
+        """SetEncodeExtraOptions' options, then the Python binding's reverse, bos, eos (sentencepiece.i:138-145)."""
+        opts = list(self._extra) + ["reverse"] * bool(reverse) + ["bos"] * bool(add_bos) + ["eos"] * bool(add_eos)
+        for o in opts:
+            self._check_defined(o)
+        return opts
+
+    def _set_frame(self, add_bos, add_eos, reverse):
+        """Makes the engine write the options' ids around every id list of the next call."""
+        sp = self._specials()
+        prefix, rev, suffix = extra_frame(self._options(add_bos, add_eos, reverse), sp["bos_id"], sp["eos_id"])
+        self._engine.set_encode_frame(prefix, rev, suffix)
 
     def _require(self):
         if self._engine is None:
@@ -219,18 +284,21 @@ class SentencePieceProcessor:
         out = [raw[int(to[i]):int(to[i + 1])].decode("utf-8", errors="replace") for i in range(len(lists))]
         return out[0] if single else out
 
-    def EncodeAsIds(self, input):
+    def EncodeAsIds(self, input, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
+        """emit_unk_piece changes piece strings only: it has no effect on ids."""
         self._require()
         single = isinstance(input, (str, bytes))
         buf, offs = pack_sentences([input] if single else input)
+        self._set_frame(add_bos, add_eos, reverse)
         ids, ido = self._engine.encode_packed(buf, offs)
         out = [ids[int(ido[i]):int(ido[i + 1])].tolist() for i in range(len(offs) - 1)]
         return out[0] if single else out
 
     # ---- pieces: ids + token ends in the normalized text (spm_encode_spans); unknown tokens keep their surface
     #      (sentencepiece_processor.cc:609-621) ----
-    def EncodeAsPieces(self, input):
+    def EncodeAsPieces(self, input, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
+        opts = self._options(add_bos, add_eos, reverse) + ["unk"] * bool(emit_unk_piece)
         single = isinstance(input, (str, bytes))
         buf, offs = pack_sentences([input] if single else input)
         r = self._engine.encode_spans(buf, offs)
@@ -248,16 +316,35 @@ class SentencePieceProcessor:
                 else:
                     row.append(self._pieces[int(ids[k])])
                 begin = end
-            out.append(row)
+            out.append(self._apply_pieces(row, ids[int(ido[i]):int(ido[i + 1])].tolist(), opts) if opts else row)
         return out[0] if single else out
 
-    def encode(self, input, out_type=int, enable_sampling=False, nbest_size=-1, alpha=0.1):
-        """python/src/sentencepiece/__init__.py Encode: out_type int | str; enable_sampling uses SampleEncode."""
+    def _apply_pieces(self, row, ids, opts):
+        """ApplyExtraOptions on piece strings (sentencepiece_processor.cc:1019-1064): the spans call returns the raw
+        segmentation, so the options are applied here."""
+        sp = self._specials()
+        pairs = list(zip(row, ids))
+        for o in opts:
+            if o == "reverse":
+                pairs.reverse()
+            elif o == "bos":
+                pairs.insert(0, (sp["bos_piece"], sp["bos_id"]))
+            elif o == "eos":
+                pairs.append((sp["eos_piece"], sp["eos_id"]))
+            elif o == "unk":
+                pairs = [(sp["unk_piece"], i) if i == self._unk_id else (p, i) for p, i in pairs]
+        return [p for p, _ in pairs]
+
+    def encode(self, input, out_type=int, enable_sampling=False, nbest_size=-1, alpha=0.1, add_bos=False, add_eos=False,
+               reverse=False, emit_unk_piece=False):
+        """python/src/sentencepiece/__init__.py Encode: out_type int | str; enable_sampling uses SampleEncode.
+        add_bos / add_eos / reverse apply after SetEncodeExtraOptions' options, in the order reverse, bos, eos."""
+        kw = dict(add_bos=add_bos, add_eos=add_eos, reverse=reverse, emit_unk_piece=emit_unk_piece)
         if enable_sampling:
             if out_type is not int:
                 raise NotImplementedError("sampled pieces: use the C++ host layer (SampleEncodeAsPieces)")
-            return self.SampleEncodeAsIds(input, nbest_size, alpha)
-        return self.EncodeAsIds(input) if out_type is int else self.EncodeAsPieces(input)
+            return self.SampleEncodeAsIds(input, nbest_size, alpha, **kw)
+        return self.EncodeAsIds(input, **kw) if out_type is int else self.EncodeAsPieces(input, **kw)
 
     Encode = encode
 
@@ -266,17 +353,19 @@ class SentencePieceProcessor:
         return single, pack_sentences([input] if single else input)
 
     # sentencepiece_processor.h:481; the draws of a batch are taken in order on one generator (SetRandomGeneratorSeed)
-    def SampleEncodeAsIds(self, input, nbest_size, alpha):
+    def SampleEncodeAsIds(self, input, nbest_size, alpha, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
         single, (buf, offs) = self._split(input)
+        self._set_frame(add_bos, add_eos, reverse)
         ids, ido = self._engine.sample_encode(buf, offs, nbest_size, alpha)
         out = [ids[int(ido[i]):int(ido[i + 1])].tolist() for i in range(len(offs) - 1)]
         return out[0] if single else out
 
     # sentencepiece_processor.h:471
-    def NBestEncodeAsIds(self, input, nbest_size):
+    def NBestEncodeAsIds(self, input, nbest_size, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
         single, (buf, offs) = self._split(input)
+        self._set_frame(add_bos, add_eos, reverse)
         r = self._engine.nbest_encode(buf, offs, nbest_size)
         K, co = r["K"], r["cand_offsets"]
         out = [[r["ids"][int(co[i * K + c]):int(co[i * K + c + 1])].tolist() for c in range(int(r["n_cands"][i]))]
