@@ -137,6 +137,25 @@ int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, 
                      const int32_t **ids, const uint32_t **tok_end, const uint64_t **id_offsets,
                      const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o);
 
+/* Replaces the per-sentence loop over SentencePieceProcessor::Encode(absl::string_view, std::vector<std::string>*)
+ * (src/sentencepiece_processor.cc:379-390 -> :547-636) for n sentences, with the encode frame
+ * (spm_engine_set_encode_frame) applied to pieces and ids alike.  The piece of a token is IdToPiece(id), except for
+ * the unknown id: its surface in the normalized text (a run of unknown characters is one token).
+ * unk_piece: NULL keeps the normalized surface of unknown tokens; otherwise it is the string that UNK_PIECE
+ *   writes (trainer_spec.unk_piece; the caller owns option parsing, as for the frame).
+ * sep: -1 = pieces abut; 0..255 = that byte between consecutive pieces of a sentence (spm_encode uses ' ').
+ * out (engine-owned pinned memory, valid until the next call): text[text_offsets[i] .. text_offsets[i+1]) is sentence
+ *   i's pieces; piece_end[id_offsets[i] + k] is the exclusive end of its k-th piece relative to text_offsets[i]
+ *   (the tok_end convention of spm_encode_spans); ids / id_offsets are the framed ids of those pieces, identical to
+ *   what spm_encode_ids returns.
+ * The ids come from the kernels of spm_encode_ids; only sentences that hold the unknown id (and only when unk_piece is
+ * NULL) are encoded a second time, by the path of spm_encode_spans, for their normalized text
+ * (spm_engine_info.last_unk_detour counts them).  Argument errors as spm_encode_ids. */
+int spm_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n,
+                      const char *unk_piece, size_t unk_piece_len, int sep,
+                      const char **text, const uint64_t **text_offsets, const uint32_t **piece_end,
+                      const int32_t **ids, const uint64_t **id_offsets);
+
 /* ------------------------------------------------------------------------
  * Batch encode, DEVICE buffers (inputs already resident in HBM; used when the
  * caller keeps corpora on the GPU, and by bench.py for the kernel-only number).
@@ -246,6 +265,7 @@ typedef struct {
   float last_main_kernel_ms;        /* device time of the dominant (encode) kernel alone */
   uint64_t last_h2d_bytes, last_d2h_bytes;
   uint64_t last_deferred;           /* sentences that took the long-sentence path */
+  uint64_t last_unk_detour;         /* spm_encode_pieces: sentences encoded again for the surfaces of unknown tokens */
 } spm_engine_info;
 int spm_engine_get_info(const spm_engine *e, spm_engine_info *info);
 

@@ -15,7 +15,7 @@ EXPORTS = [
     "spm_last_error", "spm_encode_ids", "spm_encode_spans", "spm_encode_ids_device", "spm_host_alloc",
     "spm_host_free", "spm_engine_get_info", "spm_engine_set_tuning", "spm_nbest_encode", "spm_set_random_seed",
     "spm_sample_encode_ids", "spm_decode_ids", "spm_engine_set_unk_surface", "spm_calculate_entropy",
-    "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame",
+    "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
 ]
 
 
@@ -36,7 +36,7 @@ class EngineInfo(ctypes.Structure):
                 ("charsmap_units", ctypes.c_uint32), ("last_kernel_launches", ctypes.c_uint64),
                 ("last_kernel_ms", ctypes.c_float), ("last_main_kernel_ms", ctypes.c_float),
                 ("last_h2d_bytes", ctypes.c_uint64), ("last_d2h_bytes", ctypes.c_uint64),
-                ("last_deferred", ctypes.c_uint64)]
+                ("last_deferred", ctypes.c_uint64), ("last_unk_detour", ctypes.c_uint64)]
 
 
 _lib = None
@@ -64,6 +64,7 @@ def load():
     L.spm_last_error.restype = cp
     L.spm_encode_ids.argtypes = [vp, vp, vp, sz, P(vp), P(vp)]
     L.spm_encode_spans.argtypes = [vp, vp, vp, sz, P(vp), P(vp), P(vp), P(vp), P(vp), P(vp)]
+    L.spm_encode_pieces.argtypes = [vp, vp, vp, sz, cp, sz, ctypes.c_int, P(vp), P(vp), P(vp), P(vp), P(vp)]
     L.spm_encode_ids_device.argtypes = [vp, vp, vp, sz, ctypes.c_uint64, vp, ctypes.c_uint64, vp,
                                         P(ctypes.c_uint64), vp]
     L.spm_host_alloc.argtypes = [sz]

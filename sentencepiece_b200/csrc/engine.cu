@@ -34,6 +34,7 @@
 #include "model_reader.h"
 #include "order_kernel.cuh"
 #include "decode_kernel.cuh"
+#include "pieces_kernel.cuh"
 #include "nbest_kernel.cuh"
 #include "lattice_kernel.cuh"
 #include "trie_builder.h"
@@ -303,6 +304,18 @@ struct spm_engine {
   PinBuf<uint8_t> h_stage[2];
   int decode_host_pipelined(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
                             const uint64_t **text_offsets);
+  // EncodeAsPieces (K9): per-id piece bytes, built on first use; the raw ids of the lane kernels, the unknown-surface
+  // subset and its spans run, the packed pieces
+  DevBuf<uint32_t> d_pc_off, d_pc_flag, d_pc_sub_of, d_pc_sub_len, d_pc_text_len, d_pc_ntok, d_pc_end;
+  DevBuf<uint8_t> d_pc_bytes, d_pc_unk, d_pc_sub_bytes, d_pc_text;
+  DevBuf<int32_t> d_pc_ids, d_pc_out_ids;
+  DevBuf<unsigned long long> d_pc_id_offsets, d_pc_pos, d_pc_sub_start, d_pc_sub_offsets, d_pc_text_offsets,
+      d_pc_out_id_offsets;
+  PinBuf<char> h_pc_text;
+  PinBuf<uint64_t> h_pc_text_offsets;
+  PinBuf<uint32_t> h_pc_end;
+  bool pc_ready = false;
+  int ensure_piece_tables();
   // n-best / sampling
   DevBuf<uint8_t> d_nb_scratch;
   DevBuf<unsigned long long> d_cand_start, d_cand_offsets;
@@ -408,7 +421,7 @@ struct spm_engine {
   bool framed() const { return frame_np + frame_ns != 0 || frame_rev; }
 
   // stats of the last call
-  uint64_t last_launches = 0, last_h2d = 0, last_d2h = 0, last_deferred = 0;
+  uint64_t last_launches = 0, last_h2d = 0, last_d2h = 0, last_deferred = 0, last_unk_detour = 0;
   float last_ms = 0.f, last_main_ms = 0.f;
 
   void set_error(const std::string &m) const { err = m; }
@@ -1703,6 +1716,25 @@ int spm_engine::ensure_decode_tables() {
   return SPM_OK;
 }
 
+// IdToPiece for every id, the raw piece bytes (U+2581 kept).  Piece strings never change after load: SetVocabulary /
+// ResetVocabulary only change types (spm_engine_set_types), and the unknown piece is replaced per call.
+int spm_engine::ensure_piece_tables() {
+  if (pc_ready) return SPM_OK;
+  const int V = model.vocab_size();
+  std::vector<uint32_t> off(V + 1, 0);
+  std::vector<uint8_t> bytes;
+  for (int i = 0; i < V; ++i) {
+    off[i] = static_cast<uint32_t>(bytes.size());
+    bytes.insert(bytes.end(), model.piece(i), model.piece(i) + model.piece_len(i));
+  }
+  off[V] = static_cast<uint32_t>(bytes.size());
+  bytes.push_back(0);
+  CUDA_TRY(d_pc_off.upload(off));
+  CUDA_TRY(d_pc_bytes.upload(bytes));
+  pc_ready = true;
+  return SPM_OK;
+}
+
 // Host-to-device copy of caller memory: pinned memory goes straight to the copy engine; pageable memory is first
 // copied into a pinned staging buffer by a few host threads (the driver's own staging of pageable memory is
 // single-threaded and synchronous), then handed to the copy engine.
@@ -2315,6 +2347,11 @@ void spm_engine_destroy(spm_engine *e) {
   e->d_dec_off.release(); e->d_dec_info.release(); e->d_dec_bytes.release(); e->d_dec_tmp.release(); e->d_dec_text.release();
   e->d_dec_ids.release(); e->d_dec_text_offsets.release(); e->h_dec_text.release(); e->h_dec_text_offsets.release();
   for (int k = 0; k < 2; ++k) { e->p_dec_ids[k].release(); e->p_dec_text[k].release(); e->p_dec_toff[k].release(); e->h_stage[k].release(); }
+  e->d_pc_off.release(); e->d_pc_flag.release(); e->d_pc_sub_of.release(); e->d_pc_sub_len.release(); e->d_pc_text_len.release();
+  e->d_pc_ntok.release(); e->d_pc_end.release(); e->d_pc_bytes.release(); e->d_pc_unk.release(); e->d_pc_sub_bytes.release();
+  e->d_pc_text.release(); e->d_pc_ids.release(); e->d_pc_out_ids.release(); e->d_pc_id_offsets.release(); e->d_pc_pos.release();
+  e->d_pc_sub_start.release(); e->d_pc_sub_offsets.release(); e->d_pc_text_offsets.release(); e->d_pc_out_id_offsets.release();
+  e->h_pc_text.release(); e->h_pc_text_offsets.release(); e->h_pc_end.release();
   e->d_frame.release();
   e->d_order.release(); e->d_order_hist.release(); e->d_seg_done.release(); e->d_sent_rel.release(); e->d_seg_words.release();
   if (e->ev_offs) cudaEventDestroy(e->ev_offs);
@@ -2535,6 +2572,7 @@ int spm_engine_get_info(const spm_engine *e, spm_engine_info *info) {
   info->last_h2d_bytes = e->last_h2d;
   info->last_d2h_bytes = e->last_d2h;
   info->last_deferred = e->last_deferred;
+  info->last_unk_detour = e->last_unk_detour;
   return SPM_OK;
 }
 
@@ -2952,6 +2990,206 @@ int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, 
   if (!e || !tok_end || !normalized || !norm_offsets || !n2o) return SPM_ERR_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_host_locked(e, bytes, offsets, n, true, ids, tok_end, id_offsets, normalized, norm_offsets, n2o);
+}
+
+// EncodeAsPieces for a host batch:
+//   1. raw ids from the kernels spm_encode_ids runs (lane / BPE-lane2 kernels, deferred and long kernels), frame off;
+//   2. without unk_piece: the sentences whose raw ids hold the unknown id are packed on the device and run through the
+//      spans path, which gives their token ends in the normalized text (the surfaces of their unknown tokens);
+//   3. K9 (pieces_kernel.cuh): size pass, scans, write pass -- the frame, reverse, unk_piece and sep applied once, to
+//      pieces and ids alike.
+static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, const char *unk_piece,
+                                size_t unk_len, int sep, const char **text, const uint64_t **text_offsets,
+                                const uint32_t **piece_end, const int32_t **ids, const uint64_t **id_offsets) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!offsets || !text || !text_offsets || !piece_end || !ids || !id_offsets || (unk_len && !unk_piece) ||
+      (n && !bytes && offsets[n] != offsets[0])) {
+    e->set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (sep < -1 || sep > 255) { e->set_error("sep must be -1 or a byte value"); return SPM_ERR_ARG; }
+  if (unk_len > 0xFFFFFFull) { e->set_error("unk_piece too long"); return SPM_ERR_ARG; }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = e->stream;
+  e->last_unk_detour = 0;
+  CUDA_TRY(e->h_pc_text_offsets.ensure(n + 1));
+  CUDA_TRY(e->h_id_offsets.ensure(n + 1));
+  if (n == 0) {
+    CUDA_TRY(e->h_pc_text.ensure(1)); CUDA_TRY(e->h_pc_end.ensure(1)); CUDA_TRY(e->h_ids.ensure(1));
+    e->h_pc_text_offsets.p[0] = 0;
+    e->h_id_offsets.p[0] = 0;
+    e->h_pc_text.p[0] = 0;
+    *text = e->h_pc_text.p; *text_offsets = e->h_pc_text_offsets.p; *piece_end = e->h_pc_end.p;
+    *ids = e->h_ids.p; *id_offsets = e->h_id_offsets.p;
+    return SPM_OK;
+  }
+  for (size_t i = 0; i < n; ++i)
+    if (offsets[i + 1] < offsets[i]) { e->set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
+  const uint64_t base = offsets[0];
+  const uint64_t total_bytes = offsets[n] - base;
+  if (e->model.model_type == SPM_UNIGRAM) e->batch_fast_words = e->pick_fast_words_host(bytes, offsets, n);
+  { const int rc = e->ensure_piece_tables(); if (rc) return rc; }
+  CUDA_TRY(e->d_bytes.ensure(total_bytes + 64));
+  CUDA_TRY(e->d_offsets.ensure(n + 1));
+  CUDA_TRY(cudaEventRecord(e->ev[3], st));
+  if (total_bytes) CUDA_TRY(cudaMemcpyAsync(e->d_bytes.p, bytes + base, total_bytes, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(e->d_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+  e->last_h2d = total_bytes + (n + 1) * sizeof(uint64_t) + unk_len;
+  // ---- 1. raw ids: the frame is written once, by K9 ----
+  uint64_t raw_tot = 0;
+  int rc;
+  {
+    struct FrameOff {
+      spm_engine *e;
+      uint32_t np, ns;
+      bool rev;
+      explicit FrameOff(spm_engine *x) : e(x), np(x->frame_np), ns(x->frame_ns), rev(x->frame_rev) {
+        x->frame_np = x->frame_ns = 0;
+        x->frame_rev = false;
+      }
+      ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
+    } off(e);
+    rc = e->run_device(e->d_bytes.p - base, e->d_offsets.p, n, total_bytes, false, nullptr, 0, nullptr, &raw_tot, nullptr, st,
+                       &e->d_pc_ids, &e->d_pc_id_offsets);
+  }
+  if (rc) return rc;
+  float main_ms = 0.f;
+  if (cudaEventElapsedTime(&main_ms, e->ev[0], e->ev[1]) != cudaSuccess) main_ms = 0.f;
+  uint64_t launches = e->last_launches, deferred = e->last_deferred;
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
+  const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  CUDA_TRY(e->d_block_sums.ensure(nb + 1));
+  KPieces P{};
+  P.n = n32;
+  P.ids = e->d_pc_ids.p;
+  P.id_offsets = e->d_pc_id_offsets.p;
+  P.pc_off = e->d_pc_off.p;
+  P.pc_bytes = e->d_pc_bytes.p;
+  P.unk_id = e->unk_id;
+  P.sep = sep;
+  P.F = e->kframe();
+  // ---- 2. unknown surfaces: only the sentences that hold the unknown id take the spans path ----
+  uint32_t m = 0;
+  if (!unk_piece && e->unk_id >= 0) {
+    CUDA_TRY(e->d_pc_flag.ensure(n));
+    CUDA_TRY(e->d_pc_pos.ensure(n + 1));
+    pieces_unk_flag_kernel<<<wgrid, 256, 0, st>>>(e->d_pc_ids.p, e->d_pc_id_offsets.p, n32, e->unk_id, e->d_pc_flag.p);
+    scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_flag.p, n32, e->d_block_sums.p, 0);
+    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
+    scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_flag.p, n32, e->d_block_sums.p, e->d_pc_pos.p, nullptr, nullptr,
+                                                          nullptr, nullptr, nullptr, 0, 0, 0ull);
+    CUDA_TRY(cudaGetLastError());
+    launches += 4;
+    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    m = static_cast<uint32_t>(e->h_ctrl64.p[2]);
+  }
+  if (m) {
+    CUDA_TRY(e->d_pc_sub_of.ensure(n));
+    CUDA_TRY(e->d_pc_sub_start.ensure(m));
+    CUDA_TRY(e->d_pc_sub_len.ensure(m));
+    CUDA_TRY(e->d_pc_sub_offsets.ensure(m + 1));
+    CUDA_TRY(e->d_pc_sub_bytes.ensure(total_bytes + 64));
+    pieces_sub_list_kernel<<<static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256)), 256, 0, st>>>(
+        e->d_pc_flag.p, e->d_pc_pos.p, e->d_offsets.p, n32, e->d_pc_sub_of.p, e->d_pc_sub_start.p, e->d_pc_sub_len.p);
+    const uint32_t mb = (m + kScanChunk - 1) / kScanChunk;
+    scan_block_sums_kernel<<<mb, 256, 0, st>>>(e->d_pc_sub_len.p, m, e->d_block_sums.p, 0);
+    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, mb, e->d_ctrl64.p + 2);
+    scan_write_gather_kernel<uint8_t><<<mb, 256, 0, st>>>(e->d_pc_sub_len.p, m, e->d_block_sums.p, e->d_pc_sub_offsets.p,
+                                                          e->d_pc_sub_start.p, e->d_bytes.p - base, e->d_pc_sub_bytes.p, nullptr,
+                                                          nullptr, e->d_pc_sub_bytes.cap, 0, 0ull);
+    CUDA_TRY(cudaGetLastError());
+    launches += 4;
+    // (the whole batch's byte count bounds the subset's: it only sizes the spans run's temporary buffers)
+    uint64_t sub_tot = 0, sub_norm = 0;
+    rc = e->run_device(e->d_pc_sub_bytes.p, reinterpret_cast<const uint64_t *>(e->d_pc_sub_offsets.p), m, total_bytes, true,
+                       nullptr, 0, nullptr, &sub_tot, &sub_norm, st);
+    if (rc) return rc;
+    launches += e->last_launches;
+    deferred += e->last_deferred;
+    P.sub_of = e->d_pc_sub_of.p;
+    P.sub_ids = e->d_ids.p;
+    P.sub_tok_end = e->d_tok_end.p;
+    P.sub_id_offsets = e->d_id_offsets.p;
+    P.norm = e->d_norm.p;
+    P.norm_offsets = e->d_norm_offsets.p;
+  }
+  // ---- 3. K9: sizes, offsets, pieces ----
+  if (unk_piece) {
+    CUDA_TRY(e->d_pc_unk.ensure(unk_len + 1));
+    if (unk_len) CUDA_TRY(cudaMemcpyAsync(e->d_pc_unk.p, unk_piece, unk_len, cudaMemcpyHostToDevice, st));
+    P.unk_piece = e->d_pc_unk.p;
+    P.unk_len = static_cast<uint32_t>(unk_len);
+  }
+  CUDA_TRY(e->d_pc_text_len.ensure(n));
+  CUDA_TRY(e->d_pc_ntok.ensure(n));
+  CUDA_TRY(e->d_pc_text_offsets.ensure(n + 1));
+  CUDA_TRY(e->d_pc_out_id_offsets.ensure(n + 1));
+  P.text_len = e->d_pc_text_len.p;
+  P.n_tok = e->d_pc_ntok.p;
+  pieces_warp_kernel<false><<<wgrid, 256, 0, st>>>(P);
+  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_text_len.p, n32, e->d_block_sums.p, 0);
+  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
+  scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_text_len.p, n32, e->d_block_sums.p, e->d_pc_text_offsets.p,
+                                                        nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0ull);
+  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_ntok.p, n32, e->d_block_sums.p, 0);
+  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 3);
+  scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_ntok.p, n32, e->d_block_sums.p, e->d_pc_out_id_offsets.p,
+                                                        nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0ull);
+  CUDA_TRY(cudaGetLastError());
+  launches += 7;
+  CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  const unsigned long long ttext = e->h_ctrl64.p[2], tids = e->h_ctrl64.p[3];
+  CUDA_TRY(e->d_pc_text.ensure(ttext + 1));
+  CUDA_TRY(e->d_pc_end.ensure(tids + 1));
+  CUDA_TRY(e->d_pc_out_ids.ensure(tids + 1));
+  P.text_offsets = e->d_pc_text_offsets.p;
+  P.out_id_offsets = e->d_pc_out_id_offsets.p;
+  P.text = e->d_pc_text.p;
+  P.piece_end = e->d_pc_end.p;
+  P.out_ids = e->d_pc_out_ids.p;
+  pieces_warp_kernel<true><<<wgrid, 256, 0, st>>>(P);
+  CUDA_TRY(cudaGetLastError());
+  ++launches;
+  CUDA_TRY(e->h_pc_text.ensure(ttext + 1));
+  CUDA_TRY(e->h_pc_end.ensure(tids + 1));
+  CUDA_TRY(e->h_ids.ensure(tids + 1));
+  if (ttext) CUDA_TRY(cudaMemcpyAsync(e->h_pc_text.p, e->d_pc_text.p, ttext, cudaMemcpyDeviceToHost, st));
+  if (tids) {
+    CUDA_TRY(cudaMemcpyAsync(e->h_pc_end.p, e->d_pc_end.p, tids * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_pc_out_ids.p, tids * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_TRY(cudaMemcpyAsync(e->h_pc_text_offsets.p, e->d_pc_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(e->h_id_offsets.p, e->d_pc_out_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaEventRecord(e->ev[2], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  e->last_d2h = ttext + tids * 8 + (n + 1) * 16;
+  e->last_launches = launches;
+  e->last_deferred = deferred;
+  e->last_unk_detour = m;
+  e->last_main_ms = main_ms;
+  float all = 0.f;
+  e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : main_ms;
+  (void)cudaGetLastError();
+  e->h_pc_text.p[ttext] = 0;
+  *text = e->h_pc_text.p;
+  *text_offsets = e->h_pc_text_offsets.p;
+  *piece_end = e->h_pc_end.p;
+  *ids = e->h_ids.p;
+  *id_offsets = e->h_id_offsets.p;
+  return SPM_OK;
+}
+
+int spm_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, const char *unk_piece,
+                      size_t unk_piece_len, int sep, const char **text, const uint64_t **text_offsets,
+                      const uint32_t **piece_end, const int32_t **ids, const uint64_t **id_offsets) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
+                              id_offsets);
 }
 
 }  // extern "C"

@@ -336,6 +336,19 @@ void SentencePieceProcessor::ApplyExtraPieces(std::vector<std::string> *v, std::
   }
 }
 
+// The engine writes the pieces with the options applied: bos / eos / reverse are the frame SetEncodeExtraOptions set,
+// UNK_PIECE is passed as trainer_spec.unk_piece.
+util::Status SentencePieceProcessor::EncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int sep,
+                                                        const char **text, const uint64_t **text_offsets,
+                                                        const uint32_t **piece_end, const uint64_t **id_offsets) const {
+  if (!engine_) return status();
+  const bool unk = std::find(extra_.begin(), extra_.end(), UNK_PIECE) != extra_.end();
+  const std::string &up = impl_->model.unk_piece;
+  const int32_t *ids;
+  return FromEngine(engine_, spm_encode_pieces(engine_, bytes, offsets, n, unk ? up.data() : nullptr, unk ? up.size() : 0, sep,
+                                               text, text_offsets, piece_end, &ids, id_offsets));
+}
+
 util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> &inputs,
                                             std::vector<std::vector<std::string>> *pieces) const {
   if (!engine_) return status();
@@ -344,27 +357,23 @@ util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> 
   std::string bytes;
   std::vector<uint64_t> offs;
   Pack(inputs, &bytes, &offs);
-  const int32_t *ids;
-  const uint32_t *tok_end, *n2o;
-  const uint64_t *ido, *no;
-  const char *norm;
-  const int rc = spm_encode_spans(engine_, bytes.data(), offs.data(), inputs.size(), &ids, &tok_end, &ido, &norm, &no, &n2o);
-  if (rc) return FromEngine(engine_, rc);
+  const char *text;
+  const uint64_t *to, *ido;
+  const uint32_t *ends;
+  const auto st = EncodePiecesPacked(bytes.data(), offs.data(), inputs.size(), -1, &text, &to, &ends, &ido);
+  if (!st.ok()) return st;
   pieces->resize(inputs.size());
-  std::vector<int> pid;
-  for (size_t i = 0; i < inputs.size(); ++i) {
-    auto &v = (*pieces)[i];
-    pid.clear();
-    uint32_t begin = 0;
-    for (uint64_t k = ido[i]; k < ido[i + 1]; ++k) {
-      // unknown pieces keep their normalized surface (sentencepiece_processor.cc:609-621)
-      if (ids[k] == unk_id_) v.emplace_back(norm + no[i] + begin, tok_end[k] - begin);
-      else v.push_back(impl_->pieces[ids[k]]);
-      pid.push_back(ids[k]);
-      begin = tok_end[k];
+  ParallelFor(inputs.size(), [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) {
+      auto &v = (*pieces)[i];
+      v.reserve(ido[i + 1] - ido[i]);
+      uint32_t begin = 0;
+      for (uint64_t k = ido[i]; k < ido[i + 1]; ++k) {
+        v.emplace_back(text + to[i] + begin, ends[k] - begin);
+        begin = ends[k];
+      }
     }
-    ApplyExtraPieces(&v, &pid);
-  }
+  });
   return util::OkStatus();
 }
 

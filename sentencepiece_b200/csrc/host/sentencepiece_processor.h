@@ -111,6 +111,11 @@ class SentencePieceProcessor {
   // zero-copy form: packed input, packed output owned by the engine until the next call
   util::Status EncodePacked(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
                             const uint64_t **id_offsets) const;
+  // the same for pieces with the extra options applied: sentence i is text[text_offsets[i] .. text_offsets[i+1]), its
+  // pieces separated by the byte `sep` (-1: none); piece_end / id_offsets as spm_encode_pieces returns them
+  util::Status EncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int sep, const char **text,
+                                  const uint64_t **text_offsets, const uint32_t **piece_end,
+                                  const uint64_t **id_offsets) const;
 
   // ---- Decode(ids) (src/sentencepiece_processor.h Decode(const std::vector<int>&, std::string*)); the batch form is
   //      one device call for all lists.  An id outside [0, GetPieceSize()) fails the call like the reference's

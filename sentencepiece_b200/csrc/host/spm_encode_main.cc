@@ -114,11 +114,24 @@ int main(int argc, char **argv) {
       st = sp.Encode(views, &ids);
       if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
       for (const auto &v : ids) join_ids(v);
-    } else if (format == "piece" || format == "proto") {
+    } else if (format == "piece") {  // the engine writes each line's pieces joined by ' '
+      std::string packed;
+      std::vector<uint64_t> offs(lines.size() + 1, 0);
+      for (size_t i = 0; i < lines.size(); ++i) { packed += lines[i]; offs[i + 1] = packed.size(); }
+      const char *text;
+      const uint64_t *to, *ido;
+      const uint32_t *ends;
+      st = sp.EncodePiecesPacked(packed.data(), offs.data(), lines.size(), ' ', &text, &to, &ends, &ido);
+      if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
+      buf.reserve(to[lines.size()] + lines.size());
+      for (size_t i = 0; i < lines.size(); ++i) {
+        buf.append(text + to[i], to[i + 1] - to[i]);
+        buf += '\n';
+      }
+    } else if (format == "proto") {
       std::vector<std::vector<std::string>> pcs;
       st = sp.Encode(views, &pcs);
       if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
-      if (format == "piece") for (const auto &v : pcs) join_pieces(v);
     } else if (format == "sample_id" || format == "sample_proto") {
       std::vector<std::vector<int>> ids;
       st = sp.SampleEncode(views, nbest_size, alpha, &ids);

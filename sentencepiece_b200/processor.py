@@ -24,6 +24,24 @@ def extra_frame(options, bos_id, eos_id):
     return prefix, rev, suffix
 
 
+def split_pieces(text, text_offsets, piece_end, id_offsets):
+    """The packed output of spm_encode_pieces (sep = -1) as one list of piece strings per sentence: piece k of sentence i is
+    text[text_offsets[i] + (piece_end[id_offsets[i] + k - 1] or 0) : text_offsets[i] + piece_end[id_offsets[i] + k]]."""
+    raw = bytes(np.ascontiguousarray(text, dtype=np.uint8))
+    to = np.asarray(text_offsets, dtype=np.uint64).tolist()
+    ido = np.asarray(id_offsets, dtype=np.uint64).tolist()
+    ends = np.asarray(piece_end, dtype=np.uint32).tolist()
+    out = []
+    for i in range(len(to) - 1):
+        s = raw[to[i]:to[i + 1]]
+        row, begin = [], 0
+        for end in ends[ido[i]:ido[i + 1]]:
+            row.append(s[begin:end].decode("utf-8", errors="replace"))
+            begin = end
+        out.append(row)
+    return out
+
+
 def pack_sentences(sentences):
     """list[bytes|str] -> (uint8[total], uint64[n+1])"""
     bs = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in sentences]
@@ -122,6 +140,28 @@ class Engine:
         norm = ctypes.string_at(p[3], tn) if tn else b""
         n2o = np.ctypeslib.as_array(ctypes.cast(p[5], ctypes.POINTER(ctypes.c_uint32)), (tn + n,)).copy()
         return dict(ids=ids, tok_end=te, id_offsets=ido, normalized=norm, norm_offsets=no, n2o=n2o)
+
+    def encode_pieces(self, buf, offs, unk_piece=None, sep=-1):
+        """spm_encode_pieces: EncodeAsPieces over a packed batch, the encode frame applied ->
+        dict(text uint8[], text_offsets uint64[n+1], piece_end uint32[], ids int32[], id_offsets uint64[n+1]).
+        unk_piece (str | bytes | None) replaces the piece of every unknown token; sep = -1 or the byte written between
+        consecutive pieces of a sentence."""
+        n = len(offs) - 1
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        if isinstance(unk_piece, str):
+            unk_piece = unk_piece.encode("utf-8")
+        p = [ctypes.c_void_p() for _ in range(5)]
+        self._check(self._lib.spm_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, unk_piece,
+                                                len(unk_piece) if unk_piece is not None else 0, sep,
+                                                *[ctypes.byref(x) for x in p]))
+        to = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+        ido = np.ctypeslib.as_array(ctypes.cast(p[4], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+        tt, tot = int(to[n]), int(ido[n])
+        text = np.frombuffer(ctypes.string_at(p[0], tt), dtype=np.uint8) if tt else np.zeros(0, np.uint8)
+        pe = np.ctypeslib.as_array(ctypes.cast(p[2], ctypes.POINTER(ctypes.c_uint32)), (max(tot, 1),))[:tot].copy()
+        ids = np.ctypeslib.as_array(ctypes.cast(p[3], ctypes.POINTER(ctypes.c_int32)), (max(tot, 1),))[:tot].copy()
+        return dict(text=text, text_offsets=to, piece_end=pe, ids=ids, id_offsets=ido)
 
     def decode_packed(self, ids, id_offsets):
         """Batch Decode of packed id lists -> (text uint8[], text_offsets uint64[n+1])."""
@@ -222,8 +262,6 @@ class SentencePieceProcessor:
     def LoadFromSerializedProto(self, serialized, device=0):
         self._model_bytes = bytes(serialized)
         self._engine = Engine(self._model_bytes, device=device)
-        self._pieces = None
-        self._unk_id = -1
         self._special = None
         self._extra = []
         return True
@@ -294,46 +332,18 @@ class SentencePieceProcessor:
         out = [ids[int(ido[i]):int(ido[i + 1])].tolist() for i in range(len(offs) - 1)]
         return out[0] if single else out
 
-    # ---- pieces: ids + token ends in the normalized text (spm_encode_spans); unknown tokens keep their surface
-    #      (sentencepiece_processor.cc:609-621) ----
+    # ---- pieces (spm_encode_pieces): IdToPiece, unknown tokens keep their surface (sentencepiece_processor.cc:609-621);
+    #      bos / eos / reverse through the encode frame, UNK_PIECE through unk_piece ----
     def EncodeAsPieces(self, input, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
         opts = self._options(add_bos, add_eos, reverse) + ["unk"] * bool(emit_unk_piece)
         single = isinstance(input, (str, bytes))
         buf, offs = pack_sentences([input] if single else input)
-        r = self._engine.encode_spans(buf, offs)
-        if self._pieces is None:
-            from . import _modelinfo
-            self._pieces, self._unk_id = _modelinfo.pieces_and_unk(self._model_bytes)
-        ids, te, ido, no, norm = r["ids"], r["tok_end"], r["id_offsets"], r["norm_offsets"], r["normalized"]
-        out = []
-        for i in range(len(offs) - 1):
-            base, begin, row = int(no[i]), 0, []
-            for k in range(int(ido[i]), int(ido[i + 1])):
-                end = int(te[k])
-                if int(ids[k]) == self._unk_id:
-                    row.append(norm[base + begin:base + end].decode("utf-8", errors="replace"))
-                else:
-                    row.append(self._pieces[int(ids[k])])
-                begin = end
-            out.append(self._apply_pieces(row, ids[int(ido[i]):int(ido[i + 1])].tolist(), opts) if opts else row)
+        self._set_frame(add_bos, add_eos, reverse)
+        unk = self._specials()["unk_piece"] if "unk" in opts else None
+        r = self._engine.encode_pieces(buf, offs, unk_piece=unk)
+        out = split_pieces(r["text"], r["text_offsets"], r["piece_end"], r["id_offsets"])
         return out[0] if single else out
-
-    def _apply_pieces(self, row, ids, opts):
-        """ApplyExtraOptions on piece strings (sentencepiece_processor.cc:1019-1064): the spans call returns the raw
-        segmentation, so the options are applied here."""
-        sp = self._specials()
-        pairs = list(zip(row, ids))
-        for o in opts:
-            if o == "reverse":
-                pairs.reverse()
-            elif o == "bos":
-                pairs.insert(0, (sp["bos_piece"], sp["bos_id"]))
-            elif o == "eos":
-                pairs.append((sp["eos_piece"], sp["eos_id"]))
-            elif o == "unk":
-                pairs = [(sp["unk_piece"], i) if i == self._unk_id else (p, i) for p, i in pairs]
-        return [p for p, _ in pairs]
 
     def encode(self, input, out_type=int, enable_sampling=False, nbest_size=-1, alpha=0.1, add_bos=False, add_eos=False,
                reverse=False, emit_unk_piece=False):
