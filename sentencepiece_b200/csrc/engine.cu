@@ -22,7 +22,9 @@
 #include <random>
 #include <thread>
 #include <string>
+#include <type_traits>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "../../include/spm_b200.h"
@@ -55,10 +57,27 @@ std::mutex g_create_mu;
     }                                                                                           \
   } while (0)
 
+// passes on the SPM_* code of a call that failed
+#define SPM_TRY(...)                                                                            \
+  do {                                                                                          \
+    const int rc__ = (__VA_ARGS__);                                                             \
+    if (rc__ != SPM_OK) return rc__;                                                            \
+  } while (0)
+
+// Device and pinned host buffers own their memory: moved, never copied, freed by their destructor.
 template <typename T>
 struct DevBuf {
   T *p = nullptr;
   size_t cap = 0;  // elements
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  DevBuf(DevBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  DevBuf &operator=(DevBuf &&o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~DevBuf() { release(); }
   cudaError_t ensure(size_t n, bool keep = false) {
     if (n <= cap) return cudaSuccess;
     size_t want = std::max(n, cap + cap / 2);
@@ -84,6 +103,15 @@ template <typename T>
 struct PinBuf {
   T *p = nullptr;
   size_t cap = 0;
+  PinBuf() = default;
+  PinBuf(const PinBuf &) = delete;
+  PinBuf &operator=(const PinBuf &) = delete;
+  PinBuf(PinBuf &&o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  PinBuf &operator=(PinBuf &&o) noexcept {
+    if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+    return *this;
+  }
+  ~PinBuf() { release(); }
   cudaError_t ensure(size_t n) {
     if (n <= cap) return cudaSuccess;
     size_t want = std::max(n, cap + cap / 2);
@@ -95,6 +123,17 @@ struct PinBuf {
     return e;
   }
   void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+};
+
+// a copy would free the same memory twice
+static_assert(!std::is_copy_constructible<DevBuf<int>>::value && !std::is_copy_constructible<PinBuf<int>>::value,
+              "buffers own their memory");
+
+// SPM_B200_TRACE: the chunked host paths print "[trace]" lines to stderr, stamped with the time since the call began.
+struct TraceClock {
+  const bool on = getenv("SPM_B200_TRACE") != nullptr;
+  const std::chrono::steady_clock::time_point t0 = std::chrono::steady_clock::now();
+  double ms() const { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(); }
 };
 
 bool valid_utf8(const char *s, size_t n) {
@@ -143,6 +182,20 @@ struct spm_engine {
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   std::mutex mu;
   mutable std::string err;
+  // Also takes down an engine that create_common gave up on part way.  The buffers free themselves after this body.
+  ~spm_engine() {
+    cudaSetDevice(device);
+    for (cudaStream_t s : {stream, s_h2d, s_d2h})
+      if (s) cudaStreamSynchronize(s);
+    for (cudaEvent_t x : ev)
+      if (x) cudaEventDestroy(x);
+    for (int k = 0; k < 2; ++k)
+      for (cudaEvent_t x : {ev_in[k], ev_out[k], ev_d2h[k]})
+        if (x) cudaEventDestroy(x);
+    if (ev_offs) cudaEventDestroy(ev_offs);
+    for (cudaStream_t s : {stream, s_h2d, s_d2h})
+      if (s) cudaStreamDestroy(s);
+  }
 
   ModelData model;
   DeviceTrie trie, user_trie;
@@ -168,7 +221,6 @@ struct spm_engine {
   // sentences with the cache emptied before every step (bench.py, H100 SXM at a 400 W limit, one run each): 2^20
   // 5.80 ms, 2^22 5.73 ms (256 MB of HBM), 2^24 5.93 ms (emptying 1 GB costs more than the extra hits save)
   int bpe_cache_log2 = 22;
-  bool fast_words = true;  // SPM_B200_FASTWORDS
   int upload_word_safe();
   KModel km{};
 
@@ -199,7 +251,19 @@ struct spm_engine {
   cudaStream_t s_h2d = nullptr, s_d2h = nullptr;
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr}, ev_d2h[2] = {nullptr, nullptr};
   int ensure_copy_streams();  // creates the copy streams and the slot events on first use
-  int grow_pinned_ids(unsigned long long have, uint64_t more, size_t done, size_t n);
+  // Makes the pinned result buffer `buf` hold `have` + `more` elements (rare), keeping the `have` that have already
+  // arrived from s_d2h; the new size extrapolates the elements per item of the first `done` of the batch's n items.
+  template <typename T>
+  int grow_pinned(PinBuf<T> &buf, unsigned long long have, uint64_t more, size_t done, size_t n) {
+    if (have + more + 1 <= buf.cap) return SPM_OK;
+    CUDA_TRY(cudaStreamSynchronize(s_d2h));
+    PinBuf<T> bigger;
+    const double per_item = static_cast<double>(have + more) / static_cast<double>(done);
+    CUDA_TRY(bigger.ensure(static_cast<size_t>(per_item * 1.25 * n) + more + 4096));
+    if (have) memcpy(bigger.p, buf.p, have * sizeof(T));
+    buf = std::move(bigger);
+    return SPM_OK;
+  }
   size_t pipeline_min_sentences = 300000, pipeline_chunk_sentences = 65536;
   DevBuf<uint32_t> d_order, d_order_hist;  // K0: length-bucketed processing order
   int build_order(const uint64_t *d_offs, size_t n, cudaStream_t st, const uint32_t **order, uint32_t seg);
@@ -221,7 +285,6 @@ struct spm_engine {
                            const uint64_t **id_offsets);
   int encode_host_fused(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids, const uint64_t **id_offsets);
   bool fused_host_path = true;
-  uint64_t fused_fallbacks = 0;
   int fused_skip = 0, fused_backoff = 8;
   DevBuf<uint32_t> d_seg_done, d_sent_rel;
   DevBuf<unsigned long long> d_seg_words;
@@ -297,6 +360,38 @@ struct spm_engine {
   PinBuf<uint64_t> h_dec_text_offsets;
   bool dec_ready = false;
   int ensure_decode_tables();
+  // decode_warp_kernel's arguments for n id lists (ids indexed by the values of id_offsets), results in d_dec_tmp
+  KDecode decode_args(const int32_t *ids, const uint64_t *id_offsets, uint32_t n, unsigned long long tmp_cap) const {
+    KDecode D{};
+    D.ids = ids;
+    D.id_offsets = reinterpret_cast<const unsigned long long *>(id_offsets);
+    D.n = n;
+    D.vocab = model.vocab_size();
+    D.dec_off = d_dec_off.p;
+    D.dec_bytes = d_dec_bytes.p;
+    D.dec_info = d_dec_info.p;
+    D.strip = (model.add_dummy_prefix || model.remove_extra_whitespaces) ? 1u : 0u;
+    D.rm = model.remove_extra_whitespaces ? 1u : 0u;
+    D.tmp = d_dec_tmp.p;
+    D.tmp_cap = tmp_cap;
+    D.cursor = d_ctrl64.p;
+    D.sent_start = d_sent_start.p;
+    D.sent_count = d_sent_count.p;
+    D.status = d_ctrl32.p;
+    return D;
+  }
+  // the error behind decode_warp_kernel's status word in h_ctrl32, or SPM_OK
+  int decode_error() const {
+    if (h_ctrl32.p[1] == 2u) {  // :915-918
+      set_error("Invalid id: " + std::to_string(static_cast<int32_t>(h_ctrl32.p[3])));
+      return SPM_ERR_ARG;
+    }
+    if (h_ctrl32.p[1] == 1u) {
+      set_error("Decode: byte piece of id " + std::to_string(h_ctrl32.p[3]) + " is not of the form <0xXX>");
+      return SPM_ERR_ENCODE;
+    }
+    return SPM_OK;
+  }
   // large host batches: chunked three-stage pipeline (staged H2D of the ids / decode kernels / D2H of the text)
   DevBuf<int32_t> p_dec_ids[2];
   DevBuf<uint8_t> p_dec_text[2];
@@ -398,9 +493,7 @@ struct spm_engine {
       ++last_launches;
       need.resize(m);
       CUDA_TRY(cudaMemcpyAsync(need.data(), d_long_need.p, m * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+      SPM_TRY(read_status(st, 16, 4));
       if (h_ctrl32.p[1]) return SPM_OK;
       for (uint32_t k = 0; k < m; ++k)
         if (need[k]) jobs.push_back(LongJob{jobs[lo + k].sent, jobs[lo + k].cap, need[k]});
@@ -425,6 +518,49 @@ struct spm_engine {
   float last_ms = 0.f, last_main_ms = 0.f;
 
   void set_error(const std::string &m) const { err = m; }
+
+  // Status words of the kernels (status, counters, cursors, scan totals): d_ctrl32 / d_ctrl64 and their pinned copies,
+  // kCtrlWords each, allocated by create_common.  copy_status queues the copy of the first n32 / n64 words on st;
+  // read_status also waits for it.
+  static constexpr size_t kCtrlWords = 16;
+  int copy_status(cudaStream_t st, size_t n32, size_t n64) {
+    if (n32) CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, n32 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, n64 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    return SPM_OK;
+  }
+  int read_status(cudaStream_t st, size_t n32, size_t n64) {
+    SPM_TRY(copy_status(st, n32, n64));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SPM_OK;
+  }
+
+  // Exclusive scan of n counts (kernels.cuh), each count plus `extra` and, with F, plus its frame's share.
+  // scan_total leaves the block prefixes in d_block_sums and the grand total at d_total (device memory); scan_gather
+  // then writes offsets[0..n] (+ off_base) and, when dst is given, copies item i's elements from src + src_start[i]
+  // (and src2 into dst2) to dst + offsets[i], within dst_cap.  Between the two a caller may read the total back to size
+  // dst.
+  int scan_total(const uint32_t *counts, uint32_t n, uint32_t extra, unsigned long long *d_total, cudaStream_t st,
+                 const KFrame *F = nullptr) {
+    const uint32_t nb = (n + kScanChunk - 1) / kScanChunk;
+    CUDA_TRY(d_block_sums.ensure(nb + 1));
+    if (F) scan_block_sums_kernel<true><<<nb, 256, 0, st>>>(counts, n, d_block_sums.p, extra, *F);
+    else scan_block_sums_kernel<<<nb, 256, 0, st>>>(counts, n, d_block_sums.p, extra);
+    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_total);
+    CUDA_TRY(cudaGetLastError());
+    last_launches += 2;
+    return SPM_OK;
+  }
+  template <typename ElemT, bool FRAMED = false>
+  int scan_gather(const uint32_t *counts, uint32_t n, unsigned long long *offsets, const unsigned long long *src_start,
+                  const ElemT *src, ElemT *dst, unsigned long long dst_cap, uint32_t extra, unsigned long long off_base,
+                  cudaStream_t st, const uint32_t *src2 = nullptr, uint32_t *dst2 = nullptr, const KFrame &F = KFrame{}) {
+    const uint32_t nb = (n + kScanChunk - 1) / kScanChunk;
+    scan_write_gather_kernel<ElemT, FRAMED><<<nb, 256, 0, st>>>(counts, n, d_block_sums.p, offsets, src_start, src, dst,
+                                                                src2, dst2, dst_cap, extra, off_base, F);
+    CUDA_TRY(cudaGetLastError());
+    ++last_launches;
+    return SPM_OK;
+  }
   int build_tables();
   int upload_types();
   int upload_node2();
@@ -697,7 +833,7 @@ int spm_engine::build_tables() {
 // most e edges of magnitude <= maxabs.
 int spm_engine::upload_word_safe() {
   std::vector<uint16_t> safe(trie_ws.link.size(), 0);
-  const bool eligible = fast_words && model.model_type == SPM_UNIGRAM && bpe_word_split && model.escape_whitespaces &&
+  const bool eligible = model.model_type == SPM_UNIGRAM && bpe_word_split && model.escape_whitespaces &&
                         !model.treat_whitespace_as_suffix && !any_user_defined && trie.max_key_len <= 62;
   km.flags &= ~kFlagFastWords;
   if (eligible) {
@@ -935,7 +1071,6 @@ int spm_engine::pick_fast_words_device(const uint8_t *d_bytes_base, const uint64
   if (force_fast_words >= 0) { *fast = force_fast_words != 0; return SPM_OK; }
   if (!(km.flags & kFlagFastWords) || n == 0) return SPM_OK;
   CUDA_TRY(d_sample.ensure(2));
-  CUDA_TRY(h_ctrl64.ensure(8));
   CUDA_TRY(cudaMemsetAsync(d_sample.p, 0, 2 * sizeof(unsigned long long), st));
   sample_spaces_kernel<<<16, 256, 0, st>>>(d_bytes_base, d_offs, static_cast<uint32_t>(n), d_sample.p);
   CUDA_TRY(cudaGetLastError());
@@ -1005,11 +1140,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
   CUDA_TRY(d_sent_start.ensure(n));
   CUDA_TRY(d_sent_count.ensure(n));
   CUDA_TRY(d_deferred.ensure(2 * n + 2));
-  CUDA_TRY(d_ctrl32.ensure(16));
   CUDA_TRY(d_deferred2.ensure(2 * n + 2));
-  CUDA_TRY(d_ctrl64.ensure(4));
-  CUDA_TRY(h_ctrl32.ensure(16));
-  CUDA_TRY(h_ctrl64.ensure(4));
   if (spans) {
     CUDA_TRY(d_norm_start.ensure(n));
     CUDA_TRY(d_norm_len.ensure(n));
@@ -1072,9 +1203,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     CUDA_TRY(cudaGetLastError());
     ++last_launches;
     CUDA_TRY(cudaEventRecord(ev[1], st));
-    CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    SPM_TRY(read_status(st, 16, 4));
     if (kstats) {
       unsigned long long ks[16];
       CUDA_TRY(cudaMemcpy(ks, d_kstats.p, sizeof ks, cudaMemcpyDeviceToHost));
@@ -1117,9 +1246,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       else encode_unigram_kernel<false><<<grid2, tile_threads, g2.smem_bytes, st>>>(M2, B2);
       CUDA_TRY(cudaGetLastError());
       ++last_launches;
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+      SPM_TRY(read_status(st, 16, 4));
       n_def = h_ctrl32.p[8];
       h_ctrl32.p[1] |= h_ctrl32.p[9];
       h_ctrl32.p[2] |= h_ctrl32.p[10];
@@ -1172,9 +1299,7 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
       }
       CUDA_TRY(cudaGetLastError());
       ++last_launches;
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+      SPM_TRY(read_status(st, 16, 4));
       h_ctrl32.p[1] |= h_ctrl32.p[9];
       h_ctrl32.p[2] |= h_ctrl32.p[10];
     }
@@ -1194,12 +1319,8 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
   if (h_ctrl32.p[2]) { set_error("temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
   // ---- offsets (exclusive scan) + compaction into sentence order; ids (not spans) get the encode frame ----
   const bool framed_ids = !spans && framed();
-  const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
-  CUDA_TRY(d_block_sums.ensure(nb + 1));
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, framed_ids ? frame_np + frame_ns : 0u);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_ctrl64.p + 2);
-  CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
+  SPM_TRY(scan_total(d_sent_count.p, n32, framed_ids ? frame_np + frame_ns : 0u, d_ctrl64.p + 2, st));
+  SPM_TRY(read_status(st, 0, 4));
   const unsigned long long tot = h_ctrl64.p[2];  // the cursor over-counts (chunked claims); the scan is exact
   *total_ids = tot;
   if (total_norm) *total_norm = spans ? h_ctrl64.p[1] : 0;
@@ -1219,35 +1340,25 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     return SPM_ERR_CAPACITY;
   }
   if (framed_ids)
-    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, off_out, d_sent_start.p,
-                                                                d_tmp_ids.p, ids_out, nullptr, nullptr, user_ids_cap, 0,
-                                                                off_base, kframe());
+    SPM_TRY(scan_gather<int32_t, true>(d_sent_count.p, n32, off_out, d_sent_start.p, d_tmp_ids.p, ids_out, user_ids_cap, 0,
+                                       off_base, st, nullptr, nullptr, kframe()));
   else
-    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(d_sent_count.p, n32, d_block_sums.p, off_out, d_sent_start.p,
-                                                          d_tmp_ids.p, ids_out,
-                                                          spans ? d_tmp_tok_end.p : nullptr, spans ? d_tok_end.p : nullptr,
-                                                          user_ids_cap, 0, off_base);
-  last_launches += 3;
+    SPM_TRY(scan_gather<int32_t>(d_sent_count.p, n32, off_out, d_sent_start.p, d_tmp_ids.p, ids_out, user_ids_cap, 0,
+                                 off_base, st, spans ? d_tmp_tok_end.p : nullptr, spans ? d_tok_end.p : nullptr));
   if (spans) {
     const unsigned long long tn = h_ctrl64.p[1];  // sum(n_i + 1)
     CUDA_TRY(d_norm.ensure(tn + 1));
     CUDA_TRY(d_n2o.ensure(tn + 1));
     CUDA_TRY(d_norm_offsets.ensure(n + 1));
     CUDA_TRY(d_n2o_offsets.ensure(n + 1));
-    scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_norm_len.p, n32, d_block_sums.p, 0);
-    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_ctrl64.p + 3);
-    scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(d_norm_len.p, n32, d_block_sums.p, d_norm_offsets.p,
-                                                          d_norm_start.p, d_tmp_norm.p, d_norm.p, nullptr, nullptr,
-                                                          d_norm.cap, 0, 0ull);
+    SPM_TRY(scan_total(d_norm_len.p, n32, 0, d_ctrl64.p + 3, st));
+    SPM_TRY(scan_gather<uint8_t>(d_norm_len.p, n32, d_norm_offsets.p, d_norm_start.p, d_tmp_norm.p, d_norm.p, d_norm.cap, 0,
+                                 0ull, st));
     // norm_to_orig has n_i + 1 entries per sentence: block sums of (len + 1)
-    scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_norm_len.p, n32, d_block_sums.p, 1);
-    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_ctrl64.p + 3);
-    scan_write_gather_kernel<uint32_t><<<nb, 256, 0, st>>>(d_norm_len.p, n32, d_block_sums.p, d_n2o_offsets.p,
-                                                           d_norm_start.p, d_tmp_n2o.p, d_n2o.p, nullptr, nullptr,
-                                                           d_n2o.cap, 1, 0ull);
-    last_launches += 6;
+    SPM_TRY(scan_total(d_norm_len.p, n32, 1, d_ctrl64.p + 3, st));
+    SPM_TRY(scan_gather<uint32_t>(d_norm_len.p, n32, d_n2o_offsets.p, d_norm_start.p, d_tmp_n2o.p, d_n2o.p, d_n2o.cap, 1,
+                                  0ull, st));
   }
-  CUDA_TRY(cudaGetLastError());
   CUDA_TRY(cudaEventRecord(ev[2], st));
   return SPM_OK;
 }
@@ -1261,20 +1372,6 @@ int spm_engine::ensure_copy_streams() {
     CUDA_TRY(cudaEventCreateWithFlags(&ev_out[k], cudaEventDisableTiming));
     CUDA_TRY(cudaEventCreateWithFlags(&ev_d2h[k], cudaEventDisableTiming));
   }
-  return SPM_OK;
-}
-
-// Makes the pinned result buffer hold `have` + `more` ids (rare), keeping the `have` ids that have already arrived;
-// the new size extrapolates the ids per sentence of the first `done` of the batch's n sentences.
-int spm_engine::grow_pinned_ids(unsigned long long have, uint64_t more, size_t done, size_t n) {
-  if (have + more + 1 <= h_ids.cap) return SPM_OK;
-  CUDA_TRY(cudaStreamSynchronize(s_d2h));
-  PinBuf<int32_t> bigger;
-  const double per_sent = static_cast<double>(have + more) / static_cast<double>(done);
-  CUDA_TRY(bigger.ensure(static_cast<size_t>(per_sent * 1.25 * n) + more + 4096));
-  if (have) memcpy(bigger.p, h_ids.p, have * sizeof(int32_t));
-  h_ids.release();
-  h_ids = bigger;
   return SPM_OK;
 }
 
@@ -1318,9 +1415,7 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
   const LaneGeom lgw = lane_geometry();
   const size_t warps = static_cast<size_t>(sm_count) * ctas_per_sm * ((lgw.ok ? lgw.threads : std::min(threads, 512)) / 32);
   const size_t groups_per_warp = is_bpe ? 2 : 1;
-  const bool trace = getenv("SPM_B200_TRACE") != nullptr;
-  const auto t_begin = std::chrono::steady_clock::now();
-  auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
+  const TraceClock trace;
   const size_t chunk = std::max<size_t>(pipeline_chunk_sentences, warps * 32 * groups_per_warp);
   const size_t C = (n + chunk - 1) / chunk;
   const uint64_t total_bytes = offsets[n] - offsets[0];
@@ -1349,7 +1444,7 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
   uint64_t launches = 0, deferred = 0;
   float main_ms = 0.f, all_ms = 0.f;
   unsigned long long id_base = 0;
-  if (trace) fprintf(stderr, "[trace] setup done at %.3f ms\n", now_ms());
+  if (trace.on) fprintf(stderr, "[trace] setup done at %.3f ms\n", trace.ms());
   { const int rc = issue_h2d(0); if (rc) return rc; }
   for (size_t c = 0; c < C; ++c) {
     const int k = static_cast<int>(c & 1);
@@ -1361,24 +1456,24 @@ int spm_engine::encode_host_pipelined(const char *bytes, const uint64_t *offsets
     const int rc = run_device(p_bytes[k].p - offsets[lo], p_offsets[k].p, hi - lo, offsets[hi] - offsets[lo], false, nullptr, 0,
                               nullptr, &tot, nullptr, stream, &p_ids[k], &p_id_offsets[k], id_base);
     if (rc) { cudaDeviceSynchronize(); return rc; }
-    const double t_ret = trace ? now_ms() : 0.0;
+    const double t_ret = trace.on ? trace.ms() : 0.0;
     CUDA_TRY(cudaEventRecord(ev_out[k], stream));
     launches += last_launches;
     deferred += last_deferred;
-    { const int rc2 = grow_pinned_ids(id_base, tot, hi, n); if (rc2) return rc2; }
+    SPM_TRY(grow_pinned(h_ids, id_base, tot, hi, n));
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_ids.p + id_base, p_ids[k].p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_id_offsets.p + lo, p_id_offsets[k].p, (hi - lo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaEventRecord(ev_d2h[k], s_d2h));
     float a = 0.f;
     if (cudaEventElapsedTime(&a, ev[0], ev[1]) == cudaSuccess) { main_ms += a; all_ms += a; }
-    if (trace) fprintf(stderr, "[trace] chunk %zu: run_device returned at %.3f ms (encode kernel %.3f ms), D2H issued at %.3f ms\n", c,
-                       t_ret, a, now_ms());
+    if (trace.on) fprintf(stderr, "[trace] chunk %zu: run_device returned at %.3f ms (encode kernel %.3f ms), D2H issued at %.3f ms\n", c,
+                       t_ret, a, trace.ms());
     id_base += tot;
   }
-  if (trace) fprintf(stderr, "[trace] all chunks issued at %.3f ms\n", now_ms());
+  if (trace.on) fprintf(stderr, "[trace] all chunks issued at %.3f ms\n", trace.ms());
   CUDA_TRY(cudaStreamSynchronize(s_d2h));
-  if (trace) fprintf(stderr, "[trace] results on host at %.3f ms (%zu chunks of %zu)\n", now_ms(), C, chunk);
+  if (trace.on) fprintf(stderr, "[trace] results on host at %.3f ms (%zu chunks of %zu)\n", trace.ms(), C, chunk);
   last_launches = launches;
   last_deferred = deferred;
   last_main_ms = main_ms;
@@ -1401,9 +1496,7 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
   CUDA_TRY(cudaSetDevice(device));
   { const int rc = ensure_copy_streams(); if (rc) return rc; }
   if (!ev_offs) CUDA_TRY(cudaEventCreateWithFlags(&ev_offs, cudaEventDisableTiming));
-  const bool trace = getenv("SPM_B200_TRACE") != nullptr;
-  const auto t_begin = std::chrono::steady_clock::now();
-  auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
+  const TraceClock trace;
   constexpr uint32_t kPieceShift = 15;
   constexpr size_t kPiece = size_t{1} << kPieceShift;
   const size_t P = (n + kPiece - 1) / kPiece;
@@ -1454,25 +1547,25 @@ int spm_engine::encode_host_streamed(const char *bytes, const uint64_t *offsets,
                               nullptr, &tot, nullptr, stream, &p_ids[k], &p_id_offsets[k], id_base);
     cur_ready = nullptr;
     if (rc) { cudaDeviceSynchronize(); return rc; }
-    const double t_ret = trace ? now_ms() : 0.0;
+    const double t_ret = trace.on ? trace.ms() : 0.0;
     CUDA_TRY(cudaEventRecord(ev_out[k], stream));
     launches += last_launches;
     deferred += last_deferred;
-    { const int rc2 = grow_pinned_ids(id_base, tot, hi, n); if (rc2) return rc2; }
+    SPM_TRY(grow_pinned(h_ids, id_base, tot, hi, n));
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_ids.p + id_base, p_ids[k].p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_id_offsets.p + lo, p_id_offsets[k].p, (hi - lo + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaEventRecord(ev_d2h[k], s_d2h));
     float a = 0.f;
     if (cudaEventElapsedTime(&a, ev[0], ev[1]) == cudaSuccess) { main_ms += a; all_ms += a; }
-    if (trace) fprintf(stderr, "[trace] chunk %zu (%zu sentences): run_device returned at %.3f ms (encode kernel %.3f ms)\n", c,
+    if (trace.on) fprintf(stderr, "[trace] chunk %zu (%zu sentences): run_device returned at %.3f ms (encode kernel %.3f ms)\n", c,
                        hi - lo, t_ret, a);
     id_base += tot;
   }
   feeder.join();
   if (feed_rc) { cudaDeviceSynchronize(); set_error("host-to-device copy of a streamed batch failed"); return SPM_ERR_CUDA; }
   CUDA_TRY(cudaStreamSynchronize(s_d2h));
-  if (trace) fprintf(stderr, "[trace] results on host at %.3f ms\n", now_ms());
+  if (trace.on) fprintf(stderr, "[trace] results on host at %.3f ms\n", trace.ms());
   last_launches = launches;
   last_deferred = deferred;
   last_main_ms = main_ms;
@@ -1494,9 +1587,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(cudaSetDevice(device));
   { const int rc = ensure_copy_streams(); if (rc) return rc; }
   if (!ev_offs) CUDA_TRY(cudaEventCreateWithFlags(&ev_offs, cudaEventDisableTiming));
-  const bool trace = getenv("SPM_B200_TRACE") != nullptr;
-  const auto t_begin = std::chrono::steady_clock::now();
-  auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
+  const TraceClock trace;
   constexpr uint32_t kPieceShift = 15;
   constexpr uint32_t kSegShift = 10;
   const size_t kPiece = size_t{1} << kPieceShift;
@@ -1519,10 +1610,6 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(d_sent_count.ensure(n));
   CUDA_TRY(d_sent_rel.ensure(n));
   CUDA_TRY(d_deferred.ensure(2 * n + 2));
-  CUDA_TRY(d_ctrl32.ensure(16));
-  CUDA_TRY(d_ctrl64.ensure(16));
-  CUDA_TRY(h_ctrl32.ensure(16));
-  CUDA_TRY(h_ctrl64.ensure(16));
   CUDA_TRY(d_seg_done.ensure(2 * S + 4));   // groups finished [S], copied flags [S], drained counter
   CUDA_TRY(d_seg_words.ensure(2 * S));
   CUDA_TRY(d_ids.ensure(h_ids.cap));
@@ -1587,7 +1674,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   B.drained_upto = d_seg_done.p + 2 * S;
   B.out_cap = std::min<unsigned long long>(h_ids.cap, d_ids.cap);
   B.out_off_base = 0;
-  B.kstats = trace ? d_ctrl64.p + 4 : nullptr;
+  B.kstats = trace.on ? d_ctrl64.p + 4 : nullptr;
   B.frame = kframe();
   CUDA_TRY(cudaEventRecord(ev[0], st));
   // processing order: sorted within each drain segment.  Sorting whole input pieces instead makes all 32 segments of a
@@ -1604,8 +1691,8 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   CUDA_TRY(cudaEventRecord(ev[1], st));
   CUDA_TRY(cudaEventRecord(ev[2], st));
   CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  if (trace) CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  if (trace) fprintf(stderr, "[trace] fused kernel launched at %.3f ms\n", now_ms());
+  if (trace.on) CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  if (trace.on) fprintf(stderr, "[trace] fused kernel launched at %.3f ms\n", trace.ms());
   // the offsets are checked while the GPU works (a decreasing pair only makes the kernels defer that sentence: the
   // lengths are taken as unsigned); a bad batch is reported after the launch has drained
   uint64_t bad = 0;
@@ -1627,10 +1714,10 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   }
   CUDA_TRY(cudaStreamSynchronize(st));
   feeder.join();
-  if (trace) fprintf(stderr, "[trace] fused kernel done at %.3f ms; warp-cycles: input wait %.1f M, compaction %.1f M (look-back %.1f M), "
-                     "%llu groups on %zu warps\n", now_ms(), h_ctrl64.p[4] * 1e-6, h_ctrl64.p[5] * 1e-6, h_ctrl64.p[6] * 1e-6,
+  if (trace.on) fprintf(stderr, "[trace] fused kernel done at %.3f ms; warp-cycles: input wait %.1f M, compaction %.1f M (look-back %.1f M), "
+                     "%llu groups on %zu warps\n", trace.ms(), h_ctrl64.p[4] * 1e-6, h_ctrl64.p[5] * 1e-6, h_ctrl64.p[6] * 1e-6,
                      static_cast<unsigned long long>(h_ctrl64.p[7]), warps_total);
-  if (trace) {
+  if (trace.on) {
     float km = 0.f;
     cudaEventElapsedTime(&km, ev[0], ev[1]);
     const double w = 1e-6 / warps_total;  // M cycles per warp
@@ -1645,10 +1732,9 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   if (h_ctrl32.p[1]) { set_error("encode failed: internal consistency check (status " + std::to_string(h_ctrl32.p[1]) + ")"); return SPM_ERR_ENCODE; }
   if (h_ctrl32.p[0] || h_ctrl32.p[2]) {
     // deferred sentences or a buffer that was too small: the chunked path has the second-chance and retry logic
-    if (trace) fprintf(stderr, "[trace] fused path incomplete (deferred %u, overflow %u): redoing the batch in chunks\n",
+    if (trace.on) fprintf(stderr, "[trace] fused path incomplete (deferred %u, overflow %u): redoing the batch in chunks\n",
                        h_ctrl32.p[0], h_ctrl32.p[2]);
     CUDA_TRY(cudaStreamSynchronize(s_d2h));
-    fused_fallbacks++;
     // data like this (long words, very long lines) tends to come in runs: go chunked for a while, longer each time
     fused_skip = fused_backoff;
     fused_backoff = std::min(fused_backoff * 4, 1 << 16);
@@ -1658,7 +1744,7 @@ int spm_engine::encode_host_fused(const char *bytes, const uint64_t *offsets, si
   const uint64_t tot = h_id_offsets.p[n];
   if (tot > copied) CUDA_TRY(cudaMemcpyAsync(h_ids.p + copied, d_ids.p + copied, (tot - copied) * sizeof(int32_t), cudaMemcpyDeviceToHost, s_d2h));
   CUDA_TRY(cudaStreamSynchronize(s_d2h));
-  if (trace) fprintf(stderr, "[trace] ids on host at %.3f ms (%llu of %llu fetched while encoding)\n", now_ms(),
+  if (trace.on) fprintf(stderr, "[trace] ids on host at %.3f ms (%llu of %llu fetched while encoding)\n", trace.ms(),
                      static_cast<unsigned long long>(copied), static_cast<unsigned long long>(tot));
   float a = 0.f;
   if (cudaEventElapsedTime(&a, ev[0], ev[1]) != cudaSuccess) a = 0.f;
@@ -1764,9 +1850,7 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
                                       const uint64_t **text_offsets) {
   { const int rc = ensure_copy_streams(); if (rc) return rc; }
   cudaStream_t st = stream;
-  const bool trace = getenv("SPM_B200_TRACE") != nullptr;
-  const auto t_begin = std::chrono::steady_clock::now();
-  auto now_ms = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
+  const TraceClock trace;
   const size_t chunk = 131072;
   const size_t C = (n + chunk - 1) / chunk;
   const bool pinned_in = is_pinned(ids);
@@ -1783,12 +1867,6 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
   CUDA_TRY(h_dec_text.ensure(std::max<size_t>(h_dec_text.cap, total_ids * 5 + 16 * n + 4096)));
   CUDA_TRY(d_sent_start.ensure(chunk));
   CUDA_TRY(d_sent_count.ensure(chunk));
-  CUDA_TRY(d_ctrl32.ensure(16));
-  CUDA_TRY(d_ctrl64.ensure(8));
-  CUDA_TRY(h_ctrl32.ensure(16));
-  CUDA_TRY(h_ctrl64.ensure(8));
-  const uint32_t nb_max = (static_cast<uint32_t>(chunk) + kScanChunk - 1) / kScanChunk;
-  CUDA_TRY(d_block_sums.ensure(nb_max + 1));
   auto issue_h2d = [&](size_t c) -> int {
     const int k = static_cast<int>(c & 1);
     const size_t lo = c * chunk, hi = std::min(n, lo + chunk);
@@ -1807,7 +1885,7 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
     CUDA_TRY(cudaEventRecord(ev_in[k], s_h2d));
     return SPM_OK;
   };
-  uint64_t launches = 0;
+  last_launches = 0;
   float main_ms = 0.f, all_ms = 0.f;  // decode kernels; scan + gather kernels
   unsigned long long text_base = 0;
   { const int rc = issue_h2d(0); if (rc) return rc; }
@@ -1825,77 +1903,39 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
       CUDA_TRY(d_dec_tmp.ensure(tmp_cap));
       CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
       CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 8 * sizeof(unsigned long long), st));
-      KDecode D{};
-      D.ids = p_dec_ids[k].p - id_offsets[lo];
-      D.id_offsets = reinterpret_cast<const unsigned long long *>(p_offsets[k].p);
-      D.n = m;
-      D.vocab = model.vocab_size();
-      D.dec_off = d_dec_off.p;
-      D.dec_bytes = d_dec_bytes.p;
-      D.dec_info = d_dec_info.p;
-      D.strip = (model.add_dummy_prefix || model.remove_extra_whitespaces) ? 1u : 0u;
-      D.rm = model.remove_extra_whitespaces ? 1u : 0u;
-      D.tmp = d_dec_tmp.p;
-      D.tmp_cap = tmp_cap;
-      D.cursor = d_ctrl64.p;
-      D.sent_start = d_sent_start.p;
-      D.sent_count = d_sent_count.p;
-      D.status = d_ctrl32.p;
       CUDA_TRY(cudaEventRecord(ev[0], st));
       const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (m + 7) / 8));
-      decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+      decode_warp_kernel<<<grid, 256, 0, st>>>(decode_args(p_dec_ids[k].p - id_offsets[lo], p_offsets[k].p, m, tmp_cap));
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaEventRecord(ev[1], st));
-      ++launches;
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      ++last_launches;
+      SPM_TRY(copy_status(st, 16, 8));
       // the next chunk's ids are staged / queued while this chunk's kernel runs
       if (!staged_next && c + 1 < C) { const int rc = issue_h2d(c + 1); if (rc) { cudaDeviceSynchronize(); return rc; } }
       staged_next = true;
       CUDA_TRY(cudaStreamSynchronize(st));
       float a = 0.f;
       if (cudaEventElapsedTime(&a, ev[0], ev[1]) == cudaSuccess) main_ms += a;
-      if (trace) fprintf(stderr, "[trace] decode chunk %zu: kernel done at %.3f ms (kernel %.3f ms, input %s)\n", c, now_ms(), a,
+      if (trace.on) fprintf(stderr, "[trace] decode chunk %zu: kernel done at %.3f ms (kernel %.3f ms, input %s)\n", c, trace.ms(), a,
                          pinned_in ? "pinned" : "pageable, staged");
-      if (h_ctrl32.p[1] == 2u) {  // :915-918
-        cudaDeviceSynchronize();
-        set_error("Invalid id: " + std::to_string(static_cast<int32_t>(h_ctrl32.p[3])));
-        return SPM_ERR_ARG;
-      }
-      if (h_ctrl32.p[1] == 1u) {
-        cudaDeviceSynchronize();
-        set_error("Decode: byte piece of id " + std::to_string(h_ctrl32.p[3]) + " is not of the form <0xXX>");
-        return SPM_ERR_ENCODE;
-      }
+      if (const int rc = decode_error()) { cudaDeviceSynchronize(); return rc; }
       tot = h_ctrl64.p[0];
       if (h_ctrl32.p[2]) { tmp_cap = tot + 1024; continue; }
       break;
     }
     if (h_ctrl32.p[2]) { cudaDeviceSynchronize(); set_error("Decode: temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
-    const uint32_t nb = (m + kScanChunk - 1) / kScanChunk;
     CUDA_TRY(p_dec_text[k].ensure(tot + 16));
     if (c > 0) {  // the previous chunk's scan + gather finished before this chunk's kernel did
       float g = 0.f;
       if (cudaEventElapsedTime(&g, ev[2], ev[3]) == cudaSuccess) all_ms += g;
     }
     CUDA_TRY(cudaEventRecord(ev[2], st));
-    scan_block_sums_kernel<<<nb, 256, 0, st>>>(d_sent_count.p, m, d_block_sums.p, 0);
-    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(d_block_sums.p, nb, d_ctrl64.p + 2);
-    scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(d_sent_count.p, m, d_block_sums.p, p_dec_toff[k].p, d_sent_start.p,
-                                                          d_dec_tmp.p, p_dec_text[k].p, nullptr, nullptr, p_dec_text[k].cap, 0,
-                                                          text_base);
-    CUDA_TRY(cudaGetLastError());
-    launches += 3;
+    SPM_TRY(scan_total(d_sent_count.p, m, 0, d_ctrl64.p + 2, st));
+    SPM_TRY(scan_gather<uint8_t>(d_sent_count.p, m, p_dec_toff[k].p, d_sent_start.p, d_dec_tmp.p, p_dec_text[k].p,
+                                 p_dec_text[k].cap, 0, text_base, st));
     CUDA_TRY(cudaEventRecord(ev[3], st));
     CUDA_TRY(cudaEventRecord(ev_out[k], st));
-    if (text_base + tot + 1 > h_dec_text.cap) {  // grow the pinned result buffer (rare): keep what has already arrived
-      CUDA_TRY(cudaStreamSynchronize(s_d2h));
-      PinBuf<char> bigger;
-      CUDA_TRY(bigger.ensure(static_cast<size_t>(static_cast<double>(text_base + tot) / static_cast<double>(hi) * 1.25 * n) + tot + 4096));
-      if (text_base) memcpy(bigger.p, h_dec_text.p, text_base);
-      h_dec_text.release();
-      h_dec_text = bigger;
-    }
+    SPM_TRY(grow_pinned(h_dec_text, text_base, tot, hi, n));
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_dec_text.p + text_base, p_dec_text[k].p, tot, cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_dec_text_offsets.p + lo, p_dec_toff[k].p, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
@@ -1903,13 +1943,12 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
     text_base += tot;
   }
   CUDA_TRY(cudaStreamSynchronize(s_d2h));
-  if (trace) fprintf(stderr, "[trace] decode: text on host at %.3f ms (%zu chunks)\n", now_ms(), C);
+  if (trace.on) fprintf(stderr, "[trace] decode: text on host at %.3f ms (%zu chunks)\n", trace.ms(), C);
   {
     float g = 0.f;
     if (cudaEventElapsedTime(&g, ev[2], ev[3]) == cudaSuccess) all_ms += g;
   }
   h_dec_text.p[text_base] = 0;
-  last_launches = launches;
   last_main_ms = main_ms;
   last_ms = main_ms + all_ms;
   last_h2d = total_ids * sizeof(int32_t) + (n + C) * sizeof(uint64_t);
@@ -1967,10 +2006,6 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
   CUDA_TRY(d_cand_count.ensure(nc));
   CUDA_TRY(d_cand_score.ensure(nc));
   CUDA_TRY(d_n_cands.ensure(n));
-  CUDA_TRY(d_ctrl32.ensure(16));
-  CUDA_TRY(d_ctrl64.ensure(4));
-  CUDA_TRY(h_ctrl32.ensure(16));
-  CUDA_TRY(h_ctrl64.ensure(4));
   // candidates: at most one id per normalized byte each; start from 2 ids per input byte per 8 candidates
   unsigned long long tmp_cap = std::max<unsigned long long>(1u << 20, total_bytes * nbest / 3 + 64ull * n);
   for (int attempt = 0; attempt < 4; ++attempt) {
@@ -2002,9 +2037,7 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(ev[1], st));
     ++last_launches;
-    CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    SPM_TRY(read_status(st, 16, 4));
     last_deferred = h_ctrl32.p[0];
     if (h_ctrl32.p[0] && !h_ctrl32.p[1]) {
       // ---- sentences the lane kernel deferred (long, large lattice, pool or agenda full): warp per sentence ----
@@ -2044,10 +2077,6 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
   lat_ids.clear();
   lat_scores.clear();
   lat_offsets.assign(1, 0);
-  CUDA_TRY(d_ctrl32.ensure(16));
-  CUDA_TRY(d_ctrl64.ensure(4));
-  CUDA_TRY(h_ctrl32.ensure(16));
-  CUDA_TRY(h_ctrl64.ensure(4));
   LatticeGeom G{};
   G.cap = lane_cap;
   G.node_cap = lane_cap * (trie.max_matches_per_start + 1) + 64;
@@ -2114,9 +2143,7 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaEventRecord(ev[1], st));
       ++last_launches;
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl32.p, d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaMemcpyAsync(h_ctrl64.p, d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+      SPM_TRY(read_status(st, 16, 4));
       float a = 0.f;
       if (cudaEventElapsedTime(&a, ev[0], ev[1]) == cudaSuccess) main_ms += a;
       const uint32_t n_def = h_ctrl32.p[0];
@@ -2270,6 +2297,10 @@ static int create_common(spm_engine *e, int device, spm_engine **out) {
   if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return fail(SPM_ERR_CUDA, "stream creation failed");
   for (auto &ev : e->ev)
     if (cudaEventCreate(&ev) != cudaSuccess) return fail(SPM_ERR_CUDA, "event creation failed");
+  const size_t w = spm_engine::kCtrlWords;
+  if (e->d_ctrl32.ensure(w) != cudaSuccess || e->d_ctrl64.ensure(w) != cudaSuccess || e->h_ctrl32.ensure(w) != cudaSuccess ||
+      e->h_ctrl64.ensure(w) != cudaSuccess)
+    return fail(SPM_ERR_CUDA, "status word allocation failed");
   rc = e->configure_kernel_attrs();
   if (rc) return fail(rc, e->err);
   *out = e;
@@ -2315,54 +2346,7 @@ int spm_engine_create_from_serialized(const void *model_proto, size_t len, int d
   return create_common(e, device, out);
 }
 
-void spm_engine_destroy(spm_engine *e) {
-  if (!e) return;
-  cudaSetDevice(e->device);
-  if (e->stream) cudaStreamSynchronize(e->stream);
-  e->d_link.release(); e->d_val.release(); e->d_user_link.release(); e->d_cm_units.release(); e->d_cm_lead.release();
-  e->d_cm_pair.release(); e->d_id.release(); e->d_id_ws.release(); e->d_cm_solo.release(); e->d_byte_to_id.release(); e->d_cm_targets.release();
-  e->d_types.release(); e->d_scores.release(); e->d_word_safe.release(); e->d_node4.release(); e->d_word_fast.release(); e->d_bpe_cache.release(); e->d_kstats.release(); e->d_sample.release(); e->d_bytes.release(); e->d_tmp_norm.release(); e->d_norm.release();
-  e->d_long_scratch.release(); e->d_offsets.release(); e->d_tmp_ids.release(); e->d_ids.release();
-  e->d_tmp_tok_end.release(); e->d_tok_end.release(); e->d_tmp_n2o.release(); e->d_n2o.release();
-  e->d_sent_count.release(); e->d_norm_len.release(); e->d_deferred.release(); e->d_deferred2.release(); e->d_long_list.release();
-  e->d_ctrl32.release(); e->d_sent_start.release(); e->d_norm_start.release(); e->d_id_offsets.release();
-  e->d_norm_offsets.release(); e->d_n2o_offsets.release(); e->d_block_sums.release(); e->d_ctrl64.release();
-  e->d_long_off.release();
-  e->d_lane_slabs.release(); e->d_bpe_long.release();
-  e->d_node2.release();
-  e->d_lat_scratch.release(); e->d_lat_nodes.release(); e->d_lat_pos.release(); e->d_lat_node_start.release();
-  e->d_lat_pos_start.release(); e->d_lat_nchars.release(); e->d_lat_entropy.release(); e->h_lat_nodes.release();
-  e->h_lat_pos.release(); e->h_lat_node_start.release(); e->h_lat_pos_start.release(); e->h_lat_nchars.release();
-  e->h_lat_entropy.release();
-  e->d_nb_scratch.release(); e->d_cand_start.release(); e->d_cand_offsets.release(); e->d_cand_count.release();
-  e->d_n_cands.release(); e->d_picks.release(); e->d_cand_score.release(); e->h_cand_score.release();
-  e->h_n_cands.release(); e->h_picks.release(); e->h_cand_offsets.release();
-  for (int k = 0; k < 2; ++k) {
-    e->p_bytes[k].release(); e->p_offsets[k].release(); e->p_ids[k].release(); e->p_id_offsets[k].release();
-    if (e->ev_in[k]) cudaEventDestroy(e->ev_in[k]);
-    if (e->ev_out[k]) cudaEventDestroy(e->ev_out[k]);
-    if (e->ev_d2h[k]) cudaEventDestroy(e->ev_d2h[k]);
-  }
-  e->s_bytes.release(); e->s_offsets.release(); e->d_ready.release(); e->h_marks.release(); e->h_progress.release();
-  e->d_dec_off.release(); e->d_dec_info.release(); e->d_dec_bytes.release(); e->d_dec_tmp.release(); e->d_dec_text.release();
-  e->d_dec_ids.release(); e->d_dec_text_offsets.release(); e->h_dec_text.release(); e->h_dec_text_offsets.release();
-  for (int k = 0; k < 2; ++k) { e->p_dec_ids[k].release(); e->p_dec_text[k].release(); e->p_dec_toff[k].release(); e->h_stage[k].release(); }
-  e->d_pc_off.release(); e->d_pc_flag.release(); e->d_pc_sub_of.release(); e->d_pc_sub_len.release(); e->d_pc_text_len.release();
-  e->d_pc_ntok.release(); e->d_pc_end.release(); e->d_pc_bytes.release(); e->d_pc_unk.release(); e->d_pc_sub_bytes.release();
-  e->d_pc_text.release(); e->d_pc_ids.release(); e->d_pc_out_ids.release(); e->d_pc_id_offsets.release(); e->d_pc_pos.release();
-  e->d_pc_sub_start.release(); e->d_pc_sub_offsets.release(); e->d_pc_text_offsets.release(); e->d_pc_out_id_offsets.release();
-  e->h_pc_text.release(); e->h_pc_text_offsets.release(); e->h_pc_end.release();
-  e->d_frame.release();
-  e->d_order.release(); e->d_order_hist.release(); e->d_seg_done.release(); e->d_sent_rel.release(); e->d_seg_words.release();
-  if (e->ev_offs) cudaEventDestroy(e->ev_offs);
-  if (e->s_h2d) cudaStreamDestroy(e->s_h2d);
-  if (e->s_d2h) cudaStreamDestroy(e->s_d2h);
-  e->h_ids.release(); e->h_tok_end.release(); e->h_n2o.release(); e->h_ctrl32.release(); e->h_deferred.release();
-  e->h_id_offsets.release(); e->h_norm_offsets.release(); e->h_ctrl64.release(); e->h_norm.release();
-  for (auto &ev : e->ev) if (ev) cudaEventDestroy(ev);
-  if (e->stream) cudaStreamDestroy(e->stream);
-  delete e;
-}
+void spm_engine_destroy(spm_engine *e) { delete e; }
 
 int spm_engine_set_types(spm_engine *e, const uint8_t *types) {
   if (!e || !types) return SPM_ERR_ARG;
@@ -2466,10 +2450,6 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
   CUDA_TRY(e->d_offsets.ensure(n + 1));
   CUDA_TRY(e->d_sent_start.ensure(n));
   CUDA_TRY(e->d_sent_count.ensure(n));
-  CUDA_TRY(e->d_ctrl32.ensure(16));
-  CUDA_TRY(e->d_ctrl64.ensure(8));
-  CUDA_TRY(e->h_ctrl32.ensure(16));
-  CUDA_TRY(e->h_ctrl64.ensure(8));
   CUDA_TRY(e->d_dec_text_offsets.ensure(n + 1));
   if (total_ids) CUDA_TRY(cudaMemcpyAsync(e->d_dec_ids.p, ids + base, total_ids * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(e->d_offsets.p, id_offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
@@ -2481,55 +2461,24 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
     CUDA_TRY(e->d_dec_tmp.ensure(tmp_cap));
     CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(e->d_ctrl64.p, 0, 8 * sizeof(unsigned long long), st));
-    KDecode D{};
-    D.ids = e->d_dec_ids.p - base;
-    D.id_offsets = reinterpret_cast<const unsigned long long *>(e->d_offsets.p);
-    D.n = n32;
-    D.vocab = e->model.vocab_size();
-    D.dec_off = e->d_dec_off.p;
-    D.dec_bytes = e->d_dec_bytes.p;
-    D.dec_info = e->d_dec_info.p;
-    D.strip = (e->model.add_dummy_prefix || e->model.remove_extra_whitespaces) ? 1u : 0u;
-    D.rm = e->model.remove_extra_whitespaces ? 1u : 0u;
-    D.tmp = e->d_dec_tmp.p;
-    D.tmp_cap = tmp_cap;
-    D.cursor = e->d_ctrl64.p;
-    D.sent_start = e->d_sent_start.p;
-    D.sent_count = e->d_sent_count.p;
-    D.status = e->d_ctrl32.p;
     CUDA_TRY(cudaEventRecord(e->ev[0], st));
     const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
-    decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+    decode_warp_kernel<<<grid, 256, 0, st>>>(e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap));
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaEventRecord(e->ev[1], st));
     ++e->last_launches;
-    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl32.p, e->d_ctrl32.p, 16 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 8 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    if (e->h_ctrl32.p[1] == 2u) {  // :915-918
-      set_error("Invalid id: " + std::to_string(static_cast<int32_t>(e->h_ctrl32.p[3])));
-      return SPM_ERR_ARG;
-    }
-    if (e->h_ctrl32.p[1] == 1u) {
-      set_error("Decode: byte piece of id " + std::to_string(e->h_ctrl32.p[3]) + " is not of the form <0xXX>");
-      return SPM_ERR_ENCODE;
-    }
+    SPM_TRY(e->read_status(st, 16, 8));
+    SPM_TRY(e->decode_error());
     tot = e->h_ctrl64.p[0];
     if (e->h_ctrl32.p[2]) { tmp_cap = tot + 1024; continue; }
     break;
   }
   if (e->h_ctrl32.p[2]) { set_error("Decode: temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
   // offsets (exclusive scan) + gather into list order: the kernels of the encode path
-  const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
-  CUDA_TRY(e->d_block_sums.ensure(nb + 1));
   CUDA_TRY(e->d_dec_text.ensure(tot + 16));
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, 0);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
-  scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_dec_text_offsets.p,
-                                                        e->d_sent_start.p, e->d_dec_tmp.p, e->d_dec_text.p, nullptr, nullptr,
-                                                        e->d_dec_text.cap, 0, 0ull);
-  CUDA_TRY(cudaGetLastError());
-  e->last_launches += 3;
+  SPM_TRY(e->scan_total(e->d_sent_count.p, n32, 0, e->d_ctrl64.p + 2, st));
+  SPM_TRY(e->scan_gather<uint8_t>(e->d_sent_count.p, n32, e->d_dec_text_offsets.p, e->d_sent_start.p, e->d_dec_tmp.p,
+                                  e->d_dec_text.p, e->d_dec_text.cap, 0, 0ull, st));
   CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(e->h_dec_text.ensure(tot + 1));
   if (tot) CUDA_TRY(cudaMemcpyAsync(e->h_dec_text.p, e->d_dec_text.p, tot, cudaMemcpyDeviceToHost, st));
@@ -2698,10 +2647,6 @@ static int encode_host_locked(spm_engine *e, const char *bytes, const uint64_t *
   return SPM_OK;
 }
 
-static int encode_host_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, bool spans,
-                              const int32_t **ids, const uint32_t **tok_end, const uint64_t **id_offsets,
-                              const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o);
-
 // spm_encode_ids with e->mu already held (also used by the n-best / sampling entry points for nbest_size <= 1)
 static int encode_ids_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
                              const uint64_t **id_offsets) {
@@ -2777,31 +2722,22 @@ int spm_nbest_encode(spm_engine *e, const char *bytes, const uint64_t *offsets, 
   { const int rc = e->run_nbest(bytes, offsets, n, K, &tmp_total); if (rc) return rc; }
   // candidate-major compaction: the shared scan + gather over n*K counts; every candidate gets the encode frame
   const uint32_t nc32 = static_cast<uint32_t>(nc);
-  const uint32_t nb = (nc32 + kScanChunk - 1) / kScanChunk;
   const bool framed = e->framed();
   const KFrame F = e->kframe(e->d_n_cands.p, K);
-  CUDA_TRY(e->d_block_sums.ensure(nb + 1));
   CUDA_TRY(e->d_cand_offsets.ensure(nc + 1));
-  if (framed) scan_block_sums_kernel<true><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, 0, F);
-  else scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, 0);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
+  SPM_TRY(e->scan_total(e->d_cand_count.p, nc32, 0, e->d_ctrl64.p + 2, st, framed ? &F : nullptr));
   uint64_t total = tmp_total;
   if (framed) {  // the frame's share depends on the candidate counts: read the total
-    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    SPM_TRY(e->read_status(st, 0, 4));
     total = e->h_ctrl64.p[2];
   }
   CUDA_TRY(e->d_ids.ensure(total + 1));
   if (framed)
-    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p,
-                                                                e->d_cand_offsets.p, e->d_cand_start.p, e->d_tmp_ids.p,
-                                                                e->d_ids.p, nullptr, nullptr, e->d_ids.cap, 0, 0ull, F);
+    SPM_TRY(e->scan_gather<int32_t, true>(e->d_cand_count.p, nc32, e->d_cand_offsets.p, e->d_cand_start.p, e->d_tmp_ids.p,
+                                          e->d_ids.p, e->d_ids.cap, 0, 0ull, st, nullptr, nullptr, F));
   else
-    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_cand_count.p, nc32, e->d_block_sums.p, e->d_cand_offsets.p,
-                                                          e->d_cand_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
-                                                          e->d_ids.cap, 0, 0ull);
-  CUDA_TRY(cudaGetLastError());
-  e->last_launches += 3;
+    SPM_TRY(e->scan_gather<int32_t>(e->d_cand_count.p, nc32, e->d_cand_offsets.p, e->d_cand_start.p, e->d_tmp_ids.p,
+                                    e->d_ids.p, e->d_ids.cap, 0, 0ull, st));
   CUDA_TRY(e->h_ids.ensure(total + 1));
   if (total) CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_ids.p, total * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(e->h_cand_offsets.p, e->d_cand_offsets.p, (nc + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -2910,25 +2846,19 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
   const uint32_t n32 = static_cast<uint32_t>(n);
   pick_candidates_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(e->d_picks.p, n32, K, e->d_cand_start.p, e->d_cand_count.p,
                                                            e->d_sent_start.p, e->d_sent_count.p);
-  const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
-  CUDA_TRY(e->d_block_sums.ensure(nb + 1));
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
   // every sentence's draw gets the encode frame
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->frame_np + e->frame_ns);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
-  CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
+  SPM_TRY(e->scan_total(e->d_sent_count.p, n32, e->frame_np + e->frame_ns, e->d_ctrl64.p + 2, st));
+  SPM_TRY(e->read_status(st, 0, 4));
   const unsigned long long tot = e->h_ctrl64.p[2];
   CUDA_TRY(e->d_ids.ensure(tot + 1));
   if (e->framed())
-    scan_write_gather_kernel<int32_t, true><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_id_offsets.p,
-                                                                e->d_sent_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr,
-                                                                nullptr, e->d_ids.cap, 0, 0ull, e->kframe());
+    SPM_TRY(e->scan_gather<int32_t, true>(e->d_sent_count.p, n32, e->d_id_offsets.p, e->d_sent_start.p, e->d_tmp_ids.p,
+                                          e->d_ids.p, e->d_ids.cap, 0, 0ull, st, nullptr, nullptr, e->kframe()));
   else
-    scan_write_gather_kernel<int32_t><<<nb, 256, 0, st>>>(e->d_sent_count.p, n32, e->d_block_sums.p, e->d_id_offsets.p,
-                                                          e->d_sent_start.p, e->d_tmp_ids.p, e->d_ids.p, nullptr, nullptr,
-                                                          e->d_ids.cap, 0, 0ull);
-  CUDA_TRY(cudaGetLastError());
-  e->last_launches += 4;
+    SPM_TRY(e->scan_gather<int32_t>(e->d_sent_count.p, n32, e->d_id_offsets.p, e->d_sent_start.p, e->d_tmp_ids.p,
+                                    e->d_ids.p, e->d_ids.cap, 0, 0ull, st));
   CUDA_TRY(e->h_ids.ensure(tot + 1));
   if (tot) CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_ids.p, tot * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaMemcpyAsync(e->h_id_offsets.p, e->d_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
@@ -3056,11 +2986,9 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   if (rc) return rc;
   float main_ms = 0.f;
   if (cudaEventElapsedTime(&main_ms, e->ev[0], e->ev[1]) != cudaSuccess) main_ms = 0.f;
-  uint64_t launches = e->last_launches, deferred = e->last_deferred;
+  uint64_t deferred = e->last_deferred;
   const uint32_t n32 = static_cast<uint32_t>(n);
-  const uint32_t nb = (n32 + kScanChunk - 1) / kScanChunk;
   const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
-  CUDA_TRY(e->d_block_sums.ensure(nb + 1));
   KPieces P{};
   P.n = n32;
   P.ids = e->d_pc_ids.p;
@@ -3076,14 +3004,11 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
     CUDA_TRY(e->d_pc_flag.ensure(n));
     CUDA_TRY(e->d_pc_pos.ensure(n + 1));
     pieces_unk_flag_kernel<<<wgrid, 256, 0, st>>>(e->d_pc_ids.p, e->d_pc_id_offsets.p, n32, e->unk_id, e->d_pc_flag.p);
-    scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_flag.p, n32, e->d_block_sums.p, 0);
-    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
-    scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_flag.p, n32, e->d_block_sums.p, e->d_pc_pos.p, nullptr, nullptr,
-                                                          nullptr, nullptr, nullptr, 0, 0, 0ull);
     CUDA_TRY(cudaGetLastError());
-    launches += 4;
-    CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
+    ++e->last_launches;
+    SPM_TRY(e->scan_total(e->d_pc_flag.p, n32, 0, e->d_ctrl64.p + 2, st));
+    SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_flag.p, n32, e->d_pc_pos.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+    SPM_TRY(e->read_status(st, 0, 4));
     m = static_cast<uint32_t>(e->h_ctrl64.p[2]);
   }
   if (m) {
@@ -3094,20 +3019,18 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
     CUDA_TRY(e->d_pc_sub_bytes.ensure(total_bytes + 64));
     pieces_sub_list_kernel<<<static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256)), 256, 0, st>>>(
         e->d_pc_flag.p, e->d_pc_pos.p, e->d_offsets.p, n32, e->d_pc_sub_of.p, e->d_pc_sub_start.p, e->d_pc_sub_len.p);
-    const uint32_t mb = (m + kScanChunk - 1) / kScanChunk;
-    scan_block_sums_kernel<<<mb, 256, 0, st>>>(e->d_pc_sub_len.p, m, e->d_block_sums.p, 0);
-    scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, mb, e->d_ctrl64.p + 2);
-    scan_write_gather_kernel<uint8_t><<<mb, 256, 0, st>>>(e->d_pc_sub_len.p, m, e->d_block_sums.p, e->d_pc_sub_offsets.p,
-                                                          e->d_pc_sub_start.p, e->d_bytes.p - base, e->d_pc_sub_bytes.p, nullptr,
-                                                          nullptr, e->d_pc_sub_bytes.cap, 0, 0ull);
     CUDA_TRY(cudaGetLastError());
-    launches += 4;
+    ++e->last_launches;
+    SPM_TRY(e->scan_total(e->d_pc_sub_len.p, m, 0, e->d_ctrl64.p + 2, st));
+    SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_sub_len.p, m, e->d_pc_sub_offsets.p, e->d_pc_sub_start.p, e->d_bytes.p - base,
+                                    e->d_pc_sub_bytes.p, e->d_pc_sub_bytes.cap, 0, 0ull, st));
     // (the whole batch's byte count bounds the subset's: it only sizes the spans run's temporary buffers)
     uint64_t sub_tot = 0, sub_norm = 0;
+    const uint64_t launches = e->last_launches;  // run_device starts its own count
     rc = e->run_device(e->d_pc_sub_bytes.p, reinterpret_cast<const uint64_t *>(e->d_pc_sub_offsets.p), m, total_bytes, true,
                        nullptr, 0, nullptr, &sub_tot, &sub_norm, st);
     if (rc) return rc;
-    launches += e->last_launches;
+    e->last_launches += launches;
     deferred += e->last_deferred;
     P.sub_of = e->d_pc_sub_of.p;
     P.sub_ids = e->d_ids.p;
@@ -3130,18 +3053,13 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   P.text_len = e->d_pc_text_len.p;
   P.n_tok = e->d_pc_ntok.p;
   pieces_warp_kernel<false><<<wgrid, 256, 0, st>>>(P);
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_text_len.p, n32, e->d_block_sums.p, 0);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 2);
-  scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_text_len.p, n32, e->d_block_sums.p, e->d_pc_text_offsets.p,
-                                                        nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0ull);
-  scan_block_sums_kernel<<<nb, 256, 0, st>>>(e->d_pc_ntok.p, n32, e->d_block_sums.p, 0);
-  scan_block_prefix_kernel<<<1, 1024, 0, st>>>(e->d_block_sums.p, nb, e->d_ctrl64.p + 3);
-  scan_write_gather_kernel<uint8_t><<<nb, 256, 0, st>>>(e->d_pc_ntok.p, n32, e->d_block_sums.p, e->d_pc_out_id_offsets.p,
-                                                        nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, 0ull);
   CUDA_TRY(cudaGetLastError());
-  launches += 7;
-  CUDA_TRY(cudaMemcpyAsync(e->h_ctrl64.p, e->d_ctrl64.p, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
+  ++e->last_launches;
+  SPM_TRY(e->scan_total(e->d_pc_text_len.p, n32, 0, e->d_ctrl64.p + 2, st));
+  SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_text_len.p, n32, e->d_pc_text_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  SPM_TRY(e->scan_total(e->d_pc_ntok.p, n32, 0, e->d_ctrl64.p + 3, st));
+  SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_ntok.p, n32, e->d_pc_out_id_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  SPM_TRY(e->read_status(st, 0, 4));
   const unsigned long long ttext = e->h_ctrl64.p[2], tids = e->h_ctrl64.p[3];
   CUDA_TRY(e->d_pc_text.ensure(ttext + 1));
   CUDA_TRY(e->d_pc_end.ensure(tids + 1));
@@ -3153,7 +3071,7 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   P.out_ids = e->d_pc_out_ids.p;
   pieces_warp_kernel<true><<<wgrid, 256, 0, st>>>(P);
   CUDA_TRY(cudaGetLastError());
-  ++launches;
+  ++e->last_launches;
   CUDA_TRY(e->h_pc_text.ensure(ttext + 1));
   CUDA_TRY(e->h_pc_end.ensure(tids + 1));
   CUDA_TRY(e->h_ids.ensure(tids + 1));
@@ -3167,7 +3085,6 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(cudaStreamSynchronize(st));
   e->last_d2h = ttext + tids * 8 + (n + 1) * 16;
-  e->last_launches = launches;
   e->last_deferred = deferred;
   e->last_unk_detour = m;
   e->last_main_ms = main_ms;
