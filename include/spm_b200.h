@@ -228,6 +228,34 @@ int spm_sample_encode_and_score(spm_engine *e, const char *bytes, const uint64_t
                                 float alpha, int wor, int include_best, const int32_t **ids,
                                 const uint64_t **cand_offsets, const float **scores);
 
+/* The same three calls with pieces, as spm_encode_pieces writes them: NBestEncodeAsPieces, SampleEncodeAsPieces and
+ * SampleEncodeAndScoreAsPieces over a batch.  unk_piece, sep and the packed layout are those of spm_encode_pieces with
+ * one list per candidate (per sample): text[text_offsets[j] .. text_offsets[j+1]) is list j's pieces,
+ * piece_end[cand_offsets[j] + k] the end of its k-th piece relative to text_offsets[j], ids the framed ids.  Every
+ * id, cand_offset, score and n_cands equals what the ids call returns, and each call consumes the engine's generator
+ * exactly as its ids call does.  Argument checks and errors are those of the ids calls and of spm_encode_pieces.
+ *   spm_nbest_encode_pieces: candidate-major as spm_nbest_encode; empty slots stay empty and unframed.
+ *     nbest_size <= 1 gives spm_encode_pieces' result with score 0.  The unknown tokens' surfaces come from the n-best
+ *     kernels themselves (token ends and the normalized text of sentences whose lattice holds an unknown character).
+ *   spm_sample_encode_pieces: as spm_sample_encode_ids; nbest_size > 1 writes the pieces of the drawn candidates on
+ *     the device, nbest_size < 0 writes them on the host next to the ids of the lattice draw.
+ *   spm_sample_encode_and_score_pieces: as spm_sample_encode_and_score (num_samples slots per sentence; an empty
+ *     sentence leaves its slots empty).
+ * Outputs are engine-owned memory, valid until the next call on this engine. */
+int spm_nbest_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int nbest_size,
+                            const char *unk_piece, size_t unk_piece_len, int sep, const char **text,
+                            const uint64_t **text_offsets, const uint32_t **piece_end, const int32_t **ids,
+                            const uint64_t **cand_offsets, const float **scores, const uint32_t **n_cands);
+int spm_sample_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int nbest_size,
+                             float alpha, const char *unk_piece, size_t unk_piece_len, int sep, const char **text,
+                             const uint64_t **text_offsets, const uint32_t **piece_end, const int32_t **ids,
+                             const uint64_t **id_offsets);
+int spm_sample_encode_and_score_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n,
+                                       int num_samples, float alpha, int wor, int include_best, const char *unk_piece,
+                                       size_t unk_piece_len, int sep, const char **text, const uint64_t **text_offsets,
+                                       const uint32_t **piece_end, const int32_t **ids, const uint64_t **cand_offsets,
+                                       const float **scores);
+
 /* Replaces SentencePieceProcessor::Decode(const std::vector<int>& ids, std::string* detokenized)
  * (src/sentencepiece_processor.cc:911-925 -> :765-909), one call for n id lists: `ids` is the packed
  * concatenation, id_offsets[n+1] delimits the lists (exactly what spm_encode_ids returns).  Outputs

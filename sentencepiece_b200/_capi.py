@@ -16,6 +16,7 @@ EXPORTS = [
     "spm_host_free", "spm_engine_get_info", "spm_engine_set_tuning", "spm_nbest_encode", "spm_set_random_seed",
     "spm_sample_encode_ids", "spm_decode_ids", "spm_engine_set_unk_surface", "spm_calculate_entropy",
     "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
+    "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
 ]
 
 
@@ -81,5 +82,9 @@ def load():
     L.spm_calculate_entropy.argtypes = [vp, vp, vp, sz, ctypes.c_float, P(vp)]
     L.spm_sample_encode_and_score.argtypes = [vp, vp, vp, sz, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int,
                                               P(vp), P(vp), P(vp)]
+    L.spm_nbest_encode_pieces.argtypes = [vp, vp, vp, sz, ctypes.c_int, cp, sz, ctypes.c_int] + [P(vp)] * 7
+    L.spm_sample_encode_pieces.argtypes = [vp, vp, vp, sz, ctypes.c_int, ctypes.c_float, cp, sz, ctypes.c_int] + [P(vp)] * 5
+    L.spm_sample_encode_and_score_pieces.argtypes = [vp, vp, vp, sz, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int,
+                                                     cp, sz, ctypes.c_int] + [P(vp)] * 6
     _lib = L
     return L

@@ -78,6 +78,9 @@ struct KModel {
   int32_t model_type;
 };
 
+// start of a sentence's normalized text in an append buffer that only some sentences use: this one has none there
+constexpr unsigned long long kNoNorm = ~0ull;
+
 // The id effect of the encode extra options (spm_engine_set_encode_frame): every id list the final writers produce
 // becomes P ++ (body, or body reversed) ++ S.  np = ns = 0 is the plain output.
 struct KFrame {

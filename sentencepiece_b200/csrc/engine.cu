@@ -411,8 +411,15 @@ struct spm_engine {
   PinBuf<uint32_t> h_pc_end;
   bool pc_ready = false;
   int ensure_piece_tables();
-  // n-best / sampling
-  DevBuf<uint8_t> d_nb_scratch;
+  // K9's size pass, scans and write pass over the P.n lists of P (sources and frame set), then the copies of the
+  // packed pieces, their ends, the framed ids and both offset arrays into the pinned results; waits for them.
+  // *d2h: the bytes copied.
+  int write_pieces(KPieces &P, const char *unk_piece, size_t unk_len, const char **text, const uint64_t **text_offsets,
+                   const uint32_t **piece_end, const int32_t **ids, const uint64_t **id_offsets, uint64_t *d2h);
+  // n-best / sampling; pieces: the candidates' token ends and the exported normalized texts (NbestOut)
+  DevBuf<uint8_t> d_nb_scratch, d_nb_norm;
+  DevBuf<uint32_t> d_nb_end;
+  DevBuf<unsigned long long> d_nb_norm_start;
   DevBuf<unsigned long long> d_cand_start, d_cand_offsets;
   DevBuf<uint32_t> d_cand_count, d_n_cands, d_picks;
   DevBuf<float> d_cand_score;
@@ -436,12 +443,29 @@ struct spm_engine {
   std::vector<int32_t> lat_ids;          // results of the last lattice sampling call
   std::vector<uint64_t> lat_offsets;
   std::vector<float> lat_scores;
+  std::vector<char> lat_text;            // and its pieces, when asked for (LatPieces)
+  std::vector<uint64_t> lat_text_offsets;
+  std::vector<uint32_t> lat_piece_end;
+  // pieces of the lattice draws, as spm_encode_pieces writes them: unk_piece (null: unknown tokens keep their surface)
+  // and sep
+  struct LatPieces {
+    const char *unk_piece;
+    size_t unk_len;
+    int sep;
+  };
   // mode 0: samples >= 1 draws per sentence from the lattice (ids, offsets[n*samples+1], scores), each with the encode
   // frame -- also the draw of an empty sentence when frame_empty (SampleEncode frames its empty result; an empty
-  // sentence has no samples in SampleEncodeAndScore); mode 1: entropy
+  // sentence has no samples in SampleEncodeAndScore) -- and, with pc, their pieces; mode 1: entropy
   int run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples,
-                  bool frame_empty = false);
-  int run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total);
+                  bool frame_empty = false, const LatPieces *pc = nullptr);
+  // ends: also the token ends of the candidates (d_nb_end); norm: also the normalized text of every sentence whose
+  // lattice holds an UNK node (d_nb_norm, d_nb_norm_start)
+  int run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total,
+                bool ends = false, bool norm = false);
+  // SampleEncode with nbest_size = K > 1: run_nbest, then the draw on this engine's generator; leaves the picked
+  // candidate of every sentence in d_sent_start / d_sent_count.  *d2h: the bytes copied.
+  int sample_picks(const char *bytes, const uint64_t *offsets, size_t n, uint32_t K, float alpha, bool ends, bool norm,
+                   uint64_t *d2h);
   // Long-sentence path of the lattice and n-best calls: one job per sentence their lane kernels deferred.
   struct LongJob {
     uint32_t sent;     // index in the launch
@@ -1978,7 +2002,8 @@ int spm_engine::read_deferred(uint32_t n_def, const uint64_t *offs, std::vector<
 }
 
 // ---- n-best (K5): lattice + A* per sentence on the GPU; leaves candidates in the temporary buffers ----
-int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total) {
+int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, uint32_t nbest, uint64_t *tmp_total,
+                          bool ends, bool norm) {
   cudaStream_t st = stream;
   const uint64_t base = offsets[0];
   const uint64_t total_bytes = offsets[n] - base;
@@ -2008,8 +2033,13 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
   CUDA_TRY(d_n_cands.ensure(n));
   // candidates: at most one id per normalized byte each; start from 2 ids per input byte per 8 candidates
   unsigned long long tmp_cap = std::max<unsigned long long>(1u << 20, total_bytes * nbest / 3 + 64ull * n);
+  // exported normalized texts: at most the bound of the whole batch's normalized length (as run_lattice's pos_cap)
+  unsigned long long norm_cap = (total_bytes * max_expand_num) / max_expand_den + 16ull * n + 1024;
+  if (norm) CUDA_TRY(d_nb_norm_start.ensure(n));
   for (int attempt = 0; attempt < 4; ++attempt) {
     CUDA_TRY(d_tmp_ids.ensure(tmp_cap));
+    if (ends) CUDA_TRY(d_nb_end.ensure(tmp_cap));
+    if (norm) CUDA_TRY(d_nb_norm.ensure(norm_cap));
     CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
     CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 4 * sizeof(unsigned long long), st));
     KBatch B{};
@@ -2030,6 +2060,13 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     O.cand_score = d_cand_score.p;
     O.n_cands = d_n_cands.p;
     O.status = d_ctrl32.p;
+    if (ends) O.tmp_end = d_nb_end.p;
+    if (norm) {
+      O.norm = d_nb_norm.p;
+      O.norm_cap = norm_cap;
+      O.norm_cursor = d_ctrl64.p + 1;
+      O.norm_start = d_nb_norm_start.p;
+    }
     CUDA_TRY(cudaEventRecord(ev[0], st));
     { const int rc = build_order(d_offsets.p, n, st, &B.order, 0); if (rc) return rc; }
     nbest_lane_kernel<kNbestTop, 1024><<<ctas, warps_per_cta * 32, nbest_smem_bytes<kNbestTop>(warps_per_cta), st>>>(
@@ -2059,7 +2096,11 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
     if (h_ctrl32.p[1] & 8u) { set_error("n-best: a long sentence normalized to more bytes than the scratch sized for it"); return SPM_ERR_ENCODE; }
     if (h_ctrl32.p[1] & 16u) { set_error("n-best: a lattice exceeds the sizes the model's trie implies"); return SPM_ERR_ENCODE; }
     if (h_ctrl32.p[1]) { set_error("n-best: internal consistency check failed"); return SPM_ERR_ENCODE; }
-    if (h_ctrl32.p[2]) { tmp_cap = h_ctrl64.p[0] + 1024; continue; }
+    if (h_ctrl32.p[2]) {
+      if (h_ctrl32.p[2] & 1u) tmp_cap = h_ctrl64.p[0] + 1024;
+      if (h_ctrl32.p[2] & 2u) norm_cap = h_ctrl64.p[1] + 1024;
+      continue;
+    }
     *tmp_total = h_ctrl64.p[0];
     return SPM_OK;
   }
@@ -2067,16 +2108,88 @@ int spm_engine::run_nbest(const char *bytes, const uint64_t *offsets, size_t n, 
   return SPM_ERR_CAPACITY;
 }
 
+// ---- SampleEncode with nbest_size > 1 (sentencepiece_processor.cc:703-718): n-best, then one draw per sentence ----
+int spm_engine::sample_picks(const char *bytes, const uint64_t *offsets, size_t n, uint32_t K, float alpha, bool ends,
+                             bool norm, uint64_t *d2h) {
+  cudaStream_t st = stream;
+  uint64_t tmp_total = 0;
+  SPM_TRY(run_nbest(bytes, offsets, n, K, &tmp_total, ends, norm));
+  const size_t nc = n * static_cast<size_t>(K);
+  CUDA_TRY(h_cand_score.ensure(nc + 1));
+  CUDA_TRY(h_n_cands.ensure(n + 1));
+  CUDA_TRY(h_picks.ensure(n + 1));
+  CUDA_TRY(cudaMemcpyAsync(h_cand_score.p, d_cand_score.p, nc * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(h_n_cands.p, d_n_cands.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  // ---- the draw (sentencepiece_processor.cc:703-718) ----
+  // The uniform of sentence i is generate_canonical<double,53>(mt) exactly as
+  // std::discrete_distribution::operator() takes it; a sentence with fewer than two candidates
+  // draws nothing.  Generated in sentence order on one generator, then the (independent)
+  // log-sum-exp / cumulative tables are evaluated by all host threads.
+  std::vector<double> u(n, 0.0);
+  for (size_t i = 0; i < n; ++i)
+    if (h_n_cands.p[i] >= 2) u[i] = std::generate_canonical<double, std::numeric_limits<double>::digits>(rng);
+  const float *sc = h_cand_score.p;
+  const uint32_t *kc = h_n_cands.p;
+  uint32_t *picks = h_picks.p;
+  auto work = [&](size_t lo, size_t hi) {
+    std::vector<double> lp(K), cp(K);
+    for (size_t i = lo; i < hi; ++i) {
+      const uint32_t k = kc[i];
+      if (k < 2) { picks[i] = 0; continue; }
+      const float *s = sc + i * K;
+      for (uint32_t c = 0; c < k; ++c) lp[c] = alpha * s[c];  // float product, widened (:705-706)
+      double Z = lp[0];                                       // log_domain::LogSum, util.cc:278-294
+      for (uint32_t c = 1; c < k; ++c) {
+        double xa = Z, xb = lp[c];
+        if (xa > xb) std::swap(xa, xb);
+        Z = xb + std::log1p(std::exp(xa - xb));
+      }
+      double sum = 0.0;
+      for (uint32_t c = 0; c < k; ++c) { lp[c] = std::exp(lp[c] - Z); sum += lp[c]; }
+      double run = 0.0;  // discrete_distribution::param_type::_M_initialize
+      for (uint32_t c = 0; c < k; ++c) { run += lp[c] / sum; cp[c] = run; }
+      cp[k - 1] = 1.0;
+      picks[i] = static_cast<uint32_t>(std::lower_bound(cp.begin(), cp.begin() + k, u[i]) - cp.begin());
+    }
+  };
+  {
+    const size_t T = std::max<size_t>(1, std::min<size_t>(std::thread::hardware_concurrency(), n / 2048 + 1));
+    std::vector<std::thread> th;
+    const size_t per = (n + T - 1) / T;
+    for (size_t t = 1; t < T; ++t) th.emplace_back(work, std::min(n, t * per), std::min(n, (t + 1) * per));
+    work(0, std::min(n, per));
+    for (auto &t : th) t.join();
+  }
+  // ---- gather the picked candidates into sentence order ----
+  CUDA_TRY(d_picks.ensure(n));
+  CUDA_TRY(d_sent_start.ensure(n));
+  CUDA_TRY(d_sent_count.ensure(n));
+  CUDA_TRY(cudaMemcpyAsync(d_picks.p, picks, n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  pick_candidates_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(d_picks.p, n32, K, d_cand_start.p, d_cand_count.p,
+                                                           d_sent_start.p, d_sent_count.p);
+  CUDA_TRY(cudaGetLastError());
+  ++last_launches;
+  *d2h = nc * 4 + n * 4;
+  return SPM_OK;
+}
+
 // ---- full-lattice operations (SURVEY 8f item 1): lattice + forward algorithm on the GPU (lattice_kernel.cuh), in
 //      chunks of sentences; mode 0 then draws on the host exactly as Lattice::Sample (unigram_model.cc:511-542) does
 //      -- std::exp in double, std::discrete_distribution<int> over float probabilities, this engine's std::mt19937 --
 //      for the sentences in order, which reproduces the reference's single-threaded stream under a seed ----
 int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n, float inv_theta, int mode, int samples,
-                            bool frame_empty) {
+                            bool frame_empty, const LatPieces *pc) {
   cudaStream_t st = stream;
   lat_ids.clear();
   lat_scores.clear();
   lat_offsets.assign(1, 0);
+  lat_text.clear();
+  lat_piece_end.clear();
+  lat_text_offsets.assign(1, 0);
+  std::string unk_bytes;         // pieces: the normalized bytes of the draw's UNK nodes, in path order
+  std::vector<uint32_t> unk_end;  // per body token: the end of its bytes in unk_bytes (known pieces add none)
   LatticeGeom G{};
   G.cap = lane_cap;
   G.node_cap = lane_cap * (trie.max_matches_per_start + 1) + 64;
@@ -2215,36 +2328,75 @@ int spm_engine::run_lattice(const char *bytes, const uint64_t *offsets, size_t n
             p = nodes[q].z;
             Z = A(p);
           }
-          // id path of PopulateSentencePieceText over the sampled nodes, left to right
+          // id path of PopulateSentencePieceText over the sampled nodes, left to right; with pc, also where the
+          // surface of each unknown token lies in unk_bytes (a merged run: its nodes' characters in order)
           bool prev_unk = false;
+          unk_bytes.clear();
+          unk_end.clear();
           for (size_t k = path.size(); k-- > 0;) {
             const uint4 nd = nodes[path[k]];
             float sc; memcpy(&sc, &nd.y, 4);
             score += inv_theta * sc;   // (:846-847)
             const int32_t id = static_cast<int32_t>(nd.x);
             const bool isunk = id == unk_id;
-            if (isunk && bf) {
-              const uint32_t first = nd.w & 0xFFu;
+            // an UNK node covers one character of the normalized text, whose bytes it carries; its byte count is the
+            // span of the character (a truncated character at the end of the text has fewer bytes: the bytes above
+            // it are zero and a zero byte never follows a multi-byte lead in normalized text)
+            auto for_char_bytes = [&](auto &&f) {
               static const uint8_t kLen[16] = {1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 3, 4};
-              uint32_t cl = kLen[first >> 4];
-              // the node covers one character of the normalized text; its byte count is the span of the character
-              // (a truncated character at the end of the text has fewer bytes: the bytes above it are zero and a
-              //  zero byte never follows a multi-byte lead in normalized text)
+              const uint32_t cl = kLen[(nd.w & 0xFFu) >> 4];
               for (uint32_t bq = 0; bq < cl; ++bq) {
                 const uint32_t bv = (nd.w >> (8 * bq)) & 0xFFu;
                 if (bq > 0 && bv == 0) break;
-                lat_ids.push_back(byte_to_id_host[bv]);
+                f(bv);
               }
-            } else if (!(isunk && prev_unk)) {
-              lat_ids.push_back(id);
+            };
+            if (isunk && bf) {
+              for_char_bytes([&](uint32_t bv) { lat_ids.push_back(byte_to_id_host[bv]); });
+            } else {
+              if (!(isunk && prev_unk)) {
+                lat_ids.push_back(id);
+                if (pc) unk_end.push_back(static_cast<uint32_t>(unk_bytes.size()));
+              }
+              if (pc && isunk) {
+                for_char_bytes([&](uint32_t bv) { unk_bytes.push_back(static_cast<char>(bv)); });
+                unk_end.back() = static_cast<uint32_t>(unk_bytes.size());
+              }
             }
             prev_unk = isunk;
           }
           score -= A(L);  // - marginal (:853)
         }
+        const size_t nbody = lat_ids.size() - body;
         if (frame_it) {  // the score stays the raw path's, as in the reference
           if (frame_rev) std::reverse(lat_ids.begin() + body, lat_ids.end());
           lat_ids.insert(lat_ids.end(), frame_ids.begin() + frame_np, frame_ids.end());
+        }
+        if (pc) {  // the pieces of the framed list, as K9 (pieces_kernel.cuh) writes them
+          const size_t first = lat_offsets.back(), T = lat_ids.size() - first;
+          const size_t t0 = lat_text.size();
+          for (size_t t = 0; t < T; ++t) {
+            const int32_t id = lat_ids[first + t];
+            const size_t q = first + t - body;  // position in the body, in its final order
+            const char *src;
+            size_t len;
+            if (id == unk_id && pc->unk_piece) {
+              src = pc->unk_piece;
+              len = pc->unk_len;
+            } else if (id == unk_id && !bf && first + t >= body && q < nbody) {
+              const size_t r = frame_it && frame_rev ? nbody - 1 - q : q;  // in path order
+              const uint32_t b = r ? unk_end[r - 1] : 0u;
+              src = unk_bytes.data() + b;
+              len = unk_end[r] - b;
+            } else {
+              src = model.piece(id);
+              len = model.piece_len(id);
+            }
+            lat_text.insert(lat_text.end(), src, src + len);
+            lat_piece_end.push_back(static_cast<uint32_t>(lat_text.size() - t0));
+            if (pc->sep >= 0 && t + 1 < T) lat_text.push_back(static_cast<char>(pc->sep));
+          }
+          lat_text_offsets.push_back(lat_text.size());
         }
         lat_offsets.push_back(lat_ids.size());
         lat_scores.push_back(score);
@@ -2788,66 +2940,10 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
   e->h_id_offsets.p[0] = 0;
   if (n == 0) return SPM_OK;
   e->last_launches = 0;
-  uint64_t tmp_total = 0;
-  { const int rc = e->run_nbest(bytes, offsets, n, K, &tmp_total); if (rc) return rc; }
-  const size_t nc = n * static_cast<size_t>(K);
-  CUDA_TRY(e->h_cand_score.ensure(nc + 1));
-  CUDA_TRY(e->h_n_cands.ensure(n + 1));
-  CUDA_TRY(e->h_picks.ensure(n + 1));
-  CUDA_TRY(cudaMemcpyAsync(e->h_cand_score.p, e->d_cand_score.p, nc * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(e->h_n_cands.p, e->d_n_cands.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  // ---- the draw (sentencepiece_processor.cc:703-718) ----
-  // The uniform of sentence i is generate_canonical<double,53>(mt) exactly as
-  // std::discrete_distribution::operator() takes it; a sentence with fewer than two candidates
-  // draws nothing.  Generated in sentence order on one generator, then the (independent)
-  // log-sum-exp / cumulative tables are evaluated by all host threads.
-  std::vector<double> u(n, 0.0);
-  for (size_t i = 0; i < n; ++i)
-    if (e->h_n_cands.p[i] >= 2) u[i] = std::generate_canonical<double, std::numeric_limits<double>::digits>(e->rng);
-  const float *sc = e->h_cand_score.p;
-  const uint32_t *kc = e->h_n_cands.p;
-  uint32_t *picks = e->h_picks.p;
-  auto work = [&](size_t lo, size_t hi) {
-    std::vector<double> lp(K), cp(K);
-    for (size_t i = lo; i < hi; ++i) {
-      const uint32_t k = kc[i];
-      if (k < 2) { picks[i] = 0; continue; }
-      const float *s = sc + i * K;
-      for (uint32_t c = 0; c < k; ++c) lp[c] = alpha * s[c];  // float product, widened (:705-706)
-      double Z = lp[0];                                       // log_domain::LogSum, util.cc:278-294
-      for (uint32_t c = 1; c < k; ++c) {
-        double xa = Z, xb = lp[c];
-        if (xa > xb) std::swap(xa, xb);
-        Z = xb + std::log1p(std::exp(xa - xb));
-      }
-      double sum = 0.0;
-      for (uint32_t c = 0; c < k; ++c) { lp[c] = std::exp(lp[c] - Z); sum += lp[c]; }
-      double run = 0.0;  // discrete_distribution::param_type::_M_initialize
-      for (uint32_t c = 0; c < k; ++c) { run += lp[c] / sum; cp[c] = run; }
-      cp[k - 1] = 1.0;
-      picks[i] = static_cast<uint32_t>(std::lower_bound(cp.begin(), cp.begin() + k, u[i]) - cp.begin());
-    }
-  };
-  {
-    const size_t T = std::max<size_t>(1, std::min<size_t>(std::thread::hardware_concurrency(), n / 2048 + 1));
-    std::vector<std::thread> th;
-    const size_t per = (n + T - 1) / T;
-    for (size_t t = 1; t < T; ++t) th.emplace_back(work, std::min(n, t * per), std::min(n, (t + 1) * per));
-    work(0, std::min(n, per));
-    for (auto &t : th) t.join();
-  }
-  // ---- gather the picked candidates into sentence order ----
-  CUDA_TRY(e->d_picks.ensure(n));
-  CUDA_TRY(e->d_sent_start.ensure(n));
-  CUDA_TRY(e->d_sent_count.ensure(n));
+  uint64_t d2h = 0;
+  SPM_TRY(e->sample_picks(bytes, offsets, n, K, alpha, false, false, &d2h));
   CUDA_TRY(e->d_id_offsets.ensure(n + 1));
-  CUDA_TRY(cudaMemcpyAsync(e->d_picks.p, picks, n * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
   const uint32_t n32 = static_cast<uint32_t>(n);
-  pick_candidates_kernel<<<(n32 + 255) / 256, 256, 0, st>>>(e->d_picks.p, n32, K, e->d_cand_start.p, e->d_cand_count.p,
-                                                           e->d_sent_start.p, e->d_sent_count.p);
-  CUDA_TRY(cudaGetLastError());
-  ++e->last_launches;
   // every sentence's draw gets the encode frame
   SPM_TRY(e->scan_total(e->d_sent_count.p, n32, e->frame_np + e->frame_ns, e->d_ctrl64.p + 2, st));
   SPM_TRY(e->read_status(st, 0, 4));
@@ -2864,7 +2960,7 @@ int spm_sample_encode_ids(spm_engine *e, const char *bytes, const uint64_t *offs
   CUDA_TRY(cudaMemcpyAsync(e->h_id_offsets.p, e->d_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
   CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  e->last_d2h = nc * 4 + n * 4 + tot * 4 + (n + 1) * 8;
+  e->last_d2h = d2h + tot * 4 + (n + 1) * 8;
   finish_timing(e);
   *ids = e->h_ids.p;
   *id_offsets = e->h_id_offsets.p;
@@ -2920,6 +3016,73 @@ int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, 
   if (!e || !tok_end || !normalized || !norm_offsets || !n2o) return SPM_ERR_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_host_locked(e, bytes, offsets, n, true, ids, tok_end, id_offsets, normalized, norm_offsets, n2o);
+}
+
+int spm_engine::write_pieces(KPieces &P, const char *unk_piece, size_t unk_len, const char **text,
+                             const uint64_t **text_offsets, const uint32_t **piece_end, const int32_t **ids,
+                             const uint64_t **id_offsets, uint64_t *d2h) {
+  cudaStream_t st = stream;
+  const uint32_t n32 = P.n;
+  const size_t n = n32;
+  const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (n + 7) / 8));
+  SPM_TRY(ensure_piece_tables());
+  P.pc_off = d_pc_off.p;
+  P.pc_bytes = d_pc_bytes.p;
+  P.unk_id = unk_id;
+  CUDA_TRY(h_pc_text_offsets.ensure(n + 1));
+  CUDA_TRY(h_id_offsets.ensure(n + 1));
+  if (unk_piece) {
+    CUDA_TRY(d_pc_unk.ensure(unk_len + 1));
+    if (unk_len) CUDA_TRY(cudaMemcpyAsync(d_pc_unk.p, unk_piece, unk_len, cudaMemcpyHostToDevice, st));
+    P.unk_piece = d_pc_unk.p;
+    P.unk_len = static_cast<uint32_t>(unk_len);
+  }
+  CUDA_TRY(d_pc_text_len.ensure(n));
+  CUDA_TRY(d_pc_ntok.ensure(n));
+  CUDA_TRY(d_pc_text_offsets.ensure(n + 1));
+  CUDA_TRY(d_pc_out_id_offsets.ensure(n + 1));
+  P.text_len = d_pc_text_len.p;
+  P.n_tok = d_pc_ntok.p;
+  pieces_warp_kernel<false><<<wgrid, 256, 0, st>>>(P);
+  CUDA_TRY(cudaGetLastError());
+  ++last_launches;
+  SPM_TRY(scan_total(d_pc_text_len.p, n32, 0, d_ctrl64.p + 2, st));
+  SPM_TRY(scan_gather<uint8_t>(d_pc_text_len.p, n32, d_pc_text_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  SPM_TRY(scan_total(d_pc_ntok.p, n32, 0, d_ctrl64.p + 3, st));
+  SPM_TRY(scan_gather<uint8_t>(d_pc_ntok.p, n32, d_pc_out_id_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  SPM_TRY(read_status(st, 0, 4));
+  const unsigned long long ttext = h_ctrl64.p[2], tids = h_ctrl64.p[3];
+  CUDA_TRY(d_pc_text.ensure(ttext + 1));
+  CUDA_TRY(d_pc_end.ensure(tids + 1));
+  CUDA_TRY(d_pc_out_ids.ensure(tids + 1));
+  P.text_offsets = d_pc_text_offsets.p;
+  P.out_id_offsets = d_pc_out_id_offsets.p;
+  P.text = d_pc_text.p;
+  P.piece_end = d_pc_end.p;
+  P.out_ids = d_pc_out_ids.p;
+  pieces_warp_kernel<true><<<wgrid, 256, 0, st>>>(P);
+  CUDA_TRY(cudaGetLastError());
+  ++last_launches;
+  CUDA_TRY(h_pc_text.ensure(ttext + 1));
+  CUDA_TRY(h_pc_end.ensure(tids + 1));
+  CUDA_TRY(h_ids.ensure(tids + 1));
+  if (ttext) CUDA_TRY(cudaMemcpyAsync(h_pc_text.p, d_pc_text.p, ttext, cudaMemcpyDeviceToHost, st));
+  if (tids) {
+    CUDA_TRY(cudaMemcpyAsync(h_pc_end.p, d_pc_end.p, tids * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_ids.p, d_pc_out_ids.p, tids * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  }
+  CUDA_TRY(cudaMemcpyAsync(h_pc_text_offsets.p, d_pc_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(h_id_offsets.p, d_pc_out_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaEventRecord(ev[2], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  *d2h = ttext + tids * 8 + (n + 1) * 16;
+  h_pc_text.p[ttext] = 0;
+  *text = h_pc_text.p;
+  *text_offsets = h_pc_text_offsets.p;
+  *piece_end = h_pc_end.p;
+  *ids = h_ids.p;
+  *id_offsets = h_id_offsets.p;
+  return SPM_OK;
 }
 
 // EncodeAsPieces for a host batch:
@@ -2993,9 +3156,6 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   P.n = n32;
   P.ids = e->d_pc_ids.p;
   P.id_offsets = e->d_pc_id_offsets.p;
-  P.pc_off = e->d_pc_off.p;
-  P.pc_bytes = e->d_pc_bytes.p;
-  P.unk_id = e->unk_id;
   P.sep = sep;
   P.F = e->kframe();
   // ---- 2. unknown surfaces: only the sentences that hold the unknown id take the spans path ----
@@ -3040,63 +3200,15 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
     P.norm_offsets = e->d_norm_offsets.p;
   }
   // ---- 3. K9: sizes, offsets, pieces ----
-  if (unk_piece) {
-    CUDA_TRY(e->d_pc_unk.ensure(unk_len + 1));
-    if (unk_len) CUDA_TRY(cudaMemcpyAsync(e->d_pc_unk.p, unk_piece, unk_len, cudaMemcpyHostToDevice, st));
-    P.unk_piece = e->d_pc_unk.p;
-    P.unk_len = static_cast<uint32_t>(unk_len);
-  }
-  CUDA_TRY(e->d_pc_text_len.ensure(n));
-  CUDA_TRY(e->d_pc_ntok.ensure(n));
-  CUDA_TRY(e->d_pc_text_offsets.ensure(n + 1));
-  CUDA_TRY(e->d_pc_out_id_offsets.ensure(n + 1));
-  P.text_len = e->d_pc_text_len.p;
-  P.n_tok = e->d_pc_ntok.p;
-  pieces_warp_kernel<false><<<wgrid, 256, 0, st>>>(P);
-  CUDA_TRY(cudaGetLastError());
-  ++e->last_launches;
-  SPM_TRY(e->scan_total(e->d_pc_text_len.p, n32, 0, e->d_ctrl64.p + 2, st));
-  SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_text_len.p, n32, e->d_pc_text_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
-  SPM_TRY(e->scan_total(e->d_pc_ntok.p, n32, 0, e->d_ctrl64.p + 3, st));
-  SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_ntok.p, n32, e->d_pc_out_id_offsets.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
-  SPM_TRY(e->read_status(st, 0, 4));
-  const unsigned long long ttext = e->h_ctrl64.p[2], tids = e->h_ctrl64.p[3];
-  CUDA_TRY(e->d_pc_text.ensure(ttext + 1));
-  CUDA_TRY(e->d_pc_end.ensure(tids + 1));
-  CUDA_TRY(e->d_pc_out_ids.ensure(tids + 1));
-  P.text_offsets = e->d_pc_text_offsets.p;
-  P.out_id_offsets = e->d_pc_out_id_offsets.p;
-  P.text = e->d_pc_text.p;
-  P.piece_end = e->d_pc_end.p;
-  P.out_ids = e->d_pc_out_ids.p;
-  pieces_warp_kernel<true><<<wgrid, 256, 0, st>>>(P);
-  CUDA_TRY(cudaGetLastError());
-  ++e->last_launches;
-  CUDA_TRY(e->h_pc_text.ensure(ttext + 1));
-  CUDA_TRY(e->h_pc_end.ensure(tids + 1));
-  CUDA_TRY(e->h_ids.ensure(tids + 1));
-  if (ttext) CUDA_TRY(cudaMemcpyAsync(e->h_pc_text.p, e->d_pc_text.p, ttext, cudaMemcpyDeviceToHost, st));
-  if (tids) {
-    CUDA_TRY(cudaMemcpyAsync(e->h_pc_end.p, e->d_pc_end.p, tids * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_pc_out_ids.p, tids * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
-  }
-  CUDA_TRY(cudaMemcpyAsync(e->h_pc_text_offsets.p, e->d_pc_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(e->h_id_offsets.p, e->d_pc_out_id_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaEventRecord(e->ev[2], st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  e->last_d2h = ttext + tids * 8 + (n + 1) * 16;
+  uint64_t d2h = 0;
+  SPM_TRY(e->write_pieces(P, unk_piece, unk_len, text, text_offsets, piece_end, ids, id_offsets, &d2h));
+  e->last_d2h = d2h;
   e->last_deferred = deferred;
   e->last_unk_detour = m;
   e->last_main_ms = main_ms;
   float all = 0.f;
   e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : main_ms;
   (void)cudaGetLastError();
-  e->h_pc_text.p[ttext] = 0;
-  *text = e->h_pc_text.p;
-  *text_offsets = e->h_pc_text_offsets.p;
-  *piece_end = e->h_pc_end.p;
-  *ids = e->h_ids.p;
-  *id_offsets = e->h_id_offsets.p;
   return SPM_OK;
 }
 
@@ -3107,6 +3219,161 @@ int spm_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets,
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
                               id_offsets);
+}
+
+// unk_piece / sep as spm_encode_pieces takes them
+static int pieces_args_ok(spm_engine *e, const char *unk_piece, size_t unk_len, int sep) {
+  if (unk_len && !unk_piece) { e->set_error("null argument"); return SPM_ERR_ARG; }
+  if (sep < -1 || sep > 255) { e->set_error("sep must be -1 or a byte value"); return SPM_ERR_ARG; }
+  if (unk_len > 0xFFFFFFull) { e->set_error("unk_piece too long"); return SPM_ERR_ARG; }
+  return SPM_OK;
+}
+
+// K9 over candidate lists of the n-best buffers (run_nbest with ends; norm unless unk_piece or byte fallback makes the
+// unknown surfaces unnecessary): list j is ids [start[j], + count[j]) of sentence j / per.
+static KPieces candidate_lists(spm_engine *e, uint32_t lists, const unsigned long long *start, const uint32_t *count,
+                               uint32_t per, bool norm, int sep, const KFrame &F) {
+  KPieces P{};
+  P.n = lists;
+  P.ids = e->d_tmp_ids.p;
+  P.list_start = start;
+  P.list_count = count;
+  if (norm) {
+    P.tok_end = e->d_nb_end.p;
+    P.sent_norm = e->d_nb_norm.p;
+    P.sent_norm_start = e->d_nb_norm_start.p;
+  }
+  P.per = per;
+  P.sep = sep;
+  P.F = F;
+  return P;
+}
+
+// Whether the pieces of a batch need the unknown tokens' normalized text (K5 exports it).
+static bool needs_unk_surface(const spm_engine *e, const char *unk_piece) {
+  return !unk_piece && e->unk_id >= 0 && !e->model.byte_fallback;
+}
+
+int spm_nbest_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int nbest_size,
+                            const char *unk_piece, size_t unk_piece_len, int sep, const char **text,
+                            const uint64_t **text_offsets, const uint32_t **piece_end, const int32_t **ids,
+                            const uint64_t **cand_offsets, const float **scores, const uint32_t **n_cands) {
+  if (!e || !text || !text_offsets || !piece_end || !ids || !cand_offsets || !scores || !n_cands) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  { const int rc = nbest_args_ok(e, bytes, offsets, n); if (rc) return rc; }
+  SPM_TRY(pieces_args_ok(e, unk_piece, unk_piece_len, sep));
+  CUDA_TRY(cudaSetDevice(e->device));
+  const uint32_t K = static_cast<uint32_t>(std::max(1, std::min(nbest_size, 1024)));  // unigram_model.cc:701
+  cudaStream_t st = e->stream;
+  const size_t nc = n * static_cast<size_t>(K);
+  if (nc >= 0xFFFFFFF0ull) { e->set_error("n-best: sentences x nbest_size must stay below 2^32; split the batch"); return SPM_ERR_ARG; }
+  CUDA_TRY(e->h_cand_score.ensure(nc + 1));
+  CUDA_TRY(e->h_n_cands.ensure(n + 1));
+  *scores = e->h_cand_score.p; *n_cands = e->h_n_cands.p;
+  if (K == 1 || n == 0) {
+    // nbest_size <= 1: {Encode(normalized), 0.0} (unigram_model.cc:703-705)
+    SPM_TRY(encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
+                                 cand_offsets));
+    for (size_t i = 0; i < n; ++i) { e->h_cand_score.p[i] = 0.f; e->h_n_cands.p[i] = 1; }
+    return SPM_OK;
+  }
+  e->last_launches = 0;
+  e->last_unk_detour = 0;
+  const bool norm = needs_unk_surface(e, unk_piece);
+  uint64_t tmp_total = 0;
+  SPM_TRY(e->run_nbest(bytes, offsets, n, K, &tmp_total, norm, norm));
+  // candidate-major lists; every real candidate gets the encode frame, empty slots stay empty
+  KPieces P = candidate_lists(e, static_cast<uint32_t>(nc), e->d_cand_start.p, e->d_cand_count.p, K, norm, sep,
+                              e->kframe(e->d_n_cands.p, K));
+  CUDA_TRY(cudaMemcpyAsync(e->h_cand_score.p, e->d_cand_score.p, nc * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CUDA_TRY(cudaMemcpyAsync(e->h_n_cands.p, e->d_n_cands.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  uint64_t d2h = 0;
+  SPM_TRY(e->write_pieces(P, unk_piece, unk_piece_len, text, text_offsets, piece_end, ids, cand_offsets, &d2h));
+  e->last_d2h = d2h + nc * 4 + n * 4;
+  finish_timing(e);
+  return SPM_OK;
+}
+
+int spm_sample_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int nbest_size,
+                             float alpha, const char *unk_piece, size_t unk_piece_len, int sep, const char **text,
+                             const uint64_t **text_offsets, const uint32_t **piece_end, const int32_t **ids,
+                             const uint64_t **id_offsets) {
+  if (!e || !text || !text_offsets || !piece_end || !ids || !id_offsets) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (nbest_size > 512) { e->set_error("nbest_size must be nbest_size <= 512"); return SPM_ERR_ARG; }  // :683
+  SPM_TRY(pieces_args_ok(e, unk_piece, unk_piece_len, sep));
+  if (e->model.model_type != SPM_UNIGRAM) {  // as spm_sample_encode_ids
+    if (alpha > 0.f) {
+      e->set_error("SampleEncode: BPE-dropout (alpha > 0) is not on the accelerated path");
+      return SPM_ERR_UNSUPPORTED;
+    }
+    return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
+                                id_offsets);
+  }
+  if (nbest_size < 0) {
+    { const int rc = nbest_args_ok(e, bytes, offsets, n); if (rc) return rc; }
+    CUDA_TRY(cudaSetDevice(e->device));
+    const spm_engine::LatPieces pc{unk_piece, unk_piece_len, sep};
+    SPM_TRY(e->run_lattice(bytes, offsets, n, alpha, 0, 1, true, &pc));
+    if (e->lat_ids.empty()) e->lat_ids.reserve(1);
+    if (e->lat_text.empty()) e->lat_text.reserve(1);
+    if (e->lat_piece_end.empty()) e->lat_piece_end.reserve(1);
+    *text = e->lat_text.data(); *text_offsets = e->lat_text_offsets.data(); *piece_end = e->lat_piece_end.data();
+    *ids = e->lat_ids.data(); *id_offsets = e->lat_offsets.data();
+    return SPM_OK;
+  }
+  if (nbest_size <= 1)
+    return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
+                                id_offsets);
+  { const int rc = nbest_args_ok(e, bytes, offsets, n); if (rc) return rc; }
+  if (n == 0)
+    return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
+                                id_offsets);
+  CUDA_TRY(cudaSetDevice(e->device));
+  e->last_launches = 0;
+  e->last_unk_detour = 0;
+  const bool norm = needs_unk_surface(e, unk_piece);
+  uint64_t d2h = 0, d2h_pieces = 0;
+  SPM_TRY(e->sample_picks(bytes, offsets, n, static_cast<uint32_t>(nbest_size), alpha, norm, norm, &d2h));
+  // every sentence's draw gets the encode frame
+  KPieces P = candidate_lists(e, static_cast<uint32_t>(n), e->d_sent_start.p, e->d_sent_count.p, 1, norm, sep, e->kframe());
+  SPM_TRY(e->write_pieces(P, unk_piece, unk_piece_len, text, text_offsets, piece_end, ids, id_offsets, &d2h_pieces));
+  e->last_d2h = d2h + d2h_pieces;
+  finish_timing(e);
+  return SPM_OK;
+}
+
+int spm_sample_encode_and_score_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n,
+                                       int num_samples, float alpha, int wor, int include_best, const char *unk_piece,
+                                       size_t unk_piece_len, int sep, const char **text, const uint64_t **text_offsets,
+                                       const uint32_t **piece_end, const int32_t **ids, const uint64_t **cand_offsets,
+                                       const float **scores) {
+  if (!e || !text || !text_offsets || !piece_end || !ids || !cand_offsets || !scores) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (e->model.model_type != SPM_UNIGRAM) {
+    e->set_error("SampleEncodeAndScore is not available for the current model.");  // sentencepiece_processor.cc:726-727
+    return SPM_ERR_UNSUPPORTED;
+  }
+  if (wor || include_best) {
+    e->set_error("SampleEncodeAndScore: wor / include_best are not on the accelerated path");
+    return SPM_ERR_UNSUPPORTED;
+  }
+  if (num_samples < 1 || num_samples > 4096) { e->set_error("num_samples must be in [1, 4096]"); return SPM_ERR_ARG; }
+  { const int rc = nbest_args_ok(e, bytes, offsets, n); if (rc) return rc; }
+  { const int rc = pieces_args_ok(e, unk_piece, unk_piece_len, sep); if (rc) return rc; }
+  if (cudaSetDevice(e->device) != cudaSuccess) { e->set_error("cudaSetDevice failed"); return SPM_ERR_CUDA; }
+  const spm_engine::LatPieces pc{unk_piece, unk_piece_len, sep};
+  const int rc = e->run_lattice(bytes, offsets, n, alpha, 0, num_samples, false, &pc);
+  if (rc) return rc;
+  if (e->lat_ids.empty()) e->lat_ids.reserve(1);
+  if (e->lat_scores.empty()) e->lat_scores.reserve(1);
+  if (e->lat_text.empty()) e->lat_text.reserve(1);
+  if (e->lat_piece_end.empty()) e->lat_piece_end.reserve(1);
+  *text = e->lat_text.data(); *text_offsets = e->lat_text_offsets.data(); *piece_end = e->lat_piece_end.data();
+  *ids = e->lat_ids.data(); *cand_offsets = e->lat_offsets.data(); *scores = e->lat_scores.data();
+  return SPM_OK;
 }
 
 }  // extern "C"

@@ -313,41 +313,63 @@ util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> 
   return util::OkStatus();
 }
 
-// The raw segmentation inside an id list the engine framed: the pieces forms lay it over the normalized text and then
-// apply the options to the piece strings.  A list shorter than the frame is an empty SampleEncodeAndScore slot.
-void SentencePieceProcessor::RawIds(const int32_t *ids, size_t n, std::vector<int> *raw) const {
-  const size_t f = frame_p_.size() + frame_s_.size();
-  if (n < f) { raw->clear(); return; }
-  raw->assign(ids + frame_p_.size(), ids + n - frame_s_.size());
-  if (frame_rev_) std::reverse(raw->begin(), raw->end());
-}
-
-// ApplyExtraOptions, sentencepiece_processor.cc:1019-1064, on piece strings
-void SentencePieceProcessor::ApplyExtraPieces(std::vector<std::string> *v, std::vector<int> *pid) const {
-  if (extra_.empty()) return;
-  const int bos = PieceToId(impl_->model.bos_piece), eos = PieceToId(impl_->model.eos_piece);
-  for (const auto o : extra_) {
-    if (o == REVERSE) { std::reverse(v->begin(), v->end()); std::reverse(pid->begin(), pid->end()); }
-    else if (o == EOS) { v->push_back(impl_->model.eos_piece); pid->push_back(eos); }
-    else if (o == BOS) { v->insert(v->begin(), impl_->model.bos_piece); pid->insert(pid->begin(), bos); }
-    else if (o == UNK_PIECE)
-      for (size_t k = 0; k < v->size(); ++k)
-        if ((*pid)[k] == unk_id_) (*v)[k] = impl_->model.unk_piece;
-  }
-}
-
 // The engine writes the pieces with the options applied: bos / eos / reverse are the frame SetEncodeExtraOptions set,
 // UNK_PIECE is passed as trainer_spec.unk_piece.
+const std::string *SentencePieceProcessor::UnkPiece() const {
+  const bool unk = std::find(extra_.begin(), extra_.end(), UNK_PIECE) != extra_.end();
+  return unk ? &impl_->model.unk_piece : nullptr;
+}
+
 util::Status SentencePieceProcessor::EncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int sep,
                                                         const char **text, const uint64_t **text_offsets,
                                                         const uint32_t **piece_end, const uint64_t **id_offsets) const {
   if (!engine_) return status();
-  const bool unk = std::find(extra_.begin(), extra_.end(), UNK_PIECE) != extra_.end();
-  const std::string &up = impl_->model.unk_piece;
+  const std::string *up = UnkPiece();
   const int32_t *ids;
-  return FromEngine(engine_, spm_encode_pieces(engine_, bytes, offsets, n, unk ? up.data() : nullptr, unk ? up.size() : 0, sep,
-                                               text, text_offsets, piece_end, &ids, id_offsets));
+  return FromEngine(engine_, spm_encode_pieces(engine_, bytes, offsets, n, up ? up->data() : nullptr, up ? up->size() : 0,
+                                               sep, text, text_offsets, piece_end, &ids, id_offsets));
 }
+
+util::Status SentencePieceProcessor::NBestEncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n,
+                                                             int nbest_size, int sep, const char **text,
+                                                             const uint64_t **text_offsets, const uint32_t **piece_end,
+                                                             const uint64_t **cand_offsets, const uint32_t **n_cands) const {
+  if (!engine_) return status();
+  const std::string *up = UnkPiece();
+  const int32_t *ids;
+  const float *scores;
+  return FromEngine(engine_, spm_nbest_encode_pieces(engine_, bytes, offsets, n, nbest_size, up ? up->data() : nullptr,
+                                                     up ? up->size() : 0, sep, text, text_offsets, piece_end, &ids,
+                                                     cand_offsets, &scores, n_cands));
+}
+
+util::Status SentencePieceProcessor::SampleEncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n,
+                                                              int nbest_size, float alpha, int sep, const char **text,
+                                                              const uint64_t **text_offsets, const uint32_t **piece_end,
+                                                              const uint64_t **id_offsets) const {
+  if (!engine_) return status();
+  SeedOnce();
+  const std::string *up = UnkPiece();
+  const int32_t *ids;
+  return FromEngine(engine_, spm_sample_encode_pieces(engine_, bytes, offsets, n, nbest_size, alpha,
+                                                      up ? up->data() : nullptr, up ? up->size() : 0, sep, text,
+                                                      text_offsets, piece_end, &ids, id_offsets));
+}
+
+namespace {
+// list j of a packed pieces result (sep = -1) as strings
+std::vector<std::string> PieceList(const char *text, const uint64_t *to, const uint32_t *ends, const uint64_t *ido,
+                                   size_t j) {
+  std::vector<std::string> v;
+  v.reserve(ido[j + 1] - ido[j]);
+  uint32_t begin = 0;
+  for (uint64_t k = ido[j]; k < ido[j + 1]; ++k) {
+    v.emplace_back(text + to[j] + begin, ends[k] - begin);
+    begin = ends[k];
+  }
+  return v;
+}
+}  // namespace
 
 util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> &inputs,
                                             std::vector<std::vector<std::string>> *pieces) const {
@@ -364,67 +386,12 @@ util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> 
   if (!st.ok()) return st;
   pieces->resize(inputs.size());
   ParallelFor(inputs.size(), [&](size_t lo, size_t hi) {
-    for (size_t i = lo; i < hi; ++i) {
-      auto &v = (*pieces)[i];
-      v.reserve(ido[i + 1] - ido[i]);
-      uint32_t begin = 0;
-      for (uint64_t k = ido[i]; k < ido[i + 1]; ++k) {
-        v.emplace_back(text + to[i] + begin, ends[k] - begin);
-        begin = ends[k];
-      }
-    }
+    for (size_t i = lo; i < hi; ++i) (*pieces)[i] = PieceList(text, to, ends, ido, i);
   });
   return util::OkStatus();
 }
 
-// ---- n-best and sampling ----
-//
-// The engine returns id sequences.  The piece forms need, for every UNKNOWN token, its surface in the normalized
-// text (sentencepiece_processor.cc:609-621); it is recovered by laying the id sequence over the normalized text: a
-// known id must spell its piece (byte pieces their byte) at the current position, an unknown id covers one or more
-// whole characters none of which has a one-character piece of its own (only such characters get an UNK node,
-// unigram_model.cc:590-594), up to wherever the rest of the sequence fits.
-bool SentencePieceProcessor::PiecesFromIds(std::string_view norm, const int32_t *ids, size_t n,
-                                           std::vector<std::string> *pieces) const {
-  pieces->assign(n, std::string());
-  static const unsigned char kLen[16] = {1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 2, 2, 3, 4};
-  const auto &m = impl_->model;
-  std::function<bool(size_t, size_t)> rec = [&](size_t k, size_t pos) -> bool {
-    if (k == n) return pos == norm.size();
-    const int id = ids[k];
-    if (id < 0 || id >= GetPieceSize()) return false;
-    const uint8_t t = m.types[id];
-    if (t == SPM_BYTE) {  // <0xXX>: one byte of the text
-      const std::string &p = impl_->pieces[id];
-      if (pos >= norm.size() || p.size() != 6) return false;
-      const int v = static_cast<int>(strtol(p.substr(3, 2).c_str(), nullptr, 16));
-      if (static_cast<unsigned char>(norm[pos]) != v) return false;
-      (*pieces)[k] = p;
-      return rec(k + 1, pos + 1);
-    }
-    if (id != unk_id_) {
-      const std::string &p = impl_->pieces[id];
-      if (norm.compare(pos, p.size(), p) != 0) return false;
-      (*pieces)[k] = p;
-      return rec(k + 1, pos + p.size());
-    }
-    size_t end = pos;
-    while (end < norm.size()) {
-      const size_t cl = std::min<size_t>(kLen[static_cast<unsigned char>(norm[end]) >> 4], norm.size() - end);
-      const auto it = impl_->piece_to_id.find(std::string(norm.substr(end, cl)));
-      if (it != impl_->piece_to_id.end()) {
-        const uint8_t ct = m.types[it->second];
-        if (ct == SPM_NORMAL || ct == SPM_USER_DEFINED) break;  // this character has its own piece: no UNK node
-      }
-      end += cl;
-      (*pieces)[k].assign(norm.substr(pos, end - pos));
-      if (rec(k + 1, end)) return true;
-    }
-    return false;
-  };
-  return rec(0, 0);
-}
-
+// ---- n-best and sampling: the engine writes the pieces of every candidate, the options applied ----
 util::Status SentencePieceProcessor::NBestEncode(const std::vector<std::string_view> &inputs, int nbest_size,
                                                  std::vector<std::vector<std::vector<int>>> *ids) const {
   if (!engine_) return status();
@@ -459,34 +426,19 @@ util::Status SentencePieceProcessor::NBestEncode(const std::vector<std::string_v
   std::string bytes;
   std::vector<uint64_t> offs;
   Pack(inputs, &bytes, &offs);
-  // normalized text first (the spans call), then the candidates: both results live in engine buffers of their own
-  const int32_t *sids;
-  const uint32_t *tok_end, *n2o;
-  const uint64_t *ido, *no;
-  const char *norm;
-  int rc = spm_encode_spans(engine_, bytes.data(), offs.data(), inputs.size(), &sids, &tok_end, &ido, &norm, &no, &n2o);
-  if (rc) return FromEngine(engine_, rc);
-  std::vector<std::string> norms(inputs.size());
-  for (size_t i = 0; i < inputs.size(); ++i) norms[i].assign(norm + no[i], norm + no[i + 1]);
-  const int32_t *out;
-  const uint64_t *co;
-  const float *sc;
-  const uint32_t *nc;
-  rc = spm_nbest_encode(engine_, bytes.data(), offs.data(), inputs.size(), nbest_size, &out, &co, &sc, &nc);
-  if (rc) return FromEngine(engine_, rc);
+  const char *text;
+  const uint64_t *to, *co;
+  const uint32_t *ends, *nc;
+  const auto st = NBestEncodePiecesPacked(bytes.data(), offs.data(), inputs.size(), nbest_size, -1, &text, &to, &ends, &co, &nc);
+  if (!st.ok()) return st;
   const size_t K = static_cast<size_t>(std::max(1, std::min(nbest_size, 1024)));
+  // One thread: with many host threads, materialising tens of millions of strings (uni32k at nbest_size 64) took
+  // four times as long as on one, on the H100 host measured in DESIGN §5.
   pieces->resize(inputs.size());
-  std::vector<int> pid;
   for (size_t i = 0; i < inputs.size(); ++i) {
     auto &cands = (*pieces)[i];
     cands.resize(nc[i]);
-    for (uint32_t c = 0; c < nc[i]; ++c) {
-      const uint64_t lo = co[i * K + c], hi = co[i * K + c + 1];
-      RawIds(out + lo, hi - lo, &pid);
-      if (!PiecesFromIds(norms[i], pid.data(), pid.size(), &cands[c]))
-        return Internal("all normalized characters are not consumed.");  // sentencepiece_processor.cc:628-629
-      ApplyExtraPieces(&cands[c], &pid);
-    }
+    for (uint32_t c = 0; c < nc[i]; ++c) cands[c] = PieceList(text, to, ends, co, i * K + c);
   }
   return util::OkStatus();
 }
@@ -516,30 +468,19 @@ util::Status SentencePieceProcessor::SampleEncode(const std::vector<std::string_
   if (!engine_) return status();
   if (!pieces) return Internal("output container is null");
   pieces->clear();
-  SeedOnce();
   std::string bytes;
   std::vector<uint64_t> offs;
   Pack(inputs, &bytes, &offs);
-  const int32_t *sids;
-  const uint32_t *tok_end, *n2o;
-  const uint64_t *ido, *no;
-  const char *norm;
-  int rc = spm_encode_spans(engine_, bytes.data(), offs.data(), inputs.size(), &sids, &tok_end, &ido, &norm, &no, &n2o);
-  if (rc) return FromEngine(engine_, rc);
-  std::vector<std::string> norms(inputs.size());
-  for (size_t i = 0; i < inputs.size(); ++i) norms[i].assign(norm + no[i], norm + no[i + 1]);
-  const int32_t *out;
-  const uint64_t *oo;
-  rc = spm_sample_encode_ids(engine_, bytes.data(), offs.data(), inputs.size(), nbest_size, alpha, &out, &oo);
-  if (rc) return FromEngine(engine_, rc);
+  const char *text;
+  const uint64_t *to, *ido;
+  const uint32_t *ends;
+  const auto st = SampleEncodePiecesPacked(bytes.data(), offs.data(), inputs.size(), nbest_size, alpha, -1, &text, &to,
+                                           &ends, &ido);
+  if (!st.ok()) return st;
   pieces->resize(inputs.size());
-  std::vector<int> pid;
-  for (size_t i = 0; i < inputs.size(); ++i) {
-    RawIds(out + oo[i], oo[i + 1] - oo[i], &pid);
-    if (!PiecesFromIds(norms[i], pid.data(), pid.size(), &(*pieces)[i]))
-      return Internal("all normalized characters are not consumed.");
-    ApplyExtraPieces(&(*pieces)[i], &pid);
-  }
+  ParallelFor(inputs.size(), [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) (*pieces)[i] = PieceList(text, to, ends, ido, i);
+  });
   return util::OkStatus();
 }
 
@@ -593,24 +534,17 @@ std::vector<std::pair<std::vector<std::string>, float>> SentencePieceProcessor::
   if (!engine_) return out;
   SeedOnce();
   const uint64_t offs[2] = {0, input.size()};
-  const int32_t *sids;
-  const uint32_t *tok_end, *n2o;
-  const uint64_t *ido, *no;
-  const char *norm;
-  if (spm_encode_spans(engine_, input.data(), offs, 1, &sids, &tok_end, &ido, &norm, &no, &n2o)) return out;
-  const std::string normalized(norm + no[0], norm + no[1]);
+  const std::string *up = UnkPiece();
+  const char *text;
+  const uint64_t *to, *co;
+  const uint32_t *ends;
   const int32_t *ids;
-  const uint64_t *co;
   const float *sc;
-  if (spm_sample_encode_and_score(engine_, input.data(), offs, 1, num_samples, alpha, wor, include_best, &ids, &co, &sc)) return out;
-  std::vector<int> pid;
-  for (int c = 0; c < num_samples; ++c) {
-    std::vector<std::string> pcs;
-    RawIds(ids + co[c], co[c + 1] - co[c], &pid);
-    if (!PiecesFromIds(normalized, pid.data(), pid.size(), &pcs)) return {};
-    if (co[c + 1] > co[c]) ApplyExtraPieces(&pcs, &pid);  // an empty slot holds no sample to frame
-    out.emplace_back(std::move(pcs), sc[c]);
-  }
+  if (spm_sample_encode_and_score_pieces(engine_, input.data(), offs, 1, num_samples, alpha, wor, include_best,
+                                         up ? up->data() : nullptr, up ? up->size() : 0, -1, &text, &to, &ends, &ids,
+                                         &co, &sc))
+    return out;
+  for (int c = 0; c < num_samples; ++c) out.emplace_back(PieceList(text, to, ends, co, c), sc[c]);
   return out;
 }
 

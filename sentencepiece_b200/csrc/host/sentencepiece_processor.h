@@ -116,6 +116,14 @@ class SentencePieceProcessor {
   util::Status EncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int sep, const char **text,
                                   const uint64_t **text_offsets, const uint32_t **piece_end,
                                   const uint64_t **id_offsets) const;
+  // NBestEncode / SampleEncode to pieces in the same layout, one list per candidate: candidate c of sentence i is list
+  // i * K + c (K = nbest_size clamped to [1, 1024]), n_cands[i] of the K are real (spm_nbest_encode_pieces)
+  util::Status NBestEncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int nbest_size, int sep,
+                                       const char **text, const uint64_t **text_offsets, const uint32_t **piece_end,
+                                       const uint64_t **cand_offsets, const uint32_t **n_cands) const;
+  util::Status SampleEncodePiecesPacked(const char *bytes, const uint64_t *offsets, size_t n, int nbest_size, float alpha,
+                                        int sep, const char **text, const uint64_t **text_offsets,
+                                        const uint32_t **piece_end, const uint64_t **id_offsets) const;
 
   // ---- Decode(ids) (src/sentencepiece_processor.h Decode(const std::vector<int>&, std::string*)); the batch form is
   //      one device call for all lists.  An id outside [0, GetPieceSize()) fails the call like the reference's
@@ -148,10 +156,8 @@ class SentencePieceProcessor {
   std::vector<int> frame_p_, frame_s_;
   bool frame_rev_ = false;
   util::Status ParseExtraOptions(std::string_view extra_option);
-  void RawIds(const int32_t *ids, size_t n, std::vector<int> *raw) const;
-  void ApplyExtraPieces(std::vector<std::string> *v, std::vector<int> *pid) const;
-  // pieces of an id sequence over the sentence's normalized text (unknown tokens keep their surface)
-  bool PiecesFromIds(std::string_view normalized, const int32_t *ids, size_t n, std::vector<std::string> *pieces) const;
+  // the unk_piece argument of the pieces calls: trainer_spec.unk_piece under UNK_PIECE, else null
+  const std::string *UnkPiece() const;
 };
 
 // sentencepiece_processor.h:731 / util.cc:23-31: the seed every generator created afterwards starts from; this

@@ -98,10 +98,6 @@ int main(int argc, char **argv) {
       for (size_t k = 0; k < v.size(); ++k) { if (k) buf += ' '; buf += std::to_string(v[k]); }
       buf += '\n';
     };
-    auto join_pieces = [&](const std::vector<std::string> &v) {
-      for (size_t k = 0; k < v.size(); ++k) { if (k) buf += ' '; buf += v[k]; }
-      buf += '\n';
-    };
     if (generate_vocabulary) {  // spm_encode_main.cc:102-110: counts of the pieces that are neither unknown nor control
       std::vector<std::vector<int>> ids;
       st = sp.Encode(views, &ids);
@@ -114,20 +110,34 @@ int main(int argc, char **argv) {
       st = sp.Encode(views, &ids);
       if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
       for (const auto &v : ids) join_ids(v);
-    } else if (format == "piece") {  // the engine writes each line's pieces joined by ' '
+    } else if (format == "piece" || format == "sample_piece" || format == "nbest_piece") {
+      // the engine writes each line's (candidate's) pieces joined by ' '
       std::string packed;
       std::vector<uint64_t> offs(lines.size() + 1, 0);
       for (size_t i = 0; i < lines.size(); ++i) { packed += lines[i]; offs[i + 1] = packed.size(); }
       const char *text;
       const uint64_t *to, *ido;
       const uint32_t *ends;
-      st = sp.EncodePiecesPacked(packed.data(), offs.data(), lines.size(), ' ', &text, &to, &ends, &ido);
-      if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
-      buf.reserve(to[lines.size()] + lines.size());
-      for (size_t i = 0; i < lines.size(); ++i) {
-        buf.append(text + to[i], to[i + 1] - to[i]);
-        buf += '\n';
+      const uint32_t *nc = nullptr;
+      size_t K = 1;
+      if (format == "piece") {
+        st = sp.EncodePiecesPacked(packed.data(), offs.data(), lines.size(), ' ', &text, &to, &ends, &ido);
+      } else if (format == "sample_piece") {
+        st = sp.SampleEncodePiecesPacked(packed.data(), offs.data(), lines.size(), nbest_size, alpha, ' ', &text, &to,
+                                         &ends, &ido);
+      } else {
+        st = sp.NBestEncodePiecesPacked(packed.data(), offs.data(), lines.size(), nbest_size, ' ', &text, &to, &ends, &ido,
+                                        &nc);
+        K = static_cast<size_t>(std::max(1, std::min(nbest_size, 1024)));
       }
+      if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
+      buf.reserve(to[lines.size() * K] + lines.size() * K);
+      for (size_t i = 0; i < lines.size(); ++i)
+        for (size_t c = 0; c < (nc ? nc[i] : 1u); ++c) {
+          const size_t j = i * K + c;
+          buf.append(text + to[j], to[j + 1] - to[j]);
+          buf += '\n';
+        }
     } else if (format == "proto") {
       std::vector<std::vector<std::string>> pcs;
       st = sp.Encode(views, &pcs);
@@ -137,21 +147,11 @@ int main(int argc, char **argv) {
       st = sp.SampleEncode(views, nbest_size, alpha, &ids);
       if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
       if (format == "sample_id") for (const auto &v : ids) join_ids(v);
-    } else if (format == "sample_piece") {
-      std::vector<std::vector<std::string>> pcs;
-      st = sp.SampleEncode(views, nbest_size, alpha, &pcs);
-      if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
-      for (const auto &v : pcs) join_pieces(v);
     } else if (format == "nbest_id" || format == "nbest_proto") {
       std::vector<std::vector<std::vector<int>>> ids;
       st = sp.NBestEncode(views, nbest_size, &ids);
       if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
       if (format == "nbest_id") for (const auto &c : ids) for (const auto &v : c) join_ids(v);
-    } else {  // nbest_piece
-      std::vector<std::vector<std::vector<std::string>>> pcs;
-      st = sp.NBestEncode(views, nbest_size, &pcs);
-      if (!st.ok()) { std::cerr << st.ToString() << "\n"; return 1; }
-      for (const auto &c : pcs) for (const auto &v : c) join_pieces(v);
     }
     enc_s += std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
     out.write(buf.data(), buf.size());

@@ -59,8 +59,29 @@ struct NbestOut {
   uint32_t *cand_count;            // [n * nbest]
   float *cand_score;               // [n * nbest]
   uint32_t *n_cands;               // [n]
-  uint32_t *status;                // [0] deferred sentences (shared with KBatch::status), [1] error, [2] overflow
+  uint32_t *status;                // [0] deferred sentences (shared with KBatch::status), [1] error, [2] overflow:
+                                   //     1u tmp_ids / tmp_end, 2u norm
+  // Pieces (null when the caller wants ids only).  tmp_end[k]: exclusive end, in bytes of the sentence's normalized
+  // text, of the token at tmp_ids[k] (the tok_end convention of spm_encode_spans).  norm: the normalized text of every
+  // sentence whose lattice holds an UNK node, appended at *norm_cursor; norm_start[sent] = its start, or kNoNorm.
+  uint32_t *tmp_end;
+  uint8_t *norm;
+  unsigned long long norm_cap;
+  unsigned long long *norm_cursor;
+  unsigned long long *norm_start;  // [n]
 };
+
+// Claims n bytes of O.norm for one sentence's normalized text, rounded up to whole 4-byte words so that the lane
+// kernel copies its slab's words as they are; kNoNorm (and the overflow bit) when they do not fit.
+__device__ __forceinline__ unsigned long long nbest_claim_norm(const NbestOut &O, uint32_t n) {
+  const uint32_t w = (n + 3u) & ~3u;
+  const unsigned long long pos = atomicAdd(O.norm_cursor, static_cast<unsigned long long>(w));
+  if (pos + w > O.norm_cap) {
+    atomicOr(O.status + 2, 2u);
+    return kNoNorm;
+  }
+  return pos;
+}
 
 // The agenda: std::push_heap / std::pop_heap on {fx bits, hypothesis} entries keyed by fx (comp: a.fx < b.fx).  Entry
 // i lives in s_top[i * 32] (shared memory, lane-strided) for i < TOP, else in heap slot i + 1.
@@ -132,6 +153,8 @@ struct NbestAgenda {
 // One result of Lattice::NBest as candidate `ck`: `cnt` ids of PopulateSentencePieceText's id path (UNK runs merged,
 // byte-fallback UNK nodes spelled as byte pieces) over the nodes that path(emit) visits left to right as
 // emit(id, begin char, end char); text_byte(k) is byte k of the normalized text, surf[c] the byte offset of char c.
+// With O.tmp_end, also each id's end in the normalized text: a merged UNK run ends where its last node ends, a
+// byte-fallback byte one byte after its start.
 template <typename SurfT, typename TextByte, typename Path>
 __device__ __forceinline__ void nbest_write_result(const KModel &M, const NbestOut &O, size_t ck, uint32_t cnt, float score,
                                                    const SurfT *surf, TextByte &&text_byte, Path &&path) {
@@ -151,11 +174,18 @@ __device__ __forceinline__ void nbest_write_result(const KModel &M, const NbestO
     const bool isunk = id == M.unk_id;
     if (isunk) {
       if (bf) {
-        for (uint32_t k = surf[b]; k < surf[e]; ++k) O.tmp_ids[pos + (w++)] = __ldg(M.byte_to_id + text_byte(k));
+        for (uint32_t k = surf[b]; k < surf[e]; ++k) {
+          if (O.tmp_end) O.tmp_end[pos + w] = k + 1u;
+          O.tmp_ids[pos + (w++)] = __ldg(M.byte_to_id + text_byte(k));
+        }
       } else if (!prev_unk) {
+        if (O.tmp_end) O.tmp_end[pos + w] = surf[e];
         O.tmp_ids[pos + (w++)] = M.unk_id;
+      } else if (O.tmp_end) {
+        O.tmp_end[pos + w - 1] = surf[e];
       }
     } else {
+      if (O.tmp_end) O.tmp_end[pos + w] = surf[e];
       O.tmp_ids[pos + (w++)] = id;
     }
     prev_unk = isunk;
@@ -199,6 +229,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
       const bool too_big = !lane_k1(M, B, c, sent, G.cap, &n);
       const size_t cbase = static_cast<size_t>(sent) * nbest;
       uint32_t K = 0;
+      unsigned long long norm_at = kNoNorm;
       if (too_big) {
         lane_defer_long(B, sent, 0u);
       } else if (n == 0) {
@@ -222,7 +253,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
         // nodes 0 = BOS, 1 = EOS (EOS's backtrace score is filled in below)
         uint32_t nn = 2;
         node[0] = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-        bool overflow = false;
+        bool overflow = false, has_unk = false;
         // ---- Model::PopulateNodes, with Lattice::Viterbi's backtrace scores folded in ----
         // backtrace(r) = max over nodes q ending where r begins of fl(backtrace(q) + score(r)); fl(x + s) is
         // monotone in x, so it equals fl(max_q backtrace(q) + score(r)), and every q is complete before r is made.
@@ -244,6 +275,7 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
                                   bp | ((bp + 1) << 16));
             maxbt[bp + 1] = fmaxf(maxbt[bp + 1], bt);
             ++nn;
+            has_unk = true;
           }
         }
         if (!overflow) {
@@ -308,9 +340,17 @@ __global__ void __launch_bounds__(THREADS, 1) nbest_lane_kernel(const KModel M, 
             }
           }
         }
-        if (overflow) lane_defer_long(B, sent, n);  // the long-sentence path redoes the sentence with 32-bit indices
+        if (overflow) {
+          lane_defer_long(B, sent, n);  // the long-sentence path redoes the sentence with 32-bit indices
+        } else if (O.norm && has_unk) {
+          norm_at = nbest_claim_norm(O, n);
+          if (norm_at != kNoNorm)  // word k of the slab holds bytes 4k .. 4k+3 (the bytes past n are padding)
+            for (uint32_t k = 0; 4u * k < n; ++k)
+              reinterpret_cast<uint32_t *>(O.norm + norm_at)[k] = c.text_w[static_cast<size_t>(k) * 32];
+        }
       }
       O.n_cands[sent] = K;
+      if (O.norm) O.norm_start[sent] = norm_at;
       for (uint32_t k = K; k < nbest; ++k) { O.cand_count[cbase + k] = 0; O.cand_start[cbase + k] = 0; O.cand_score[cbase + k] = 0.f; }
     }
     __syncwarp();
@@ -379,6 +419,7 @@ __global__ void __launch_bounds__(256) nbest_long_kernel(const KModel M, const K
       continue;
     }
     uint32_t K = 0;
+    unsigned long long norm_at = kNoNorm;
     if (n == 0) {
       if (lane == 0) { O.cand_start[cbase] = 0; O.cand_count[cbase] = 0; O.cand_score[cbase] = 0.f; }
       K = 1;
@@ -387,13 +428,17 @@ __global__ void __launch_bounds__(256) nbest_long_kernel(const KModel M, const K
       auto text_byte = [&](uint32_t k) -> uint32_t { return text[k]; };
       // ---- Model::PopulateNodes: count the nodes of every start, then write them at their offsets ----
       uint32_t nn = 2;  // BOS, EOS
+      bool has_unk = false;
       for (uint32_t b0 = 0; b0 < L; b0 += 32) {
         const uint32_t bp = b0 + lane;
         uint32_t cnt = 0;
+        bool unk_here = false;
         if (bp < L) {
           const bool single = populate_from(M, text_byte, root, surf, bp, n, [&](uint32_t, uint32_t, float) { ++cnt; return true; });
           cnt += single ? 0u : 1u;
+          unk_here = !single;
         }
+        has_unk |= __any_sync(0xFFFFFFFFu, unk_here);
         const uint32_t incl = T.incl_scan(cnt);
         if (bp < L) nstart[bp] = nn + incl - cnt;
         nn += T.shfl(incl, 31);
@@ -418,6 +463,7 @@ __global__ void __launch_bounds__(256) nbest_long_kernel(const KModel M, const K
       for (uint32_t p = lane; p <= L + 1; p += 32) { maxbt[p] = -INFINITY; end_off[p] = 0; }
       for (uint32_t i = lane; i < hyp_cap; i += 32) fwd[i] = 0;
       __syncwarp();
+      uint32_t need = 0;
       if (lane == 0) {
         node[0] = make_uint4(kNull, 0u, 0u, 0u);
         node[1] = make_uint4(kNull, 0u, 0u, L);
@@ -448,7 +494,7 @@ __global__ void __launch_bounds__(256) nbest_long_kernel(const KModel M, const K
           elist[sort_cur[e]++] = make_uint4(i, nd.z, nd.y, contrib | (isunk ? 0x80000000u : 0u));
         }
         // ---- Lattice::NBest: backward A* ----
-        uint32_t pn = 1, hn = 0, need = 0;
+        uint32_t pn = 1, hn = 0;
         hyp[0] = make_uint4(kNull, 0u, 1u, 0u);  // EOS: next = null, gx = 0, no ids yet
         ag.push(hn, make_uint2(__float_as_uint(eos_bt), 0u));
         const uint32_t shrink_to = nbest * 10 < 512 ? nbest * 10 : 512;
@@ -509,8 +555,19 @@ __global__ void __launch_bounds__(256) nbest_long_kernel(const KModel M, const K
         long_need[w] = need;
       }
       K = T.shfl(K, 0);
+      need = T.shfl(need, 0);
+      if (O.norm && has_unk && need == 0) {  // a sentence that runs again with a larger pool exports its text then
+        unsigned long long pos = 0;
+        if (lane == 0) pos = nbest_claim_norm(O, n);
+        norm_at = __shfl_sync(0xFFFFFFFFu, pos, 0);
+        if (norm_at != kNoNorm)
+          for (uint32_t k = lane; k < n; k += 32) O.norm[norm_at + k] = text[k];
+      }
     }
-    if (lane == 0) O.n_cands[sent] = K;
+    if (lane == 0) {
+      O.n_cands[sent] = K;
+      if (O.norm) O.norm_start[sent] = norm_at;
+    }
     for (uint32_t k = K + lane; k < nbest; k += 32) { O.cand_count[cbase + k] = 0; O.cand_start[cbase + k] = 0; O.cand_score[cbase + k] = 0.f; }
     __syncwarp();
   }

@@ -10,9 +10,14 @@
 // is id == unk_id.  Every other piece comes from a per-id table of the raw piece bytes (U+2581 kept).  Unknown
 // surfaces come from the spans path, which only the sentences that hold an unknown id take (the flag pass below).
 //
-// One WARP per sentence, one token per lane, output positions by a warp scan -- the shape of K7
-// (decode_kernel.cuh).  A size pass writes each sentence's byte and token counts; the scan kernels of the encode path
+// One WARP per list, one token per lane, output positions by a warp scan -- the shape of K7
+// (decode_kernel.cuh).  A size pass writes each list's byte and token counts; the scan kernels of the encode path
 // turn them into offsets; the write pass writes the bytes, the piece ends and the framed ids in place.
+//
+// A list is one sentence's segmentation (EncodeAsPieces) or one candidate of the n-best / sampling paths
+// (spm_nbest_encode_pieces, spm_sample_encode_pieces): list j then reads its ids from the candidate buffer at
+// list_start[j], the ends of its tokens from the parallel tok_end, and the normalized text of sentence j / per, which
+// K5 exported only for sentences whose lattice holds an UNK node.
 #ifndef SPM_B200_PIECES_KERNEL_CUH_
 #define SPM_B200_PIECES_KERNEL_CUH_
 
@@ -26,10 +31,19 @@ constexpr uint32_t kNoSub = 0xFFFFFFFFu;  // sub_of[i]: sentence i did not take 
 constexpr uint32_t kPieceWarpCopy = 32;   // pieces longer than this are copied by the whole warp
 
 struct KPieces {
-  uint32_t n;
-  // raw segmentation of the lane / BPE-lane2 kernels (no frame)
+  uint32_t n;  // lists
+  // raw segmentation (no frame): list j is ids[id_offsets[j], id_offsets[j + 1]) or, when list_start is given,
+  // ids[list_start[j], + list_count[j])
   const int32_t *ids;
   const unsigned long long *id_offsets;
+  const unsigned long long *list_start;
+  const uint32_t *list_count;
+  // token ends parallel to ids (null: none); list j's normalized text at sent_norm + sent_norm_start[j / per] (kNoNorm:
+  // the sentence has no unknown surface)
+  const uint32_t *tok_end;
+  const uint8_t *sent_norm;
+  const unsigned long long *sent_norm_start;
+  uint32_t per;
   // the unknown-surface subset: sentence i is sentence sub_of[i] of a spans run (null: no subset)
   const uint32_t *sub_of;
   const int32_t *sub_ids;
@@ -69,9 +83,22 @@ __device__ __forceinline__ PiecesSrc pieces_src(const KPieces &P, uint32_t sent)
   PiecesSrc s{};
   const uint32_t j = P.sub_of ? P.sub_of[sent] : kNoSub;
   if (j == kNoSub) {
-    const unsigned long long a = P.id_offsets[sent];
+    unsigned long long a;
+    if (P.list_start) {
+      a = P.list_start[sent];
+      s.L = P.list_count[sent];
+    } else {
+      a = P.id_offsets[sent];
+      s.L = static_cast<uint32_t>(P.id_offsets[sent + 1] - a);
+    }
     s.ids = P.ids + a;
-    s.L = static_cast<uint32_t>(P.id_offsets[sent + 1] - a);
+    if (P.tok_end) {
+      const unsigned long long b = P.sent_norm_start[sent / P.per];
+      if (b != kNoNorm) {
+        s.tok_end = P.tok_end + a;
+        s.norm = P.sent_norm + b;
+      }
+    }
   } else {
     const unsigned long long a = P.sub_id_offsets[j];
     s.ids = P.sub_ids + a;
@@ -82,10 +109,9 @@ __device__ __forceinline__ PiecesSrc pieces_src(const KPieces &P, uint32_t sent)
   return s;
 }
 
-// Token t (< np + L + ns) of the framed list: its id and the bytes of its piece.
-__device__ __forceinline__ int32_t piece_at(const KPieces &P, const PiecesSrc &s, uint32_t t, const uint8_t **src,
-                                            uint32_t *len) {
-  const uint32_t np = P.F.np;
+// Token t (< np + L + ns) of the framed list: its id and the bytes of its piece.  np = 0 for a list without a frame.
+__device__ __forceinline__ int32_t piece_at(const KPieces &P, const PiecesSrc &s, uint32_t np, uint32_t t,
+                                            const uint8_t **src, uint32_t *len) {
   int32_t id;
   uint32_t q = 0xFFFFFFFFu;  // index in the raw segmentation, for body tokens
   if (t < np) {
@@ -148,7 +174,9 @@ __global__ void __launch_bounds__(256) pieces_warp_kernel(const KPieces P) {
   const uint32_t sep_w = P.sep >= 0 ? 1u : 0u;
   for (uint32_t sent = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; sent < P.n; sent += warps) {
     const PiecesSrc s = pieces_src(P, sent);
-    const uint32_t T = P.F.np + s.L + P.F.ns;
+    const uint32_t added = P.F.added(sent);  // 0: an empty n-best slot, which stays empty
+    const uint32_t np = added ? P.F.np : 0u;
+    const uint32_t T = s.L + added;
     uint8_t *out = nullptr;
     uint32_t *ends = nullptr;
     int32_t *oids = nullptr;
@@ -164,7 +192,7 @@ __global__ void __launch_bounds__(256) pieces_warp_kernel(const KPieces P) {
       uint32_t len = 0, w = 0;
       int32_t id = 0;
       if (t < T) {
-        id = piece_at(P, s, t, &src, &len);
+        id = piece_at(P, s, np, t, &src, &len);
         w = len + (t + 1 < T ? sep_w : 0u);
       }
       uint32_t incl = w;

@@ -149,19 +149,74 @@ class Engine:
         n = len(offs) - 1
         buf = np.ascontiguousarray(buf, dtype=np.uint8)
         offs = np.ascontiguousarray(offs, dtype=np.uint64)
-        if isinstance(unk_piece, str):
-            unk_piece = unk_piece.encode("utf-8")
         p = [ctypes.c_void_p() for _ in range(5)]
-        self._check(self._lib.spm_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, unk_piece,
-                                                len(unk_piece) if unk_piece is not None else 0, sep,
+        self._check(self._lib.spm_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, *self._unk(unk_piece), sep,
                                                 *[ctypes.byref(x) for x in p]))
-        to = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
-        ido = np.ctypeslib.as_array(ctypes.cast(p[4], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
-        tt, tot = int(to[n]), int(ido[n])
-        text = np.frombuffer(ctypes.string_at(p[0], tt), dtype=np.uint8) if tt else np.zeros(0, np.uint8)
+        return self._pieces_result(p, n)
+
+    @staticmethod
+    def _pieces_result(p, lists):
+        """text, text_offsets, piece_end, ids and the id offsets of `lists` packed piece lists (pointers p[0..4])"""
+        to = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (lists + 1,)).copy()
+        ido = np.ctypeslib.as_array(ctypes.cast(p[4], ctypes.POINTER(ctypes.c_uint64)), (lists + 1,)).copy()
+        tt, tot = int(to[lists]), int(ido[lists])
+        # (not ctypes.string_at: its size is a C int, and n-best text passes 2 GB at config 5's sizes)
+        text = np.ctypeslib.as_array(ctypes.cast(p[0], ctypes.POINTER(ctypes.c_uint8)), (max(tt, 1),))[:tt].copy()
         pe = np.ctypeslib.as_array(ctypes.cast(p[2], ctypes.POINTER(ctypes.c_uint32)), (max(tot, 1),))[:tot].copy()
         ids = np.ctypeslib.as_array(ctypes.cast(p[3], ctypes.POINTER(ctypes.c_int32)), (max(tot, 1),))[:tot].copy()
         return dict(text=text, text_offsets=to, piece_end=pe, ids=ids, id_offsets=ido)
+
+    @staticmethod
+    def _unk(unk_piece):
+        if isinstance(unk_piece, str):
+            unk_piece = unk_piece.encode("utf-8")
+        return unk_piece, len(unk_piece) if unk_piece is not None else 0
+
+    def nbest_encode_pieces(self, buf, offs, nbest_size, unk_piece=None, sep=-1):
+        """spm_nbest_encode_pieces: NBestEncodeAsPieces over a packed batch -> dict(text, text_offsets uint64[n*K+1],
+        piece_end, ids, cand_offsets uint64[n*K+1], scores float32[n*K], n_cands uint32[n], K); candidate c of sentence
+        i is list i*K + c, laid out as encode_pieces lays out a sentence."""
+        n = len(offs) - 1
+        K = max(1, min(nbest_size, 1024))
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(7)]
+        self._check(self._lib.spm_nbest_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, nbest_size,
+                                                      *self._unk(unk_piece), sep, *[ctypes.byref(x) for x in p]))
+        nc = n * K
+        r = self._pieces_result(p[:5], nc)
+        r["cand_offsets"] = r.pop("id_offsets")
+        r["scores"] = np.ctypeslib.as_array(ctypes.cast(p[5], ctypes.POINTER(ctypes.c_float)), (max(nc, 1),))[:nc].copy()
+        r["n_cands"] = np.ctypeslib.as_array(ctypes.cast(p[6], ctypes.POINTER(ctypes.c_uint32)), (max(n, 1),))[:n].copy()
+        r["K"] = K
+        return r
+
+    def sample_encode_pieces(self, buf, offs, nbest_size, alpha, unk_piece=None, sep=-1):
+        """spm_sample_encode_pieces: SampleEncodeAsPieces over a packed batch -> the dict of encode_pieces"""
+        n = len(offs) - 1
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(5)]
+        self._check(self._lib.spm_sample_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, nbest_size, alpha,
+                                                       *self._unk(unk_piece), sep, *[ctypes.byref(x) for x in p]))
+        return self._pieces_result(p, n)
+
+    def sample_encode_and_score_pieces(self, buf, offs, num_samples, alpha, wor=False, include_best=False,
+                                       unk_piece=None, sep=-1):
+        """spm_sample_encode_and_score_pieces -> dict(text, text_offsets, piece_end, ids, cand_offsets, scores) over
+        n*num_samples lists, sample c of sentence i being list i*num_samples + c"""
+        n = len(offs) - 1
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(6)]
+        self._check(self._lib.spm_sample_encode_and_score_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, num_samples,
+                                                                 alpha, int(wor), int(include_best), *self._unk(unk_piece),
+                                                                 sep, *[ctypes.byref(x) for x in p]))
+        nc = n * num_samples
+        r = self._pieces_result(p[:5], nc)
+        r["cand_offsets"] = r.pop("id_offsets")
+        r["scores"] = np.ctypeslib.as_array(ctypes.cast(p[5], ctypes.POINTER(ctypes.c_float)), (max(nc, 1),))[:nc].copy()
+        return r
 
     def decode_packed(self, ids, id_offsets):
         """Batch Decode of packed id lists -> (text uint8[], text_offsets uint64[n+1])."""
@@ -336,11 +391,8 @@ class SentencePieceProcessor:
     #      bos / eos / reverse through the encode frame, UNK_PIECE through unk_piece ----
     def EncodeAsPieces(self, input, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
-        opts = self._options(add_bos, add_eos, reverse) + ["unk"] * bool(emit_unk_piece)
-        single = isinstance(input, (str, bytes))
-        buf, offs = pack_sentences([input] if single else input)
-        self._set_frame(add_bos, add_eos, reverse)
-        unk = self._specials()["unk_piece"] if "unk" in opts else None
+        single, (buf, offs) = self._split(input)
+        unk = self._pieces_frame(add_bos, add_eos, reverse, emit_unk_piece)
         r = self._engine.encode_pieces(buf, offs, unk_piece=unk)
         out = split_pieces(r["text"], r["text_offsets"], r["piece_end"], r["id_offsets"])
         return out[0] if single else out
@@ -351,9 +403,9 @@ class SentencePieceProcessor:
         add_bos / add_eos / reverse apply after SetEncodeExtraOptions' options, in the order reverse, bos, eos."""
         kw = dict(add_bos=add_bos, add_eos=add_eos, reverse=reverse, emit_unk_piece=emit_unk_piece)
         if enable_sampling:
-            if out_type is not int:
-                raise NotImplementedError("sampled pieces: use the C++ host layer (SampleEncodeAsPieces)")
-            return self.SampleEncodeAsIds(input, nbest_size, alpha, **kw)
+            if out_type is int:
+                return self.SampleEncodeAsIds(input, nbest_size, alpha, **kw)
+            return self.SampleEncodeAsPieces(input, nbest_size, alpha, **kw)
         return self.EncodeAsIds(input, **kw) if out_type is int else self.EncodeAsPieces(input, **kw)
 
     Encode = encode
@@ -371,6 +423,21 @@ class SentencePieceProcessor:
         out = [ids[int(ido[i]):int(ido[i + 1])].tolist() for i in range(len(offs) - 1)]
         return out[0] if single else out
 
+    def SampleEncodeAsPieces(self, input, nbest_size, alpha, add_bos=False, add_eos=False, reverse=False,
+                             emit_unk_piece=False):
+        self._require()
+        single, (buf, offs) = self._split(input)
+        unk = self._pieces_frame(add_bos, add_eos, reverse, emit_unk_piece)
+        r = self._engine.sample_encode_pieces(buf, offs, nbest_size, alpha, unk_piece=unk)
+        out = split_pieces(r["text"], r["text_offsets"], r["piece_end"], r["id_offsets"])
+        return out[0] if single else out
+
+    def _pieces_frame(self, add_bos, add_eos, reverse, emit_unk_piece):
+        """Sets the frame for a pieces call and returns its unk_piece argument."""
+        opts = self._options(add_bos, add_eos, reverse) + ["unk"] * bool(emit_unk_piece)
+        self._set_frame(add_bos, add_eos, reverse)
+        return self._specials()["unk_piece"] if "unk" in opts else None
+
     # sentencepiece_processor.h:471
     def NBestEncodeAsIds(self, input, nbest_size, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
         self._require()
@@ -381,6 +448,50 @@ class SentencePieceProcessor:
         out = [[r["ids"][int(co[i * K + c]):int(co[i * K + c + 1])].tolist() for c in range(int(r["n_cands"][i]))]
                for i in range(len(offs) - 1)]
         return out[0] if single else out
+
+    def NBestEncodeAsPieces(self, input, nbest_size, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
+        self._require()
+        single, (buf, offs) = self._split(input)
+        unk = self._pieces_frame(add_bos, add_eos, reverse, emit_unk_piece)
+        r = self._engine.nbest_encode_pieces(buf, offs, nbest_size, unk_piece=unk)
+        K = r["K"]
+        lists = split_pieces(r["text"], r["text_offsets"], r["piece_end"], r["cand_offsets"])
+        out = [lists[i * K:i * K + int(r["n_cands"][i])] for i in range(len(offs) - 1)]
+        return out[0] if single else out
+
+    # python/src/sentencepiece/__init__.py NBestEncode
+    def NBestEncode(self, input, out_type=int, nbest_size=-1, add_bos=False, add_eos=False, reverse=False,
+                    emit_unk_piece=False):
+        f = self.NBestEncodeAsIds if out_type is int else self.NBestEncodeAsPieces
+        return f(input, nbest_size, add_bos=add_bos, add_eos=add_eos, reverse=reverse, emit_unk_piece=emit_unk_piece)
+
+    # sentencepiece_processor.h:500-510: (list, score) pairs, num_samples per sentence; wor / include_best are not on
+    # the device path
+    def SampleEncodeAndScore(self, input, out_type=int, num_samples=-1, alpha=0.1, wor=False, include_best=False,
+                             add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
+        self._require()
+        single, (buf, offs) = self._split(input)
+        if out_type is int:
+            self._set_frame(add_bos, add_eos, reverse)
+            ids, co, sc = self._engine.sample_encode_and_score(buf, offs, num_samples, alpha, wor, include_best)
+            lists = [ids[int(co[j]):int(co[j + 1])].tolist() for j in range(len(co) - 1)]
+        else:
+            unk = self._pieces_frame(add_bos, add_eos, reverse, emit_unk_piece)
+            r = self._engine.sample_encode_and_score_pieces(buf, offs, num_samples, alpha, wor, include_best, unk_piece=unk)
+            co, sc = r["cand_offsets"], r["scores"]
+            lists = split_pieces(r["text"], r["text_offsets"], r["piece_end"], co)
+        out = []
+        for i in range(len(offs) - 1):
+            js = range(i * num_samples, (i + 1) * num_samples)
+            # a sentence that normalizes to nothing has no samples (unigram_model.cc:745-747); only its slots are empty
+            out.append([(lists[j], float(sc[j])) for j in js] if int(co[js[-1] + 1]) > int(co[js[0]]) else [])
+        return out[0] if single else out
+
+    def SampleEncodeAndScoreAsIds(self, input, num_samples=-1, alpha=0.1, wor=False, include_best=False, **kw):
+        return self.SampleEncodeAndScore(input, int, num_samples, alpha, wor, include_best, **kw)
+
+    def SampleEncodeAndScoreAsPieces(self, input, num_samples=-1, alpha=0.1, wor=False, include_best=False, **kw):
+        return self.SampleEncodeAndScore(input, str, num_samples, alpha, wor, include_best, **kw)
 
     # sentencepiece_processor.h:521-526
     def CalculateEntropy(self, input, alpha):
