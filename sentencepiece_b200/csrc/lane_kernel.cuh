@@ -133,6 +133,15 @@ __device__ __forceinline__ unsigned long long slab_policy() {
   const uint32_t hi = __reduce_or_sync(0xFFFFFFFFu, static_cast<uint32_t>(pol >> 32));
   return (static_cast<unsigned long long>(hi) << 32) | lo;
 }
+// The same redux for a value that is equal on every lane (a kernel parameter, a pointer into it): the compiler keeps it in
+// a uniform register instead of reloading it from the constant bank (LDC) inside the loops that use it.
+__device__ __forceinline__ uint32_t warp_uniform(uint32_t v) { return __reduce_or_sync(0xFFFFFFFFu, v); }
+template <typename T>
+__device__ __forceinline__ T *warp_uniform(T *p) {
+  const unsigned long long v = reinterpret_cast<uintptr_t>(p);
+  const unsigned long long lo = warp_uniform(static_cast<uint32_t>(v)), hi = warp_uniform(static_cast<uint32_t>(v >> 32));
+  return reinterpret_cast<T *>(static_cast<uintptr_t>((hi << 32) | lo));
+}
 __device__ __forceinline__ uint32_t slab_ld(const uint32_t *p, unsigned long long pol) {
   uint32_t v;
   asm volatile("ld.global.L2::cache_hint.u32 %0, [%1], %2;" : "=r"(v) : "l"(p), "l"(pol) : "memory");
@@ -747,6 +756,22 @@ constexpr uint32_t kParkNum = 1, kParkDen = 2;
 static_assert(0 < kParkNum && kParkNum <= kParkDen, "the start step must run at the latest when every live lane is parked");
 __device__ __forceinline__ uint32_t park_need(uint32_t live) { return (live * kParkNum + kParkDen - 1u) / kParkDen; }
 
+// Slides K2's text window w0..w3 (words aw .. aw+3 of the lane's text) forward by jw words, to the words at p (the
+// lane's word aw + jw in the slab).  Branch-free: the words the window still holds move down by selects, and only the
+// ones it does not hold are reloaded, by predicated loads -- w3 once jw >= 1, w2 once jw >= 2, all four once jw >= 3
+// (a long whole word).  The loads go straight to the registers that need them, so the walk waits for w3 (bytes 12..15
+// of the window) only when it gets there.
+__device__ __forceinline__ void lane_window_slide(uint32_t &w0, uint32_t &w1, uint32_t &w2, uint32_t &w3, uint32_t jw,
+                                                  const uint32_t *p, unsigned long long pol) {
+  const uint32_t n0 = jw == 0u ? w0 : (jw == 1u ? w1 : w2);
+  const uint32_t n1 = jw == 0u ? w1 : (jw == 1u ? w2 : w3);
+  const uint32_t n2 = jw == 0u ? w2 : w3;
+  w0 = n0; w1 = n1; w2 = n2;
+  if (jw >= 1u) w3 = slab_ld(p + 96, pol);
+  if (jw >= 2u) w2 = slab_ld(p + 64, pol);
+  if (jw >= 3u) { w0 = slab_ld(p, pol); w1 = slab_ld(p + 32, pol); }
+}
+
 constexpr uint32_t kLogWordStep = 1u << 31;  // log entry: the previous logged position is plen bytes back (whole word)
 constexpr uint32_t kWsWord = 0x8196E2u;      // U+2581 as the low three bytes of a little-endian word
 // OneCharLen in the kWsByte spelling: U+2581 is one byte
@@ -771,7 +796,11 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  const LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  // One 64-bit base for the lane's column of the slab, c.text_w, and 32-bit word offsets from it: text word w is at w*32,
+  // log entry t at log0 + t*32.  K4 takes its log pointer from the same base.
+  const uint32_t log0 = (cap / 4 + kLaneTextSlack) * 32;
+  c.log = c.text_w + log0;
   // ring offsets (see kRingSlot): the lane's score in slot 0, one past the last slot.  Position tags: a slot belongs to
   // position p iff its tag == p (no clearing: skipped positions of whole words leave stale slots behind that simply
   // fail the test).
@@ -780,11 +809,14 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
   const uint32_t ring_span = lane_ring_bytes(R);
   const uint32_t ring_hi = ring_lo + ring_span;
   const uint32_t tag_delta = kRingTag - 2u * lane;
-  const uint4 *node4 = M.trie_node4;
+  // What K2 reads on every trip or every start step stays in (uniform) registers: the trie, the model's flags and
+  // max_score.  wstart does not test kFlagFastWords: the engine launches this kernel only with the flag set, and
+  // without it every word_safe entry is 0, so that no walk could take the shortcut anyway.
+  const uint4 *node4 = warp_uniform(M.trie_node4);
   const uint32_t root = __ldg(&node4[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
-  const bool regular = M.flags & kFlagRegularScores;
-  const bool fastwords = M.flags & kFlagFastWords;
+  const bool regular = warp_uniform(M.flags & kFlagRegularScores) != 0u;
+  const float max_score = __uint_as_float(warp_uniform(__float_as_uint(M.max_score)));
 
   uint32_t first = 0;
   while (lane_claim_group(B, lane, &first)) {
@@ -805,9 +837,10 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; ch = the byte at the walk position k and `cur`
     // streams the bytes after it (low byte first).  ss = ring offset of s's slot.  When the walk ends, ch is the byte
     // that failed the label test or the child mask, for the word-end test of the start step.
-    uint32_t s = 0, ss = ring_lo, k = 0, l = root, lsafe = 0, mblen = 1, nlog = 0, ch = 0;
+    // lg: word offset of the lane's next log entry.
+    uint32_t s = 0, ss = ring_lo, k = 0, l = root, lsafe = 0, mblen = 1, lg = log0, ch = 0;
     bool has_single = false, parked = false;  // the lane is done once s reaches n
-    bool wstart = fastwords;  // the shortcut is on and s is the first character of a word (text start or kWsByte)
+    bool wstart = true;  // s is the first character of a word (text start or kWsByte)
     float base = 0.f;
     bool base_regular = regular;  // base == 0
     uint32_t w0 = 0, w1 = 0, w2 = 0, w3 = 0;
@@ -825,7 +858,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
     if (n != 0) {
       for (uint32_t r = 0; r < R; ++r) ring_st_tag(ring_lo + r * kRingSlot + tag_delta, 0xFFFFu);  // no slot belongs to a position of this sentence
       ring_st_score(ring_lo, 0.f);
-      w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
+      w0 = slab_ld(c.text_w, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len_ws1(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
@@ -849,61 +882,43 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
         ++st_steps;
         if (parked) {
           // the walk from s is over (traverse() == -2, or end of text).  Whole word: the walk covered [s, k) from a
-          // word start and ended on a NORMAL piece at the end of the word, early enough to be safe.
+          // word start and ended on a NORMAL piece at the end of the word, early enough to be safe; the piece was
+          // relaxed into k when the walk stepped onto its node, and nothing else can win there.  Otherwise the step is
+          // one character, with the UNK edge if no one-character piece began at s.  The two cases differ only in the
+          // step, the log tag and the UNK edge, so the block is straight-line code for both: a start step issues one
+          // path whatever mix of whole-word and character lanes it runs.
           const bool fast = wstart && k > s && ((l >> kLinkKindShift) & 3u) == kKindNormal && (k >= n || ch == kWsByte) &&
                             k <= lsafe;
-          const uint32_t s_old = s;
-          uint32_t steplog;
-          if (fast) {
-            // the piece was relaxed into k when the walk stepped onto its node; nothing else can win there
-            ss += (k - s) * kRingSlot;
-            if (ss >= ring_hi) ss -= ring_span;
-            s = k;
-            steplog = kLogWordStep;
-          } else {
-            uint32_t sl = ss + mblen * kRingSlot;
-            if (sl >= ring_hi) sl -= ring_span;
-            if (!has_single) {  // UNK edge, unigram_model.cc:995-1005
-              const float cand = __fadd_rn(M.unk_score, base);
-              if (ring_ld_tag(sl + tag_delta) != s + mblen || cand > ring_ld_score(sl)) {
-                ring_st_score(sl, cand);
-                ring_st_bp(sl, (mblen << 24) | kLaneUnk);
-                ring_st_tag(sl + tag_delta, s + mblen);
-              }
+          const uint32_t step = fast ? k - s : mblen;
+          uint32_t sl = ss + step * kRingSlot;
+          if (sl >= ring_hi) sl -= ring_span;
+          if (!fast && !has_single) {  // UNK edge, unigram_model.cc:995-1005
+            const float cand = __fadd_rn(M.unk_score, base);
+            if (ring_ld_tag(sl + tag_delta) != s + mblen || cand > ring_ld_score(sl)) {
+              ring_st_score(sl, cand);
+              ring_st_bp(sl, (mblen << 24) | kLaneUnk);
+              ring_st_tag(sl + tag_delta, s + mblen);
             }
-            ss = sl;
-            s += mblen;
-            steplog = (mblen - 1u) << 22;
           }
+          const uint32_t aw = s >> 2;
+          ss = sl;
+          s += step;
           // position s is final: append (plen | previous char length or whole-word step | unit) to the log
-          slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | steplog, c.pol);
-          ++nlog;
-          if (s < n) {
-            base = ring_ld_score(ss);
-            base_regular = regular && score_regular(base);
-            // slide the text window so that it is anchored at s; prefetch the new tail word
-            const uint32_t jw = (s >> 2) - (s_old >> 2);
-            if (jw == 1u) {
-              w0 = w1; w1 = w2; w2 = w3;
-              w3 = slab_ld(c.text_w + static_cast<size_t>((s >> 2) + 3) * 32, c.pol);
-            } else if (jw == 2u) {
-              w0 = w2; w1 = w3;
-              w2 = slab_ld(c.text_w + static_cast<size_t>((s >> 2) + 2) * 32, c.pol);
-              w3 = slab_ld(c.text_w + static_cast<size_t>((s >> 2) + 3) * 32, c.pol);
-            } else if (jw != 0u) {
-              const uint32_t *tw = c.text_w + static_cast<size_t>(s >> 2) * 32;
-              w0 = slab_ld(tw + 0, c.pol); w1 = slab_ld(tw + 32, c.pol); w2 = slab_ld(tw + 64, c.pol); w3 = slab_ld(tw + 96, c.pol);
-            }
-            cur = window_low();
-            ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
-            cur >>= 8;
-            wstart = fastwords && ch == kWsByte;
-            mblen = one_char_len_ws1(ch);
-            if (mblen > n - s) mblen = n - s;
-            k = s;
-            l = root;
-            has_single = false;
-          }
+          slab_st(c.text_w + lg, ring_ld_bp(ss) | (fast ? kLogWordStep : (mblen - 1u) << 22), c.pol);
+          lg += 32;
+          // the next walk, from s.  A lane that has reached n is done and ignores it (the window words past the text
+          // are within the slab's slack).
+          base = ring_ld_score(ss);
+          base_regular = regular && score_regular(base);
+          lane_window_slide(w0, w1, w2, w3, (s >> 2) - aw, c.text_w + (s >> 2) * 32, c.pol);
+          cur = window_low();
+          ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
+          cur >>= 8;
+          wstart = ch == kWsByte;
+          mblen = min(one_char_len_ws1(ch), n - s);
+          k = s;
+          l = root;
+          has_single = false;
           parked = false;
         }
         need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
@@ -940,7 +955,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
             } else {
               const double sc = kind == kKindNormal
                                     ? static_cast<double>(__uint_as_float(nd.z))
-                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
+                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), max_score)) - 0.1;
               const double cand = sc + static_cast<double>(base);
               better = unset || cand > static_cast<double>(curs);
               ns = static_cast<float>(cand);
@@ -957,7 +972,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
           if (k < n) {
             const uint32_t d = k - s;
             if (d >= 13u) {  // beyond the register window: long piece, rare
-              ch = lane_text_byte(c, k);
+              ch = (slab_ld(c.text_w + (k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
             } else {
               if (d == 8u) cur = window_high();
               ch = static_cast<uint32_t>(cur) & 0xFFu;
@@ -968,6 +983,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_kernel(const KMod
         }
       }
     }
+    const uint32_t nlog = (lg - log0) >> 5;
     if (kst) {
       typedef unsigned long long ull;
       uint32_t st_fast = 0;
@@ -1005,16 +1021,21 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warp_in_cta = threadIdx.x >> 5;
   const uint32_t warp_global = blockIdx.x * (blockDim.x >> 5) + warp_in_cta;
-  const LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  LaneCtx c = lane_ctx(s_tab, slabs, cap, warp_global, lane);
+  // slab addressing, K2's parameters in (uniform) registers: see encode_unigram_lane_kernel
+  const uint32_t log0 = (cap / 4 + kLaneTextSlack) * 32;
+  c.log = c.text_w + log0;
   // ring offsets (see kRingSlot): the lane's score in slot 0, one past the last slot
   const uint32_t ring_lo = static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + kLaneTableBytes +
                            warp_in_cta * lane_plain_ring_bytes(R) + lane * 4u;
   const uint32_t ring_span = lane_plain_ring_bytes(R);
   const uint32_t ring_hi = ring_lo + ring_span;
-  const uint2 *node2 = M.trie_node2;
+  const uint2 *node2 = warp_uniform(M.trie_node2);
+  const uint32_t *trie_val = warp_uniform(M.trie_val);
   const uint32_t root = __ldg(&node2[0]).x;
   const bool bf = M.flags & kFlagByteFallback;
-  const bool regular = M.flags & kFlagRegularScores;
+  const bool regular = warp_uniform(M.flags & kFlagRegularScores) != 0u;
+  const float max_score = __uint_as_float(warp_uniform(__float_as_uint(M.max_score)));
 
   uint32_t first = 0;
   while (lane_claim_group(B, lane, &first)) {
@@ -1034,7 +1055,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
     // ---------------- K2: flat state machine, one trie transition per trip (parked-lane schedule) ----------------
     // text window: words w0..w3 = bytes [4*aw, 4*aw+16), aw = s >> 2; ch = the byte at the walk position k and `cur`
     // streams the bytes after it (low byte first).
-    uint32_t s = 0, ss = ring_lo /* ring offset of s's slot */, k = 0, l = root, mblen = 1, nlog = 0, ch = 0;
+    uint32_t s = 0, ss = ring_lo /* ring offset of s's slot */, k = 0, l = root, mblen = 1, lg = log0, ch = 0;
     bool has_single = false, parked = false;  // the lane is done once s reaches n
     float base = 0.f;
     bool base_regular = regular;  // base == 0
@@ -1053,7 +1074,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
     if (n != 0) {
       for (uint32_t r = 0; r < R; ++r) ring_st_bp(ring_lo + r * kPlainRingSlot, 0u);  // all positions unset
       ring_st_score(ring_lo, 0.f);
-      w0 = slab_ld(c.text_w + 0, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
+      w0 = slab_ld(c.text_w, c.pol); w1 = slab_ld(c.text_w + 32, c.pol); w2 = slab_ld(c.text_w + 64, c.pol); w3 = slab_ld(c.text_w + 96, c.pol);
       mblen = one_char_len(w0 & 0xFFu);
       if (mblen > n) mblen = n;
       cur = window_low();
@@ -1078,28 +1099,27 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
           // position s leaves the window; only character starts are ever targets, so its
           // slot is the only one that has to be cleared for position s + R
           ring_st_bp(ss, 0u);
+          const uint32_t aw = s >> 2;
           s += mblen;
           ss = sl;
           // position s is final: append (plen | previous char length | unit) to the log
-          slab_st(c.log + static_cast<size_t>(nlog) * 32, ring_ld_bp(ss) | ((mblen - 1u) << 22), c.pol);
-          ++nlog;
-          if (s < n) {
-            base = ring_ld_score(ss);
-            base_regular = regular && score_regular(base);
-            // slide the text window so that it is anchored at s; prefetch the new tail word
-            if ((s >> 2) != ((s - mblen) >> 2)) {
-              w0 = w1; w1 = w2; w2 = w3;
-              w3 = slab_ld(c.text_w + static_cast<size_t>((s >> 2) + 3) * 32, c.pol);
-            }
-            cur = window_low();
-            ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
-            cur >>= 8;
-            mblen = one_char_len(ch);
-            if (mblen > n - s) mblen = n - s;
-            k = s;
-            l = root;
-            has_single = false;
-          }
+          slab_st(c.text_w + lg, ring_ld_bp(ss) | ((mblen - 1u) << 22), c.pol);
+          lg += 32;
+          // the next walk, from s (straight-line code, see encode_unigram_lane_kernel).  A character has at most four
+          // bytes, so the window moves by at most one word: the words shift down by selects and only the new tail
+          // word is loaded, by a predicated load.
+          base = ring_ld_score(ss);
+          base_regular = regular && score_regular(base);
+          const bool slide = (s >> 2) != aw;
+          w0 = slide ? w1 : w0; w1 = slide ? w2 : w1; w2 = slide ? w3 : w2;
+          if (slide) w3 = slab_ld(c.text_w + (s >> 2) * 32 + 96, c.pol);
+          cur = window_low();
+          ch = static_cast<uint32_t>(cur) & 0xFFu;  // the first byte of the new walk
+          cur >>= 8;
+          mblen = min(one_char_len(ch), n - s);
+          k = s;
+          l = root;
+          has_single = false;
           parked = false;
         }
         need = park_need(__popc(__ballot_sync(0xFFFFFFFFu, s < n)));
@@ -1126,15 +1146,15 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
               // |score|, |base| in {0} U [2^-10, 2^18) the double sum a + b is exact, so
               // (float)cand == fl(a + b) and cand > cur <=> ns > cur || (ns == cur && err > 0),
               // err being the exact rounding error of the float add (Knuth two-sum).
-              const float a = __uint_as_float(__ldg(M.trie_val + v));
+              const float a = __uint_as_float(__ldg(trie_val + v));
               ns = __fadd_rn(a, base);
               const float bb = __fsub_rn(ns, a);
               const float err = __fadd_rn(__fsub_rn(a, __fsub_rn(ns, bb)), __fsub_rn(base, bb));
               better = unset || ns > curs || (ns == curs && err > 0.f);
             } else {
               const double sc = kind == kKindNormal
-                                    ? static_cast<double>(__uint_as_float(__ldg(M.trie_val + v)))
-                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), M.max_score)) - 0.1;
+                                    ? static_cast<double>(__uint_as_float(__ldg(trie_val + v)))
+                                    : static_cast<double>(__fmul_rn(static_cast<float>(plen), max_score)) - 0.1;
               const double cand = sc + static_cast<double>(base);
               better = unset || cand > static_cast<double>(curs);
               ns = static_cast<float>(cand);
@@ -1150,7 +1170,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
           if (k < n) {
             const uint32_t d = k - s;
             if (d >= 13u) {  // beyond the register window: long piece, rare
-              ch = lane_text_byte(c, k);
+              ch = (slab_ld(c.text_w + (k >> 2) * 32, c.pol) >> ((k & 3u) * 8u)) & 0xFFu;
             } else {
               if (d == 8u) cur = window_high();
               ch = static_cast<uint32_t>(cur) & 0xFFu;
@@ -1162,7 +1182,7 @@ __global__ void __launch_bounds__(1024, 1) encode_unigram_lane_plain_kernel(cons
       }
     }
     clk.mark();
-    lane_finish(M, B, c, n, nlog, lane, have, defer, sent, bf);  // K4
+    lane_finish(M, B, c, n, (lg - log0) >> 5, lane, have, defer, sent, bf);  // K4
     clk.mark();
     lane_drain(B, sent, have, lane);  // K6 (fused host path only)
     __syncwarp();
