@@ -169,6 +169,26 @@ int spm_encode_ids_device(spm_engine *e, const char *d_bytes, const uint64_t *d_
                           uint64_t total_bytes, int32_t *d_ids, uint64_t ids_capacity,
                           uint64_t *d_id_offsets, uint64_t *total_ids, void *stream);
 
+/* The same batch as rows of one width, the layout a model consumes: an int32 [n, w] id tensor in row-major order.
+ * Row i holds F_i, sentence i's framed ids exactly as spm_encode_ids_device returns them, and pad_id (any int32,
+ * -1 included) in every other cell.  d_lengths[i] receives the number of real cells of row i.
+ *   width: 0 = the longest |F_i| of the batch; otherwise the fixed width w.
+ *   SPM_PAD_TRUNCATE: a row longer than a fixed width keeps its frame, prefix ++ body[:width - np - ns] ++ suffix,
+ *     where body is the framed list's middle part (already reversed under a reversing frame) and np / ns the frame's
+ *     prefix and suffix sizes; width < np + ns is SPM_ERR_ARG.  Without it, a row longer than a fixed width fails the
+ *     call with SPM_ERR_CAPACITY and the longest row length in *width_out.
+ *   SPM_PAD_LEFT: the real ids sit at the end of their row (left padding, as batched generation prompts want).
+ * Rows are written at stride w into d_out (capacity out_capacity int32); if n * w > out_capacity the call returns
+ * SPM_ERR_CAPACITY with *width_out = w.  In both capacity errors nothing is written to d_out or d_lengths; the batch
+ * has been encoded, and a retry with room enough encodes it again.  On success *width_out = w.
+ * Device pointers, stream, synchronisation and argument rules as spm_encode_ids_device; n == 0 writes nothing and sets
+ * *width_out = 0.  There is no offsets scan: one synchronisation reads the longest row back. */
+enum { SPM_PAD_TRUNCATE = 1, SPM_PAD_LEFT = 2 };
+int spm_encode_ids_device_padded(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                                 uint64_t total_bytes, int32_t *d_out, uint64_t out_capacity, uint32_t width,
+                                 int32_t pad_id, uint32_t flags, int32_t *d_lengths, uint32_t *width_out,
+                                 void *stream);
+
 /* ------------------------------------------------------------------------
  * N-best and sampling (unigram models; BASELINE.json config 5).
  *
@@ -268,6 +288,18 @@ int spm_sample_encode_and_score_pieces(spm_engine *e, const char *bytes, const u
  * decode_extra_options (a host-side reordering the caller applies to the id lists). */
 int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
                    const uint64_t **text_offsets);
+
+/* Decode of device-resident id rows, e.g. a generation output tensor [n, >= row_len] still on the GPU: row i starts at
+ * element i * row_stride of d_ids (int32 when id_bytes == 4, int64 when 8 -- a cast of int64 ids to int32 would wrap
+ * large values silently) and holds min(row_len, d_lengths[i]) ids (row_len when d_lengths is NULL; a negative length is
+ * 0), cut further just before its first stop_id when stop_id >= 0.  Cells after a row's end are never read or
+ * validated.  The text of a row is exactly spm_decode_ids of its id list, with the same errors ("Invalid id: N", where
+ * int64 ids outside the int32 range are invalid too) and the same outputs: engine-owned pinned text and
+ * text_offsets[n+1], valid until the next call on this engine.  Models with a denormalizer_spec charsmap:
+ * SPM_ERR_UNSUPPORTED.  `stream` as in spm_encode_ids_device; the call returns after the text has arrived. */
+int spm_decode_ids_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, uint64_t row_stride, size_t n,
+                          uint32_t row_len, const int32_t *d_lengths, int64_t stop_id, const char **text,
+                          const uint64_t **text_offsets, void *stream);
 
 /* TrainerSpec.unk_surface (src/sentencepiece_model.proto:228, read at sentencepiece_processor.cc:771-773) for
  * engines created from an spm_model_desc; engines created from a serialized ModelProto take it from the proto. */

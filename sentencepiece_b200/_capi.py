@@ -17,7 +17,12 @@ EXPORTS = [
     "spm_sample_encode_ids", "spm_decode_ids", "spm_engine_set_unk_surface", "spm_calculate_entropy",
     "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
     "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
+    "spm_encode_ids_device_padded", "spm_decode_ids_device",
 ]
+
+# spm_encode_ids_device_padded flags
+PAD_TRUNCATE, PAD_LEFT = 1, 2
+SPM_ERR_CAPACITY = 4
 
 
 class ModelDesc(ctypes.Structure):
@@ -68,6 +73,9 @@ def load():
     L.spm_encode_pieces.argtypes = [vp, vp, vp, sz, cp, sz, ctypes.c_int, P(vp), P(vp), P(vp), P(vp), P(vp)]
     L.spm_encode_ids_device.argtypes = [vp, vp, vp, sz, ctypes.c_uint64, vp, ctypes.c_uint64, vp,
                                         P(ctypes.c_uint64), vp]
+    u32, u64 = ctypes.c_uint32, ctypes.c_uint64
+    L.spm_encode_ids_device_padded.argtypes = [vp, vp, vp, sz, u64, vp, u64, u32, ctypes.c_int32, u32, vp, P(u32), vp]
+    L.spm_decode_ids_device.argtypes = [vp, vp, u32, u64, sz, u32, vp, ctypes.c_int64, P(vp), P(vp), vp]
     L.spm_host_alloc.argtypes = [sz]
     L.spm_host_alloc.restype = vp
     L.spm_host_free.argtypes = [vp]

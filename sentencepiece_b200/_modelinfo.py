@@ -14,7 +14,18 @@ def _varint(b, p):
 
 
 def pieces_and_unk(data):
-    pieces, unk, p, n = [], -1, 0, len(data)
+    pieces, types = pieces_and_types(data)
+    return pieces, _unk_id(types)
+
+
+def _unk_id(types):
+    """the last UNKNOWN piece, -1 when there is none"""
+    return max((i for i, t in enumerate(types) if t == 2), default=-1)
+
+
+def pieces_and_types(data):
+    """Piece strings and their types (ModelProto.SentencePiece.Type, NORMAL = 1 when absent)."""
+    pieces, types, p, n = [], [], 0, len(data)
     while p < n:
         key, p = _varint(data, p)
         fno, wt = key >> 3, key & 7
@@ -40,8 +51,7 @@ def pieces_and_unk(data):
                         q += 8
                     else:
                         raise ValueError("unsupported wire type in SentencePiece")
-                if typ == 2:  # UNKNOWN
-                    unk = len(pieces)
+                types.append(typ)
                 pieces.append(piece.decode("utf-8", errors="replace"))
             p += ln
         elif wt == 0:
@@ -52,7 +62,7 @@ def pieces_and_unk(data):
             p += 8
         else:
             raise ValueError("unsupported wire type in ModelProto")
-    return pieces, unk
+    return pieces, types
 
 
 def _fields(b, p, end):
@@ -78,14 +88,17 @@ def _fields(b, p, end):
 def special_pieces(data):
     """TrainerSpec unk_piece / bos_piece / eos_piece (sentencepiece_model.proto:220-222, field 2 of ModelProto) and
     their ids as the reference's bos_id() / eos_id() see them: PieceToId of the piece (the first definition wins,
-    model_interface.cc:51-61), -1 when that is the unknown id (the piece is not defined)."""
-    names = {45: "<unk>", 46: "<s>", 47: "</s>"}
+    model_interface.cc:51-61), -1 when that is the unknown id (the piece is not defined).  pad_piece (field 48) and
+    pad_id as the reference's pad_id() (sentencepiece_processor.cc:1011-1015): PieceToId of the piece when that is a
+    CONTROL piece, else -1."""
+    names = {45: "<unk>", 46: "<s>", 47: "</s>", 48: "<pad>"}
     for fno, wt, v in _fields(data, 0, len(data)):
         if fno == 2 and wt == 2:
             for f2, w2, v2 in _fields(v, 0, len(v)):
                 if f2 in names and w2 == 2:
                     names[f2] = v2.decode("utf-8", errors="replace")
-    pieces, unk = pieces_and_unk(data)
+    pieces, types = pieces_and_types(data)
+    unk = _unk_id(types)
     first = {}
     for i, p in enumerate(pieces):
         first.setdefault(p, i)
@@ -94,5 +107,7 @@ def special_pieces(data):
         i = first.get(p, unk)
         return -1 if i == unk else i
 
-    return dict(unk_piece=names[45], bos_piece=names[46], eos_piece=names[47],
-                bos_id=piece_id(names[46]), eos_id=piece_id(names[47]))
+    pad = piece_id(names[48])
+    return dict(unk_piece=names[45], bos_piece=names[46], eos_piece=names[47], pad_piece=names[48],
+                bos_id=piece_id(names[46]), eos_id=piece_id(names[47]),
+                pad_id=pad if pad >= 0 and types[pad] == 3 else -1)  # 3 = CONTROL

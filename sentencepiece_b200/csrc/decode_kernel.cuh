@@ -47,6 +47,10 @@ struct KDecode {
   unsigned long long *sent_start;  // [n]
   uint32_t *sent_count;            // [n]
   uint32_t *status;                // [1] error: 2 = id out of range, 1 = malformed byte piece; [2] overflow; [3] the offending id
+  // ROWS mode (decode_warp_kernel<IdT, true>): list i is ids[i * row_stride ..] of row_len[i] ids, and an id out of
+  // range is also stored whole, sign-extended, at cursor[1]
+  unsigned long long row_stride;
+  const uint32_t *row_len;  // [n]
 };
 
 // IsValidDecodeUTF8 (src/util.h:173-176 over DecodeUTF8, src/util.cc:51-84): bytes consumed by one valid character
@@ -70,14 +74,16 @@ __device__ __forceinline__ uint32_t dec_utf8_valid(const uint32_t *b, uint32_t a
   return 0;
 }
 
-// Sequential restatement for one list (lists with BYTE pieces); WRITE = false only counts.
-template <bool WRITE>
+// Sequential restatement for one list (lists with BYTE pieces); WRITE = false only counts.  IdT: the ids' type (every
+// id has been checked to lie in [0, vocab) before).
+template <bool WRITE, typename IdT = int32_t>
 __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, unsigned long long a, uint32_t L, uint8_t *out) {
+  const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   uint32_t n = 0;  // bytes of text so far
   bool is_bos_ws = true, bos_ws_seen = false;
   uint32_t i = 0;
   while (i < L) {
-    const int32_t id = D.ids[a + i];
+    const int32_t id = static_cast<int32_t>(ids[a + i]);
     const uint32_t info = __ldg(D.dec_info + id);
     const uint32_t kind = info & kDecKindMask;
     if (kind == kDecKindByte) {
@@ -85,7 +91,7 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
       uint32_t b[4] = {info >> kDecByteShift, 0, 0, 0};
       uint32_t avail = 1;
       while (avail < 4 && i + avail < L) {
-        const uint32_t inf2 = __ldg(D.dec_info + D.ids[a + i + avail]);
+        const uint32_t inf2 = __ldg(D.dec_info + static_cast<int32_t>(ids[a + i + avail]));
         if ((inf2 & kDecKindMask) != kDecKindByte) break;
         b[avail] = inf2 >> kDecByteShift;
         ++avail;
@@ -120,12 +126,24 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
   return n;
 }
 
+// IdT, ROWS: the ids are int32 or int64, and list i is either [id_offsets[i], id_offsets[i+1]) (packed) or row_len[i]
+// ids from i * row_stride (rows of a padded [n, row_stride] tensor).  Template flags, so that the packed int32
+// instantiation keeps its code.
+template <typename IdT = int32_t, bool ROWS = false>
 __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
+  static_assert(ROWS || sizeof(IdT) == 4, "packed lists are int32");
+  const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t sent = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; sent < D.n; sent += warps) {
-    const unsigned long long a = D.id_offsets[sent];
-    const unsigned long long len64 = D.id_offsets[sent + 1] - a;
+    unsigned long long a, len64;
+    if constexpr (ROWS) {
+      a = static_cast<unsigned long long>(sent) * D.row_stride;
+      len64 = D.row_len[sent];
+    } else {
+      a = D.id_offsets[sent];
+      len64 = D.id_offsets[sent + 1] - a;
+    }
     const uint32_t L = static_cast<uint32_t>(len64);
     // ---- pass 0: ids in range, any BYTE piece ----
     uint32_t err = len64 > 0x7FFFFFFFull ? 2u : 0u;  // 2 = id out of range (checked first by the reference), 1 = malformed byte piece
@@ -134,9 +152,12 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
     for (uint32_t base = 0; base < L && !stop; base += 32) {
       const uint32_t t = base + lane;
       if (t < L) {
-        const int32_t id = D.ids[a + t];
-        if (id < 0 || id >= D.vocab) { err = 2; err_id = id; }
-        else {
+        const IdT id = ids[a + t];
+        if (id < 0 || id >= D.vocab) {
+          err = 2;
+          err_id = static_cast<int32_t>(id);
+          if constexpr (ROWS) atomicExch(D.cursor + 1, static_cast<unsigned long long>(static_cast<long long>(id)));
+        } else {
           const uint32_t info = __ldg(D.dec_info + id);
           has_byte |= (info & kDecKindMask) == kDecKindByte;
           if ((info & kDecBadByte) && !err) { err = 1; err_id = id; }
@@ -158,10 +179,10 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
     if (has_byte) {
       // ---- sequential path on lane 0 ----
       if (lane == 0) {
-        total = decode_list_sequential<false>(D, a, L, nullptr);
+        total = decode_list_sequential<false, IdT>(D, a, L, nullptr);
         pos = atomicAdd(D.cursor, static_cast<unsigned long long>(total));
         if (pos + total > D.tmp_cap) { atomicOr(D.status + 2, 1u); total = 0; }
-        else decode_list_sequential<true>(D, a, L, D.tmp + pos);
+        else decode_list_sequential<true, IdT>(D, a, L, D.tmp + pos);
         D.sent_start[sent] = pos;
         D.sent_count[sent] = total;
       }
@@ -177,7 +198,7 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
         const bool valid = t < L;
         uint32_t info = kDecKindControl, off = 0, n0 = 0;
         if (valid) {
-          const int32_t id = D.ids[a + t];
+          const int32_t id = static_cast<int32_t>(ids[a + t]);
           info = __ldg(D.dec_info + id);
           off = __ldg(D.dec_off + id);
           n0 = __ldg(D.dec_off + id + 1) - off;
@@ -220,6 +241,33 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
         if (pos + total > D.tmp_cap) break;
       }
     }
+  }
+}
+
+// Row ends of a padded id tensor for decode_warp_kernel<IdT, true>, one warp per row: row i holds
+// min(row_len, lengths[i]) ids (row_len when lengths is null; a negative length is 0), cut before its first stop_id
+// when stop_id >= 0.  Ids past a row's end are never read.
+template <typename IdT>
+__global__ void __launch_bounds__(256) decode_row_len_kernel(const IdT *ids, unsigned long long row_stride, uint32_t n,
+                                                             uint32_t row_len, const int32_t *lengths, long long stop_id,
+                                                             uint32_t *len_out) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < n; row += warps) {
+    uint32_t L = row_len;
+    if (lengths) L = min(L, static_cast<uint32_t>(max(lengths[row], 0)));
+    if (stop_id >= 0) {
+      const IdT *r = ids + static_cast<unsigned long long>(row) * row_stride;
+      for (uint32_t base = 0; base < L; base += 32) {
+        const uint32_t t = base + lane;
+        const uint32_t hit = __ballot_sync(0xFFFFFFFFu, t < L && static_cast<long long>(r[t]) == stop_id);
+        if (hit) {
+          L = base + __ffs(hit) - 1u;
+          break;
+        }
+      }
+    }
+    if (lane == 0) len_out[row] = L;
   }
 }
 

@@ -36,6 +36,7 @@
 #include "model_reader.h"
 #include "order_kernel.cuh"
 #include "decode_kernel.cuh"
+#include "padded_kernel.cuh"
 #include "pieces_kernel.cuh"
 #include "nbest_kernel.cuh"
 #include "lattice_kernel.cuh"
@@ -380,10 +381,12 @@ struct spm_engine {
     D.status = d_ctrl32.p;
     return D;
   }
-  // the error behind decode_warp_kernel's status word in h_ctrl32, or SPM_OK
-  int decode_error() const {
+  // the error behind decode_warp_kernel's status word in h_ctrl32, or SPM_OK; rows: the ROWS mode, which keeps the
+  // offending id whole in h_ctrl64[1]
+  int decode_error(bool rows = false) const {
     if (h_ctrl32.p[1] == 2u) {  // :915-918
-      set_error("Invalid id: " + std::to_string(static_cast<int32_t>(h_ctrl32.p[3])));
+      set_error("Invalid id: " + (rows ? std::to_string(static_cast<long long>(h_ctrl64.p[1]))
+                                       : std::to_string(static_cast<int32_t>(h_ctrl32.p[3]))));
       return SPM_ERR_ARG;
     }
     if (h_ctrl32.p[1] == 1u) {
@@ -399,6 +402,50 @@ struct spm_engine {
   PinBuf<uint8_t> h_stage[2];
   int decode_host_pipelined(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
                             const uint64_t **text_offsets);
+  DevBuf<uint32_t> d_row_len;  // spm_decode_ids_device: the length of every row
+  // The decode of n lists on st after the caller's checks: launch(tmp_cap) queues decode_warp_kernel, which is run again
+  // with the exact temporary size if it overflowed; then the text is put into list order and copied into the pinned
+  // results, and the call waits for it.  rows: launch runs the ROWS mode (for decode_error).
+  template <typename Launch>
+  int decode_text(uint32_t n, unsigned long long tmp_cap, bool rows, cudaStream_t st, Launch &&launch, const char **text,
+                  const uint64_t **text_offsets) {
+    CUDA_TRY(d_sent_start.ensure(n));
+    CUDA_TRY(d_sent_count.ensure(n));
+    CUDA_TRY(d_dec_text_offsets.ensure(n + 1));
+    CUDA_TRY(h_dec_text_offsets.ensure(n + 1));
+    unsigned long long tot = 0;
+    for (int attempt = 0; attempt < 3; ++attempt) {
+      CUDA_TRY(d_dec_tmp.ensure(tmp_cap));
+      CUDA_TRY(cudaMemsetAsync(d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
+      CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 8 * sizeof(unsigned long long), st));
+      CUDA_TRY(cudaEventRecord(ev[0], st));
+      launch(tmp_cap);
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(cudaEventRecord(ev[1], st));
+      ++last_launches;
+      SPM_TRY(read_status(st, 16, 8));
+      SPM_TRY(decode_error(rows));
+      tot = h_ctrl64.p[0];
+      if (h_ctrl32.p[2]) { tmp_cap = tot + 1024; continue; }
+      break;
+    }
+    if (h_ctrl32.p[2]) { set_error("Decode: temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
+    // offsets (exclusive scan) + gather into list order: the kernels of the encode path
+    CUDA_TRY(d_dec_text.ensure(tot + 16));
+    SPM_TRY(scan_total(d_sent_count.p, n, 0, d_ctrl64.p + 2, st));
+    SPM_TRY(scan_gather<uint8_t>(d_sent_count.p, n, d_dec_text_offsets.p, d_sent_start.p, d_dec_tmp.p, d_dec_text.p,
+                                 d_dec_text.cap, 0, 0ull, st));
+    CUDA_TRY(cudaEventRecord(ev[2], st));
+    CUDA_TRY(h_dec_text.ensure(tot + 1));
+    if (tot) CUDA_TRY(cudaMemcpyAsync(h_dec_text.p, d_dec_text.p, tot, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_dec_text_offsets.p, d_dec_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    last_d2h = tot + (n + 1) * sizeof(uint64_t);
+    h_dec_text.p[tot] = 0;
+    *text = h_dec_text.p;
+    *text_offsets = h_dec_text_offsets.p;
+    return SPM_OK;
+  }
   // EncodeAsPieces (K9): per-id piece bytes, built on first use; the raw ids of the lane kernels, the unknown-surface
   // subset and its spans run, the packed pieces
   DevBuf<uint32_t> d_pc_off, d_pc_flag, d_pc_sub_of, d_pc_sub_len, d_pc_text_len, d_pc_ntok, d_pc_end;
@@ -589,6 +636,11 @@ struct spm_engine {
   int upload_types();
   int upload_node2();
   int configure_kernel_attrs();
+  // The encode stage of run_device: the encode kernels (lane, second-chance and long-sentence) leave sentence i's raw
+  // ids at d_tmp_ids + d_sent_start[i], d_sent_count[i] of them (with spans, also the token ends and the normalized
+  // text); its writers follow: run_device's packed one, the padded one of spm_encode_ids_device_padded.
+  int encode_stage(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes, bool spans,
+                   cudaStream_t st);
   int run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes, bool spans,
                  int32_t *user_ids, uint64_t user_ids_cap, unsigned long long *user_id_offsets, uint64_t *total_ids,
                  uint64_t *total_norm, cudaStream_t st, DevBuf<int32_t> *out_ids = nullptr,
@@ -1127,12 +1179,8 @@ int spm_engine::build_order(const uint64_t *d_offs, size_t n, cudaStream_t st, c
   return SPM_OK;
 }
 
-// Encodes a device-resident batch.  Outputs: ids (+offsets) either into the
-// engine's buffers (user_ids == nullptr) or the caller's.
-int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes,
-                           bool spans, int32_t *user_ids, uint64_t user_ids_cap, unsigned long long *user_id_offsets,
-                           uint64_t *total_ids, uint64_t *total_norm, cudaStream_t st, DevBuf<int32_t> *out_ids,
-                           DevBuf<unsigned long long> *out_offs, unsigned long long off_base) {
+int spm_engine::encode_stage(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes,
+                             bool spans, cudaStream_t st) {
   last_launches = 0;
   last_deferred = 0;
   const uint32_t n32 = static_cast<uint32_t>(n);
@@ -1341,6 +1389,17 @@ int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, 
     break;
   }
   if (h_ctrl32.p[2]) { set_error("temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
+  return SPM_OK;
+}
+
+// Encodes a device-resident batch.  Outputs: ids (+offsets) either into the
+// engine's buffers (user_ids == nullptr) or the caller's.
+int spm_engine::run_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes,
+                           bool spans, int32_t *user_ids, uint64_t user_ids_cap, unsigned long long *user_id_offsets,
+                           uint64_t *total_ids, uint64_t *total_norm, cudaStream_t st, DevBuf<int32_t> *out_ids,
+                           DevBuf<unsigned long long> *out_offs, unsigned long long off_base) {
+  SPM_TRY(encode_stage(d_bytes_base, d_offs, n, total_bytes, spans, st));
+  const uint32_t n32 = static_cast<uint32_t>(n);
   // ---- offsets (exclusive scan) + compaction into sentence order; ids (not spans) get the encode frame ----
   const bool framed_ids = !spans && framed();
   SPM_TRY(scan_total(d_sent_count.p, n32, framed_ids ? frame_np + frame_ns : 0u, d_ctrl64.p + 2, st));
@@ -2600,47 +2659,70 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
   }
   CUDA_TRY(e->d_dec_ids.ensure(total_ids + 1));
   CUDA_TRY(e->d_offsets.ensure(n + 1));
-  CUDA_TRY(e->d_sent_start.ensure(n));
-  CUDA_TRY(e->d_sent_count.ensure(n));
-  CUDA_TRY(e->d_dec_text_offsets.ensure(n + 1));
   if (total_ids) CUDA_TRY(cudaMemcpyAsync(e->d_dec_ids.p, ids + base, total_ids * sizeof(int32_t), cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(e->d_offsets.p, id_offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
   e->last_h2d = total_ids * sizeof(int32_t) + (n + 1) * sizeof(uint64_t);
   const uint32_t n32 = static_cast<uint32_t>(n);
-  unsigned long long tmp_cap = total_ids * 6 + 16ull * n + (1u << 20);  // retried with the exact size on overflow
-  unsigned long long tot = 0;
-  for (int attempt = 0; attempt < 3; ++attempt) {
-    CUDA_TRY(e->d_dec_tmp.ensure(tmp_cap));
-    CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, 16 * sizeof(uint32_t), st));
-    CUDA_TRY(cudaMemsetAsync(e->d_ctrl64.p, 0, 8 * sizeof(unsigned long long), st));
-    CUDA_TRY(cudaEventRecord(e->ev[0], st));
-    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
-    decode_warp_kernel<<<grid, 256, 0, st>>>(e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap));
-    CUDA_TRY(cudaGetLastError());
-    CUDA_TRY(cudaEventRecord(e->ev[1], st));
-    ++e->last_launches;
-    SPM_TRY(e->read_status(st, 16, 8));
-    SPM_TRY(e->decode_error());
-    tot = e->h_ctrl64.p[0];
-    if (e->h_ctrl32.p[2]) { tmp_cap = tot + 1024; continue; }
-    break;
-  }
-  if (e->h_ctrl32.p[2]) { set_error("Decode: temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
-  // offsets (exclusive scan) + gather into list order: the kernels of the encode path
-  CUDA_TRY(e->d_dec_text.ensure(tot + 16));
-  SPM_TRY(e->scan_total(e->d_sent_count.p, n32, 0, e->d_ctrl64.p + 2, st));
-  SPM_TRY(e->scan_gather<uint8_t>(e->d_sent_count.p, n32, e->d_dec_text_offsets.p, e->d_sent_start.p, e->d_dec_tmp.p,
-                                  e->d_dec_text.p, e->d_dec_text.cap, 0, 0ull, st));
-  CUDA_TRY(cudaEventRecord(e->ev[2], st));
-  CUDA_TRY(e->h_dec_text.ensure(tot + 1));
-  if (tot) CUDA_TRY(cudaMemcpyAsync(e->h_dec_text.p, e->d_dec_text.p, tot, cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaMemcpyAsync(e->h_dec_text_offsets.p, e->d_dec_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  e->last_d2h = tot + (n + 1) * sizeof(uint64_t);
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  SPM_TRY(e->decode_text(n32, total_ids * 6 + 16ull * n + (1u << 20), false, st,  // retried with the exact size on overflow
+                         [&](unsigned long long tmp_cap) {
+                           decode_warp_kernel<<<grid, 256, 0, st>>>(
+                               e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap));
+                         },
+                         text, text_offsets));
   finish_timing(e);
-  e->h_dec_text.p[tot] = 0;
-  *text = e->h_dec_text.p;
-  *text_offsets = e->h_dec_text_offsets.p;
+  return SPM_OK;
+}
+
+int spm_decode_ids_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, uint64_t row_stride, size_t n,
+                          uint32_t row_len, const int32_t *d_lengths, int64_t stop_id, const char **text,
+                          const uint64_t **text_offsets, void *stream) {
+  if (!e || !text || !text_offsets) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (id_bytes != 4 && id_bytes != 8) { e->set_error("id_bytes must be 4 or 8"); return SPM_ERR_ARG; }
+  if (n && row_len && !d_ids) { e->set_error("null argument"); return SPM_ERR_ARG; }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many rows in one call"); return SPM_ERR_ARG; }
+  if (!e->model.denormalizer_charsmap.empty()) {
+    e->set_error("Decode: models with a denormalizer_spec are not on the device path");
+    return SPM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  { const int rc = e->ensure_decode_tables(); if (rc) return rc; }
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  e->last_launches = 0;
+  e->last_h2d = e->last_d2h = 0;
+  if (n == 0) {
+    CUDA_TRY(e->h_dec_text.ensure(1));
+    CUDA_TRY(e->h_dec_text_offsets.ensure(1));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    e->h_dec_text_offsets.p[0] = 0;
+    *text = e->h_dec_text.p;
+    *text_offsets = e->h_dec_text_offsets.p;
+    return SPM_OK;
+  }
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  CUDA_TRY(e->d_row_len.ensure(n));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  const bool wide = id_bytes == 8;
+  if (wide) decode_row_len_kernel<<<grid, 256, 0, st>>>(static_cast<const int64_t *>(d_ids), row_stride, n32, row_len,
+                                                         d_lengths, stop_id, e->d_row_len.p);
+  else decode_row_len_kernel<<<grid, 256, 0, st>>>(static_cast<const int32_t *>(d_ids), row_stride, n32, row_len,
+                                                    d_lengths, stop_id, e->d_row_len.p);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  // about 6 text bytes per id; the kernel reports the exact size when a batch needs more
+  const unsigned long long guess = 6ull * n * std::min<uint32_t>(row_len, 256u) + 16ull * n + (1u << 20);
+  SPM_TRY(e->decode_text(n32, guess, true, st,
+                         [&](unsigned long long tmp_cap) {
+                           KDecode D = e->decode_args(static_cast<const int32_t *>(d_ids), nullptr, n32, tmp_cap);
+                           D.row_stride = row_stride;
+                           D.row_len = e->d_row_len.p;
+                           if (wide) decode_warp_kernel<int64_t, true><<<grid, 256, 0, st>>>(D);
+                           else decode_warp_kernel<int32_t, true><<<grid, 256, 0, st>>>(D);
+                         },
+                         text, text_offsets));
+  finish_timing(e);
   return SPM_OK;
 }
 
@@ -2732,6 +2814,72 @@ int spm_encode_ids_device(spm_engine *e, const char *d_bytes, const uint64_t *d_
   const int rc = e->run_device(reinterpret_cast<const uint8_t *>(d_bytes), d_offsets, n, total_bytes, false, d_ids,
                                ids_capacity, reinterpret_cast<unsigned long long *>(d_id_offsets), total_ids, nullptr, st);
   if (rc) return rc;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  finish_timing(e);
+  return SPM_OK;
+}
+
+int spm_encode_ids_device_padded(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                                 uint64_t total_bytes, int32_t *d_out, uint64_t out_capacity, uint32_t width,
+                                 int32_t pad_id, uint32_t flags, int32_t *d_lengths, uint32_t *width_out,
+                                 void *stream) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!d_offsets || !width_out || (n && (!d_out || !d_lengths)) || (n && !d_bytes && total_bytes)) {
+    e->set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  if (flags & ~static_cast<uint32_t>(SPM_PAD_TRUNCATE | SPM_PAD_LEFT)) { e->set_error("unknown flags"); return SPM_ERR_ARG; }
+  const bool truncate = flags & SPM_PAD_TRUNCATE;
+  const uint32_t frame = e->frame_np + e->frame_ns;
+  if (truncate && width && width < frame) {
+    e->set_error("width " + std::to_string(width) + " is shorter than the encode frame (" + std::to_string(frame) + " ids)");
+    return SPM_ERR_ARG;
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  *width_out = 0;
+  if (n == 0) {
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SPM_OK;
+  }
+  e->last_h2d = e->last_d2h = 0;
+  if (e->model.model_type == SPM_UNIGRAM) {
+    const int rc0 = e->pick_fast_words_device(reinterpret_cast<const uint8_t *>(d_bytes), d_offsets, n, st, &e->batch_fast_words);
+    if (rc0) return rc0;
+  }
+  SPM_TRY(e->encode_stage(reinterpret_cast<const uint8_t *>(d_bytes), d_offsets, n, total_bytes, false, st));
+  // ---- the longest framed row decides the width, or whether the call fails ----
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  CUDA_TRY(cudaMemsetAsync(e->d_ctrl64.p + 2, 0, sizeof(unsigned long long), st));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256));
+  row_max_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, frame, e->d_ctrl64.p + 2);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  SPM_TRY(e->read_status(st, 0, 4));
+  const unsigned long long longest = e->h_ctrl64.p[2];
+  if (longest > 0xFFFFFFFFull) { e->set_error("a row is longer than 2^32 - 1 ids"); return SPM_ERR_UNSUPPORTED; }
+  if (width && !truncate && longest > width) {
+    *width_out = static_cast<uint32_t>(longest);
+    e->set_error("a row of " + std::to_string(longest) + " ids does not fit width " + std::to_string(width));
+    return SPM_ERR_CAPACITY;
+  }
+  const uint32_t w = width ? width : static_cast<uint32_t>(longest);
+  *width_out = w;
+  if (static_cast<unsigned long long>(n) * w > out_capacity) {
+    e->set_error("out_capacity too small: need " + std::to_string(static_cast<unsigned long long>(n) * w));
+    return SPM_ERR_CAPACITY;
+  }
+  // ---- the padded writer: one warp per row ----
+  const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  write_padded_kernel<<<wgrid, 256, 0, st>>>(e->d_sent_count.p, e->d_sent_start.p, e->d_tmp_ids.p, n32, e->kframe(), w,
+                                             pad_id, truncate ? 1u : 0u, (flags & SPM_PAD_LEFT) ? 1u : 0u, d_out,
+                                             d_lengths);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(cudaStreamSynchronize(st));
   finish_timing(e);
   return SPM_OK;

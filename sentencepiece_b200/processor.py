@@ -62,6 +62,10 @@ class Engine:
         if rc:
             raise RuntimeError(f"spm_engine_create failed ({rc}): {self._lib.spm_last_error(None).decode()}")
         self._h = h
+        self.device = device
+        self._model_bytes = model_bytes
+        self._pad_guess = 64  # cells per row encode_device_padded(width=0) allocates first: the last such call's width
+        self._pad = None  # pad_id(), read from the model on first use
 
     def close(self):
         if getattr(self, "_h", None):
@@ -297,6 +301,91 @@ class Engine:
         return tot.value
 
 
+    # ---- torch CUDA tensors on this engine's device, on torch's current stream ----
+    def _stream(self, *tensors):
+        import torch
+        for t in tensors:
+            if t is not None and (not t.is_cuda or t.device.index != self.device):
+                raise ValueError(f"tensors must live on cuda:{self.device}, the engine's device (got {t.device})")
+        return torch.cuda.current_stream(self.device).cuda_stream
+
+    def pad_id(self):
+        """The reference's pad_id(): the id of trainer_spec.pad_piece when that is a CONTROL piece, else -1."""
+        if self._pad is None:  # (parsing the ModelProto takes tens of milliseconds: once per engine)
+            from . import _modelinfo
+            self._pad = _modelinfo.special_pieces(self._model_bytes)["pad_id"]
+        return self._pad
+
+    def encode_device_padded(self, d_bytes, d_offsets, width=0, pad_id=None, truncate=False, pad_left=False, out=None):
+        """spm_encode_ids_device_padded: a batch already on the GPU (d_bytes uint8 [total], d_offsets int64 or uint64
+        [n+1], byte offsets into d_bytes) -> (ids int32 [n, w], lengths int32 [n]).  Row i is sentence i's ids under the
+        encode frame, then pad_id (None = the model's pad_id(); a model without a pad piece needs an explicit one);
+        pad_left puts the ids at the end of their rows.  width = 0: w is the longest row; a fixed width fails on a
+        longer row (ValueError) unless truncate, which keeps the frame and cuts the body.
+        Without `out`, the ids go to n * guess new cells, guess being the width of this engine's previous width = 0 call
+        (64 at first); when the longest row is wider, the call is repeated into n * w cells, which encodes the batch a
+        second time.  out: a contiguous int32 tensor whose first n * w cells take the rows (ValueError when too small).
+        The result is a [n, w] view of the cells."""
+        import torch
+        if pad_id is None:
+            pad_id = self.pad_id()
+            if pad_id < 0:
+                raise ValueError("the model defines no pad piece (trainer_spec.pad_piece): pass pad_id explicitly")
+        st = self._stream(d_bytes, d_offsets, out)
+        if d_bytes.dtype != torch.uint8 or d_bytes.dim() != 1 or not d_bytes.is_contiguous():
+            raise ValueError("d_bytes must be a contiguous 1-D uint8 tensor")
+        if d_offsets.dtype not in (torch.int64, torch.uint64) or d_offsets.dim() != 1 or not d_offsets.is_contiguous():
+            raise ValueError("d_offsets must be a contiguous 1-D int64 or uint64 tensor of n + 1 offsets")
+        if out is not None and (out.dtype != torch.int32 or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int32 tensor")
+        n = d_offsets.numel() - 1
+        flags = (_capi.PAD_TRUNCATE if truncate else 0) | (_capi.PAD_LEFT if pad_left else 0)
+        lengths = torch.empty(n, dtype=torch.int32, device=d_bytes.device)
+
+        def call(cells):
+            w = ctypes.c_uint32()
+            rc = self._lib.spm_encode_ids_device_padded(self._h, d_bytes.data_ptr(), d_offsets.data_ptr(), n,
+                                                        d_bytes.numel(), cells.data_ptr(), cells.numel(), width, pad_id,
+                                                        flags, lengths.data_ptr(), ctypes.byref(w), st)
+            return rc, w.value
+
+        cells = out if out is not None else torch.empty(n * (width or self._pad_guess), dtype=torch.int32,
+                                                        device=d_bytes.device)
+        rc, w = call(cells)
+        too_long = width and not truncate and w > width
+        if rc == _capi.SPM_ERR_CAPACITY and out is None and not too_long:
+            cells = torch.empty(n * w, dtype=torch.int32, device=d_bytes.device)
+            rc, w = call(cells)
+        if rc == _capi.SPM_ERR_CAPACITY:
+            raise ValueError(self._lib.spm_last_error(self._h).decode())
+        self._check(rc)
+        if not width and n:
+            self._pad_guess = max(w, 1)  # (an all-empty batch gives 0, and zero cells have no device pointer)
+        return cells.view(-1)[:n * w].view(n, w), lengths
+
+    def decode_device(self, ids2d, lengths=None, stop_id=-1):
+        """spm_decode_ids_device: the rows of an int32 or int64 [n, L] CUDA tensor (any row stride, e.g. a column slice;
+        each row contiguous) -> list of n str.  Row i holds min(L, lengths[i]) ids (lengths: int32 [n], or None for L),
+        cut before its first stop_id when stop_id >= 0; its text is DecodeIds of that list."""
+        import torch
+        if ids2d.dim() != 2 or ids2d.dtype not in (torch.int32, torch.int64):
+            raise ValueError("ids2d must be a 2-D int32 or int64 tensor")
+        n, L = ids2d.shape
+        if L > 1 and ids2d.stride(1) != 1:
+            raise ValueError("the ids of a row must be contiguous")
+        if lengths is not None and (lengths.dtype != torch.int32 or lengths.shape != (n,) or not lengths.is_contiguous()):
+            raise ValueError("lengths must be a contiguous int32 tensor of n entries")
+        st = self._stream(ids2d, lengths)
+        text = ctypes.c_void_p()
+        to = ctypes.c_void_p()
+        self._check(self._lib.spm_decode_ids_device(self._h, ids2d.data_ptr(), ids2d.element_size(), ids2d.stride(0), n,
+                                                    L, lengths.data_ptr() if lengths is not None else None, stop_id,
+                                                    ctypes.byref(text), ctypes.byref(to), st))
+        o = np.ctypeslib.as_array(ctypes.cast(to, ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).tolist()
+        raw = np.ctypeslib.as_array(ctypes.cast(text, ctypes.POINTER(ctypes.c_uint8)), (max(o[n], 1),))[:o[n]].tobytes()
+        return [raw[o[i]:o[i + 1]].decode("utf-8", errors="replace") for i in range(n)]
+
+
 class SentencePieceProcessor:
     """Mirror of the reference's encode API (same method names / argument meaning as
     python/src/sentencepiece/__init__.py and src/sentencepiece_processor.h for this path)."""
@@ -492,6 +581,34 @@ class SentencePieceProcessor:
 
     def SampleEncodeAndScoreAsPieces(self, input, num_samples=-1, alpha=0.1, wor=False, include_best=False, **kw):
         return self.SampleEncodeAndScore(input, str, num_samples, alpha, wor, include_best, **kw)
+
+    # ---- padded id tensors on the device (no reference counterpart): a model's [batch, seq_len] input, and the text
+    #      of a [batch, T] generation output ----
+    def encode_padded(self, input, max_len=None, pad_id=None, truncate=False, pad_left=False, add_bos=False,
+                      add_eos=False, reverse=False):
+        """EncodeAsIds of a batch as padded rows on the GPU -> (ids int32 [n, w], lengths int32 [n]) on the engine's
+        device.  input: a list of str / bytes (packed and uploaded through pinned memory) or a (bytes, offsets) pair of
+        CUDA tensors as Engine.encode_device_padded takes them.  max_len = None: w is the longest row; otherwise rows
+        longer than max_len fail (ValueError) unless truncate, which keeps bos / eos and cuts the ids between them.
+        pad_id = None: the model's pad_id(), and ValueError when it has none."""
+        self._require()
+        if isinstance(input, tuple):
+            d_bytes, d_offs = input
+        else:
+            import torch
+            buf, offs = pack_sentences(input)
+            dev = torch.device("cuda", self._engine.device)
+            d_bytes = torch.from_numpy(np.require(buf, requirements="W")).pin_memory().to(dev, non_blocking=True)
+            d_offs = torch.from_numpy(offs.view(np.int64)).pin_memory().to(dev, non_blocking=True)
+        self._set_frame(add_bos, add_eos, reverse)
+        return self._engine.encode_device_padded(d_bytes, d_offs, width=max_len or 0, pad_id=pad_id, truncate=truncate,
+                                                 pad_left=pad_left)
+
+    def decode_padded(self, ids, lengths=None, stop_id=None):
+        """DecodeIds of every row of an int32 / int64 [n, L] CUDA tensor -> list of n str: row i holds lengths[i] ids
+        (all L when lengths is None), cut before its first stop_id (e.g. eos_id()) when one is given."""
+        self._require()
+        return self._engine.decode_device(ids, lengths, -1 if stop_id is None else stop_id)
 
     # sentencepiece_processor.h:521-526
     def CalculateEntropy(self, input, alpha):
