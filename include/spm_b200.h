@@ -137,6 +137,24 @@ int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, 
                      const int32_t **ids, const uint32_t **tok_end, const uint64_t **id_offsets,
                      const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o);
 
+/* The n2o entry of a sentence whose reference norm_to_orig is empty: its input is empty (src/normalizer.cc:77-79), or
+ * remove_extra_whitespaces drops all of it as heading whitespace (:97-100).  A sentence that normalizes to nothing
+ * otherwise gets {consumed}, as the reference does. */
+#define SPM_NORM_TO_ORIG_EMPTY 0xFFFFFFFFu
+
+/* Replaces SentencePieceProcessor::Normalize (src/sentencepiece_processor.cc:933-950, all three overloads) and
+ * Normalizer::Normalize (src/normalizer.cc:71-186) for n sentences: the model's own normalizer, with the prefix matcher
+ * of its USER_DEFINED pieces (those stay verbatim, normalizer.cc:201-205), for unigram and BPE models alike.  The
+ * encode frame does not apply.  Inputs as spm_encode_ids.
+ * out (engine-owned pinned memory, valid until the next call): normalized[norm_offsets[i] .. norm_offsets[i+1]) is
+ *   sentence i's text, U+2581 as its three bytes; with_offsets != 0: n2o holds its norm_to_orig,
+ *   norm_offsets[i+1]-norm_offsets[i]+1 entries stored at n2o[norm_offsets[i] + i ...] (the spm_encode_spans layout),
+ *   the one entry SPM_NORM_TO_ORIG_EMPTY where the reference's norm_to_orig is empty; with_offsets == 0: *n2o = NULL
+ *   (n2o itself may then be NULL).
+ * Argument errors and "sentence too long" as spm_encode_ids; n == 0 succeeds with norm_offsets = {0}. */
+int spm_normalize(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int with_offsets,
+                  const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o);
+
 /* Replaces the per-sentence loop over SentencePieceProcessor::Encode(absl::string_view, std::vector<std::string>*)
  * (src/sentencepiece_processor.cc:379-390 -> :547-636) for n sentences, with the encode frame
  * (spm_engine_set_encode_frame) applied to pieces and ids alike.  The piece of a token is IdToPiece(id), except for

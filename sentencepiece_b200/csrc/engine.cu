@@ -39,6 +39,7 @@
 #include "padded_kernel.cuh"
 #include "pieces_kernel.cuh"
 #include "nbest_kernel.cuh"
+#include "normalize_kernel.cuh"
 #include "lattice_kernel.cuh"
 #include "trie_builder.h"
 
@@ -3164,6 +3165,144 @@ int spm_encode_spans(spm_engine *e, const char *bytes, const uint64_t *offsets, 
   if (!e || !tok_end || !normalized || !norm_offsets || !n2o) return SPM_ERR_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_host_locked(e, bytes, offsets, n, true, ids, tok_end, id_offsets, normalized, norm_offsets, n2o);
+}
+
+// Slab elements per chunk of spm_normalize: the slabs take this many bytes of text scratch and as many n2o entries,
+// the packed chunk at most as much again (1.25 GB of device memory with offsets at most).  A single sentence whose slab
+// is larger is a chunk of its own.  Every chunk waits for its totals; at 2^25 the 1M-sentence uni32k/en batch (10
+// bytes of slab per input byte) took 40 chunks and spm_normalize with offsets was slower than spm_encode_spans.
+static constexpr unsigned long long kNormChunkSlab = 1ull << 27;
+
+// SentencePieceProcessor::Normalize for a host batch, in chunks of at most kNormChunkSlab slab elements: per chunk the
+// input goes up, normalize_kernel (K10) fills the slabs, the scan kernels pack them, and the packed chunk comes down
+// into the pinned results behind the earlier chunks.
+static int normalize_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, bool with_offsets,
+                            const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!offsets || !normalized || !norm_offsets || (with_offsets && !n2o) || (n && !bytes && offsets[n] != offsets[0])) {
+    e->set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  for (size_t i = 0; i < n; ++i)
+    if (offsets[i + 1] < offsets[i]) { e->set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
+  const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
+  for (size_t i = 0; i < n; ++i)
+    if (norm_slab_start(offsets[i + 1] - offsets[i], 1, expand) > 0x7FFFFF00ull) {
+      e->set_error("sentence too long for the device path");
+      return SPM_ERR_UNSUPPORTED;
+    }
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = e->stream;
+  e->last_launches = 0;
+  e->last_deferred = 0;
+  e->last_h2d = 0;
+  e->last_d2h = 0;
+  e->last_main_ms = 0.f;
+  e->last_ms = 0.f;
+  const uint64_t total_bytes = n ? offsets[n] - offsets[0] : 0;
+  CUDA_TRY(e->h_norm_offsets.ensure(n + 1));
+  CUDA_TRY(e->h_norm.ensure(total_bytes + total_bytes / 2 + 64));
+  if (with_offsets) CUDA_TRY(e->h_n2o.ensure(total_bytes + total_bytes / 2 + n + 64));
+  e->h_norm_offsets.p[0] = 0;
+  // the stream is idle when a pinned result grows (after read_status): what has arrived is kept
+  auto grow = [&](auto &buf, size_t have, size_t need) -> cudaError_t {
+    if (need <= buf.cap) return cudaSuccess;
+    std::remove_reference_t<decltype(buf)> bigger;
+    const cudaError_t err = bigger.ensure(need + need / 2);
+    if (err != cudaSuccess) return err;
+    if (have) memcpy(bigger.p, buf.p, have * sizeof(*buf.p));
+    buf = std::move(bigger);
+    return cudaSuccess;
+  };
+  KModel M = e->km;
+  M.hot_link = M.hot_val = 0;
+  unsigned long long done = 0;  // normalized bytes of the earlier chunks
+  for (size_t lo = 0; lo < n;) {
+    size_t hi = lo + 1;
+    while (hi < n && norm_slab_start(offsets[hi + 1] - offsets[lo], static_cast<uint32_t>(hi + 1 - lo), expand) <= kNormChunkSlab)
+      ++hi;
+    const uint32_t m = static_cast<uint32_t>(hi - lo);
+    const uint64_t chunk_bytes = offsets[hi] - offsets[lo];
+    const unsigned long long slab = norm_slab_start(chunk_bytes, m, expand);
+    CUDA_TRY(e->d_bytes.ensure(chunk_bytes + 64));
+    CUDA_TRY(e->d_offsets.ensure(m + 1));
+    CUDA_TRY(e->d_tmp_norm.ensure(slab + 16));
+    CUDA_TRY(e->d_norm_start.ensure(m));
+    CUDA_TRY(e->d_norm_len.ensure(m));
+    CUDA_TRY(e->d_norm.ensure(slab + 16));
+    CUDA_TRY(e->d_norm_offsets.ensure(m + 1));
+    if (with_offsets) {
+      CUDA_TRY(e->d_tmp_n2o.ensure(slab + 16));
+      CUDA_TRY(e->d_n2o.ensure(slab + 16));
+      CUDA_TRY(e->d_n2o_offsets.ensure(m + 1));
+    }
+    if (chunk_bytes) CUDA_TRY(cudaMemcpyAsync(e->d_bytes.p, bytes + offsets[lo], chunk_bytes, cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(e->d_offsets.p, offsets + lo, (m + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+    e->last_h2d += chunk_bytes + (m + 1) * sizeof(uint64_t);
+    CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, sizeof(uint32_t), st));
+    KNormalize A{};
+    A.bytes = e->d_bytes.p;
+    A.offsets = e->d_offsets.p;
+    A.n = m;
+    A.expand = expand;
+    A.text = e->d_tmp_norm.p;
+    A.n2o = with_offsets ? e->d_tmp_n2o.p : nullptr;
+    A.slab = e->d_norm_start.p;
+    A.len = e->d_norm_len.p;
+    A.status = e->d_ctrl32.p;
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (m + 7) / 8));
+    CUDA_TRY(cudaEventRecord(e->ev[0], st));
+    if (with_offsets) normalize_kernel<true><<<grid, 256, 0, st>>>(M, A);
+    else normalize_kernel<false><<<grid, 256, 0, st>>>(M, A);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+    CUDA_TRY(cudaEventRecord(e->ev[1], st));
+    SPM_TRY(e->scan_total(e->d_norm_len.p, m, 0, e->d_ctrl64.p + 2, st));
+    SPM_TRY(e->scan_gather<uint8_t>(e->d_norm_len.p, m, e->d_norm_offsets.p, e->d_norm_start.p, e->d_tmp_norm.p,
+                                    e->d_norm.p, e->d_norm.cap, 0, done, st));
+    if (with_offsets) {  // n_i + 1 entries per sentence
+      SPM_TRY(e->scan_total(e->d_norm_len.p, m, 1, e->d_ctrl64.p + 3, st));
+      SPM_TRY(e->scan_gather<uint32_t>(e->d_norm_len.p, m, e->d_n2o_offsets.p, e->d_norm_start.p, e->d_tmp_n2o.p,
+                                       e->d_n2o.p, e->d_n2o.cap, 1, 0ull, st));
+    }
+    CUDA_TRY(cudaEventRecord(e->ev[2], st));
+    SPM_TRY(e->read_status(st, 1, 4));
+    float k_ms = 0.f, all_ms = 0.f;
+    if (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess) e->last_main_ms += k_ms;
+    if (cudaEventElapsedTime(&all_ms, e->ev[0], e->ev[2]) == cudaSuccess) e->last_ms += all_ms;
+    if (e->h_ctrl32.p[0]) {
+      set_error("normalize: a sentence normalized to more bytes than its bound");
+      return SPM_ERR_ENCODE;
+    }
+    const unsigned long long tot = e->h_ctrl64.p[2];
+    CUDA_TRY(grow(e->h_norm, done, done + tot + 1));
+    if (tot) CUDA_TRY(cudaMemcpyAsync(e->h_norm.p + done, e->d_norm.p, tot, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(e->h_norm_offsets.p + lo, e->d_norm_offsets.p, (m + 1) * sizeof(uint64_t),
+                             cudaMemcpyDeviceToHost, st));
+    e->last_d2h += tot + (m + 1) * sizeof(uint64_t);
+    if (with_offsets) {
+      const unsigned long long n2o_done = done + lo;
+      CUDA_TRY(grow(e->h_n2o, n2o_done, n2o_done + tot + m + 1));
+      CUDA_TRY(cudaMemcpyAsync(e->h_n2o.p + n2o_done, e->d_n2o.p, (tot + m) * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+      e->last_d2h += (tot + m) * sizeof(uint32_t);
+    }
+    done += tot;
+    lo = hi;
+  }
+  CUDA_TRY(cudaStreamSynchronize(st));
+  e->h_norm.p[done] = 0;
+  *normalized = reinterpret_cast<const char *>(e->h_norm.p);
+  *norm_offsets = e->h_norm_offsets.p;
+  if (n2o) *n2o = with_offsets ? e->h_n2o.p : nullptr;
+  return SPM_OK;
+}
+
+int spm_normalize(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int with_offsets,
+                  const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return normalize_locked(e, bytes, offsets, n, with_offsets != 0, normalized, norm_offsets, n2o);
 }
 
 int spm_engine::write_pieces(KPieces &P, const char *unk_piece, size_t unk_len, const char **text,

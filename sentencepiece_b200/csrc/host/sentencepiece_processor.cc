@@ -313,6 +313,70 @@ util::Status SentencePieceProcessor::Encode(const std::vector<std::string_view> 
   return util::OkStatus();
 }
 
+util::Status SentencePieceProcessor::NormalizePacked(const char *bytes, const uint64_t *offsets, size_t n,
+                                                     bool with_offsets, const char **normalized,
+                                                     const uint64_t **norm_offsets, const uint32_t **n2o) const {
+  if (!engine_) return status();
+  return FromEngine(engine_, spm_normalize(engine_, bytes, offsets, n, with_offsets ? 1 : 0, normalized, norm_offsets, n2o));
+}
+
+util::Status SentencePieceProcessor::Normalize(const std::vector<std::string_view> &inputs,
+                                               std::vector<std::string> *normalized,
+                                               std::vector<std::vector<size_t>> *norm_to_orig) const {
+  if (!engine_) return status();
+  if (!normalized) return Internal("output container is null");
+  normalized->clear();
+  if (norm_to_orig) norm_to_orig->clear();
+  std::string bytes;
+  std::vector<uint64_t> offs;
+  Pack(inputs, &bytes, &offs);
+  const char *text = nullptr;
+  const uint64_t *no = nullptr;
+  const uint32_t *n2o = nullptr;
+  const auto st = NormalizePacked(bytes.data(), offs.data(), inputs.size(), norm_to_orig != nullptr, &text, &no, &n2o);
+  if (!st.ok()) return st;
+  normalized->resize(inputs.size());
+  if (norm_to_orig) norm_to_orig->resize(inputs.size());
+  ParallelFor(inputs.size(), [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) {
+      (*normalized)[i].assign(text + no[i], text + no[i + 1]);
+      if (!norm_to_orig) continue;
+      const uint32_t *m = n2o + no[i] + i;
+      if (m[0] != SPM_NORM_TO_ORIG_EMPTY) (*norm_to_orig)[i].assign(m, m + (no[i + 1] - no[i]) + 1);
+    }
+  });
+  return util::OkStatus();
+}
+
+util::Status SentencePieceProcessor::Normalize(std::string_view input, std::string *normalized,
+                                               std::vector<size_t> *norm_to_orig) const {
+  if (!engine_) return status();
+  if (!normalized || !norm_to_orig) return Internal("output container is null");
+  std::vector<std::string> t;
+  std::vector<std::vector<size_t>> m;
+  const auto st = Normalize(std::vector<std::string_view>{input}, &t, &m);
+  if (!st.ok()) return st;
+  *normalized = std::move(t[0]);
+  *norm_to_orig = std::move(m[0]);
+  return util::OkStatus();
+}
+
+util::Status SentencePieceProcessor::Normalize(std::string_view input, std::string *normalized) const {
+  if (!engine_) return status();
+  if (!normalized) return Internal("output container is null");
+  std::vector<std::string> t;
+  const auto st = Normalize(std::vector<std::string_view>{input}, &t);
+  if (!st.ok()) return st;
+  *normalized = std::move(t[0]);
+  return util::OkStatus();
+}
+
+std::string SentencePieceProcessor::Normalize(std::string_view input) const {
+  std::string normalized;
+  Normalize(input, &normalized).IgnoreError();
+  return normalized;
+}
+
 // The engine writes the pieces with the options applied: bos / eos / reverse are the frame SetEncodeExtraOptions set,
 // UNK_PIECE is passed as trainer_spec.unk_piece.
 const std::string *SentencePieceProcessor::UnkPiece() const {

@@ -125,6 +125,20 @@ class SentencePieceProcessor {
                                         int sep, const char **text, const uint64_t **text_offsets,
                                         const uint32_t **piece_end, const uint64_t **id_offsets) const;
 
+  // ---- Normalize (sentencepiece_processor.h:621-631): the model's normalizer, on the device (spm_normalize).
+  //      norm_to_orig as the reference returns it: empty for empty input and for input that is all heading
+  //      whitespace, else one entry per normalized byte and one for the end. ----
+  util::Status Normalize(std::string_view input, std::string *normalized) const;
+  util::Status Normalize(std::string_view input, std::string *normalized, std::vector<size_t> *norm_to_orig) const;
+  std::string Normalize(std::string_view input) const;
+  // one device call for all sentences; norm_to_orig may be null
+  util::Status Normalize(const std::vector<std::string_view> &inputs, std::vector<std::string> *normalized,
+                         std::vector<std::vector<size_t>> *norm_to_orig = nullptr) const;
+  // zero-copy form, the layout of spm_normalize: sentence i is normalized[norm_offsets[i] .. norm_offsets[i+1]), its
+  // norm_to_orig at n2o[norm_offsets[i] + i ...] (n2o null unless with_offsets), owned by the engine until the next call
+  util::Status NormalizePacked(const char *bytes, const uint64_t *offsets, size_t n, bool with_offsets,
+                               const char **normalized, const uint64_t **norm_offsets, const uint32_t **n2o) const;
+
   // ---- Decode(ids) (src/sentencepiece_processor.h Decode(const std::vector<int>&, std::string*)); the batch form is
   //      one device call for all lists.  An id outside [0, GetPieceSize()) fails the call like the reference's
   //      kOutOfRange (sentencepiece_processor.cc:915-918); decode_extra_options are not applied. ----

@@ -42,6 +42,70 @@ def split_pieces(text, text_offsets, piece_end, id_offsets):
     return out
 
 
+def _one_char_len(b):
+    """string_util::OneCharLen (util.h:151-153) of every byte of a uint8 array"""
+    return np.array([1] * 12 + [2, 2, 3, 4], np.int64)[b >> 4]
+
+
+def char_index(buf, offs):
+    """The utf8_to_unicode_offsets table of ConvertToUnicodeAlignment (sentencepiece_trainer.cc:369-388) for every
+    sentence of a packed batch, in the n2o layout: entry offs[i] - offs[0] + i + p is the index of the character that
+    holds byte p of sentence i (p = its length: the number of characters).  Characters are stepped by their lead byte's
+    OneCharLen; a step past the end of a malformed sentence, which the reference does not guard, stops at the end."""
+    buf = np.asarray(buf, np.uint8)
+    offs = np.asarray(offs, np.int64) - int(offs[0])
+    n = len(offs) - 1
+    lens = np.diff(offs)
+    # every byte that is not a trail byte starts a character, and so does the first byte of a sentence; that is the
+    # chain of OneCharLen steps wherever each step lands on the next such byte (always, for valid UTF-8)
+    start = (buf & 0xC0) != 0x80
+    start[offs[:-1][lens > 0]] = True
+    sid = np.repeat(np.arange(n), lens)
+    pos = np.flatnonzero(start)
+    nxt = np.append(pos[1:], len(buf))
+    ends = offs[1:][sid[pos]]
+    nxt = np.minimum(nxt, ends)
+    good = np.ones(n, bool)
+    step = np.minimum(pos + _one_char_len(buf[pos]), ends)
+    good[sid[pos[step != nxt]]] = False
+    for i in np.flatnonzero(~good):  # malformed sentences only: follow the steps
+        s = np.zeros(lens[i], bool)
+        p, lead = 0, _one_char_len(buf[offs[i]:offs[i + 1]])
+        while p < lens[i]:
+            s[p] = True
+            p += int(lead[p])
+        start[offs[i]:offs[i + 1]] = s
+    # one more slot per sentence (its end), counted as a start: the running count minus one is the character index
+    ext = np.insert(start.astype(np.int64), offs[1:], 1)
+    csum = np.cumsum(ext)
+    first = offs[:-1] + np.arange(n)
+    before = np.where(first > 0, csum[np.maximum(first - 1, 0)], 0)
+    return csum - np.repeat(before, lens + 1) - 1
+
+
+def unicode_alignment(orig, orig_offs, norm, norm_offs, n2o):
+    """ConvertToUnicodeAlignment (sentencepiece_trainer.cc:369-397) of spm_normalize's byte offsets, for a whole batch
+    -> (uint64 offsets[n+1], int64 values): sentence i's character offsets are values[offsets[i]:offsets[i+1]], one
+    per normalized character and one for the end.  Where the byte offsets are empty (n2o entry NORM_TO_ORIG_EMPTY) the
+    reference's table of one zero is left as it is: [0]."""
+    n = len(norm_offs) - 1
+    norm_offs = np.asarray(norm_offs, np.int64)
+    n2o = np.asarray(n2o, np.int64)
+    ni = char_index(norm, norm_offs)
+    oi = char_index(orig, orig_offs)
+    sent = np.repeat(np.arange(n), np.diff(norm_offs) + 1)
+    last = np.zeros(len(ni), bool)  # the last byte of each normalized character wins, and every sentence's end
+    last[:-1] = ni[:-1] != ni[1:]
+    last[norm_offs[1:] - norm_offs[0] + np.arange(n)] = True
+    sel = np.flatnonzero(last)
+    empty = n2o[sel] == _capi.NORM_TO_ORIG_EMPTY
+    orig_base = np.asarray(orig_offs, np.int64)[:-1] - int(orig_offs[0]) + np.arange(n)
+    values = np.where(empty, 0, oi[np.where(empty, 0, orig_base[sent[sel]] + n2o[sel])])
+    offsets = np.zeros(n + 1, np.uint64)
+    offsets[1:] = np.cumsum(np.bincount(sent[sel], minlength=n))
+    return offsets, values
+
+
 def pack_sentences(sentences):
     """list[bytes|str] -> (uint8[total], uint64[n+1])"""
     bs = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in sentences]
@@ -144,6 +208,24 @@ class Engine:
         norm = ctypes.string_at(p[3], tn) if tn else b""
         n2o = np.ctypeslib.as_array(ctypes.cast(p[5], ctypes.POINTER(ctypes.c_uint32)), (tn + n,)).copy()
         return dict(ids=ids, tok_end=te, id_offsets=ido, normalized=norm, norm_offsets=no, n2o=n2o)
+
+    def normalize(self, buf, offs, with_offsets=False):
+        """spm_normalize: the model's normalizer over a packed batch -> (normalized uint8[], norm_offsets uint64[n+1],
+        n2o uint32[] or None).  With offsets, sentence i's norm_to_orig is n2o[norm_offsets[i] + i : norm_offsets[i+1] +
+        i + 1], the one entry _capi.NORM_TO_ORIG_EMPTY where the reference's is empty."""
+        n = len(offs) - 1
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(3)]
+        self._check(self._lib.spm_normalize(self._h, buf.ctypes.data, offs.ctypes.data, n, int(bool(with_offsets)),
+                                            *[ctypes.byref(x) for x in p]))
+        no = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+        tn = int(no[n])
+        text = np.ctypeslib.as_array(ctypes.cast(p[0], ctypes.POINTER(ctypes.c_uint8)), (max(tn, 1),))[:tn].copy()
+        if not with_offsets:
+            return text, no, None
+        n2o = np.ctypeslib.as_array(ctypes.cast(p[2], ctypes.POINTER(ctypes.c_uint32)), (max(tn + n, 1),))[:tn + n].copy()
+        return text, no, n2o
 
     def encode_pieces(self, buf, offs, unk_piece=None, sep=-1):
         """spm_encode_pieces: EncodeAsPieces over a packed batch, the encode frame applied ->
@@ -609,6 +691,33 @@ class SentencePieceProcessor:
         (all L when lengths is None), cut before its first stop_id (e.g. eos_id()) when one is given."""
         self._require()
         return self._engine.decode_device(ids, lengths, -1 if stop_id is None else stop_id)
+
+    # python/src/sentencepiece/__init__.py Normalize, sentencepiece.i _Normalize / _NormalizeWithOffsets
+    def Normalize(self, input, with_offsets=None):
+        """The model's normalizer (SentencePieceProcessor::Normalize) on one str / bytes or a list of them: the same type
+        back, with with_offsets a (text, offsets) pair per item.  Offsets map each normalized position, and the end, to
+        the input: in characters for str input (ConvertToUnicodeAlignment), in bytes for bytes input."""
+        self._require()
+        single = not isinstance(input, list)
+        items = [input] if single else input
+        buf, offs = pack_sentences(items)
+        text, no, n2o = self._engine.normalize(buf, offs, with_offsets=bool(with_offsets))
+        raw = text.tobytes()
+        outs = [raw[int(no[i]):int(no[i + 1])] for i in range(len(items))]
+        outs = [o.decode("utf-8") if isinstance(x, str) else o for o, x in zip(outs, items)]
+        if not with_offsets:
+            return outs[0] if single else outs
+        uo, uv = unicode_alignment(buf, offs, text, no, n2o)
+        res = []
+        for i, x in enumerate(items):
+            if isinstance(x, str):
+                res.append((outs[i], uv[int(uo[i]):int(uo[i + 1])].tolist()))
+            else:
+                m = n2o[int(no[i]) + i:int(no[i + 1]) + i + 1]
+                res.append((outs[i], [] if m[0] == _capi.NORM_TO_ORIG_EMPTY else m.tolist()))
+        return res[0] if single else res
+
+    normalize = Normalize
 
     # sentencepiece_processor.h:521-526
     def CalculateEntropy(self, input, alpha):
