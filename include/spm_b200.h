@@ -174,6 +174,29 @@ int spm_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets,
                       const char **text, const uint64_t **text_offsets, const uint32_t **piece_end,
                       const int32_t **ids, const uint64_t **id_offsets);
 
+/* Replaces the per-sentence loop over SentencePieceProcessor::Encode(absl::string_view, SentencePieceText*) /
+ * EncodeAsImmutableProto (src/sentencepiece_processor.cc:547-636 and ApplyExtraOptions, :1019-1064) for n sentences:
+ * the ids of every token and where it came from in the input.
+ * out (engine-owned pinned memory, valid until the next call):
+ *   ids / id_offsets: exactly what spm_encode_ids returns under the current encode frame;
+ *   begin[k] / end[k]: the byte range of ids[k] in its sentence's input (relative to offsets[i]), as the reference's
+ *     SentencePieceText.pieces(k).begin() / end().  A normal or user-defined piece covers the input that normalized to
+ *     it; an unknown token (a whole run of unknown characters) the run's input; with byte fallback, the byte tokens of
+ *     an unknown character all begin at the character, the last ends after it and the others end where they begin.
+ *     Frame entries equal to eos_id get (len, len), every other frame entry (0, 0); the frame reverses the body
+ *     together with its offsets.  The surface of a token is input[begin, end).
+ *   text != NULL: text / text_offsets / piece_end are exactly spm_encode_pieces with the same unk_piece and sep.
+ *     text == NULL: no pieces are written (text_offsets and piece_end may be NULL too); unk_piece and sep are only
+ *     checked.
+ * Sentences that hold the unknown id are encoded a second time by the spans path for the extents of their unknown
+ * tokens, with or without unk_piece (spm_engine_info.last_unk_detour counts them).  Argument errors as
+ * spm_encode_pieces, and "sentence too long" as spm_normalize; n == 0 succeeds with id_offsets = {0}. */
+int spm_encode_offsets(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int32_t eos_id,
+                       const char *unk_piece, size_t unk_piece_len, int sep,
+                       const int32_t **ids, const uint64_t **id_offsets,
+                       const uint32_t **begin, const uint32_t **end,
+                       const char **text, const uint64_t **text_offsets, const uint32_t **piece_end);
+
 /* ------------------------------------------------------------------------
  * Batch encode, DEVICE buffers (inputs already resident in HBM; used when the
  * caller keeps corpora on the GPU, and by bench.py for the kernel-only number).

@@ -17,7 +17,7 @@ EXPORTS = [
     "spm_sample_encode_ids", "spm_decode_ids", "spm_engine_set_unk_surface", "spm_calculate_entropy",
     "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
     "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
-    "spm_encode_ids_device_padded", "spm_decode_ids_device", "spm_normalize",
+    "spm_encode_ids_device_padded", "spm_decode_ids_device", "spm_normalize", "spm_encode_offsets",
 ]
 
 # spm_normalize: the n2o entry of a sentence whose reference norm_to_orig is empty
@@ -75,6 +75,7 @@ def load():
     L.spm_encode_spans.argtypes = [vp, vp, vp, sz, P(vp), P(vp), P(vp), P(vp), P(vp), P(vp)]
     L.spm_normalize.argtypes = [vp, vp, vp, sz, ctypes.c_int, P(vp), P(vp), P(vp)]
     L.spm_encode_pieces.argtypes = [vp, vp, vp, sz, cp, sz, ctypes.c_int, P(vp), P(vp), P(vp), P(vp), P(vp)]
+    L.spm_encode_offsets.argtypes = [vp, vp, vp, sz, ctypes.c_int32, cp, sz, ctypes.c_int] + [P(vp)] * 7
     L.spm_encode_ids_device.argtypes = [vp, vp, vp, sz, ctypes.c_uint64, vp, ctypes.c_uint64, vp,
                                         P(ctypes.c_uint64), vp]
     u32, u64 = ctypes.c_uint32, ctypes.c_uint64

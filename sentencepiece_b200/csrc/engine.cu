@@ -40,6 +40,7 @@
 #include "pieces_kernel.cuh"
 #include "nbest_kernel.cuh"
 #include "normalize_kernel.cuh"
+#include "offsets_kernel.cuh"
 #include "lattice_kernel.cuh"
 #include "trie_builder.h"
 
@@ -464,6 +465,15 @@ struct spm_engine {
   // *d2h: the bytes copied.
   int write_pieces(KPieces &P, const char *unk_piece, size_t unk_len, const char **text, const uint64_t **text_offsets,
                    const uint32_t **piece_end, const int32_t **ids, const uint64_t **id_offsets, uint64_t *d2h);
+  // The raw segmentation of a host batch (n > 0, offsets checked) on the device, for K9 and K11: uploads the input
+  // into d_bytes / d_offsets and fills P's sources (ids, id_offsets and, with `detour`, the unknown-surface subset).
+  // Sets last_h2d, last_deferred and last_unk_detour; *raw_ids: the ids of the raw segmentation, *main_ms: the encode
+  // kernel's time.
+  int raw_segmentation(const char *bytes, const uint64_t *offsets, size_t n, bool detour, KPieces *P, uint64_t *raw_ids,
+                       float *main_ms);
+  // spm_encode_offsets (K11): begin / end of the framed tokens
+  DevBuf<uint32_t> d_off_begin, d_off_end;
+  PinBuf<uint32_t> h_off_begin, h_off_end;
   // n-best / sampling; pieces: the candidates' token ends and the exported normalized texts (NbestOut)
   DevBuf<uint8_t> d_nb_scratch, d_nb_norm;
   DevBuf<uint32_t> d_nb_end;
@@ -3372,12 +3382,95 @@ int spm_engine::write_pieces(KPieces &P, const char *unk_piece, size_t unk_len, 
   return SPM_OK;
 }
 
+int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, size_t n, bool detour, KPieces *P,
+                                 uint64_t *raw_ids, float *main_ms) {
+  cudaStream_t st = stream;
+  const uint64_t base = offsets[0];
+  const uint64_t total_bytes = offsets[n] - base;
+  if (model.model_type == SPM_UNIGRAM) batch_fast_words = pick_fast_words_host(bytes, offsets, n);
+  CUDA_TRY(d_bytes.ensure(total_bytes + 64));
+  CUDA_TRY(d_offsets.ensure(n + 1));
+  CUDA_TRY(cudaEventRecord(ev[3], st));
+  if (total_bytes) CUDA_TRY(cudaMemcpyAsync(d_bytes.p, bytes + base, total_bytes, cudaMemcpyHostToDevice, st));
+  CUDA_TRY(cudaMemcpyAsync(d_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
+  last_h2d = total_bytes + (n + 1) * sizeof(uint64_t);
+  // ---- 1. raw ids: the frame is written once, by K9 / K11 ----
+  int rc;
+  {
+    struct FrameOff {
+      spm_engine *e;
+      uint32_t np, ns;
+      bool rev;
+      explicit FrameOff(spm_engine *x) : e(x), np(x->frame_np), ns(x->frame_ns), rev(x->frame_rev) {
+        x->frame_np = x->frame_ns = 0;
+        x->frame_rev = false;
+      }
+      ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
+    } off(this);
+    rc = run_device(d_bytes.p - base, d_offsets.p, n, total_bytes, false, nullptr, 0, nullptr, raw_ids, nullptr, st,
+                    &d_pc_ids, &d_pc_id_offsets);
+  }
+  if (rc) return rc;
+  if (cudaEventElapsedTime(main_ms, ev[0], ev[1]) != cudaSuccess) *main_ms = 0.f;
+  uint64_t deferred = last_deferred;
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (n + 7) / 8));
+  P->n = n32;
+  P->ids = d_pc_ids.p;
+  P->id_offsets = d_pc_id_offsets.p;
+  // ---- 2. unknown extents: only the sentences that hold the unknown id take the spans path ----
+  uint32_t m = 0;
+  if (detour && unk_id >= 0) {
+    CUDA_TRY(d_pc_flag.ensure(n));
+    CUDA_TRY(d_pc_pos.ensure(n + 1));
+    pieces_unk_flag_kernel<<<wgrid, 256, 0, st>>>(d_pc_ids.p, d_pc_id_offsets.p, n32, unk_id, d_pc_flag.p);
+    CUDA_TRY(cudaGetLastError());
+    ++last_launches;
+    SPM_TRY(scan_total(d_pc_flag.p, n32, 0, d_ctrl64.p + 2, st));
+    SPM_TRY(scan_gather<uint8_t>(d_pc_flag.p, n32, d_pc_pos.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+    SPM_TRY(read_status(st, 0, 4));
+    m = static_cast<uint32_t>(h_ctrl64.p[2]);
+  }
+  if (m) {
+    CUDA_TRY(d_pc_sub_of.ensure(n));
+    CUDA_TRY(d_pc_sub_start.ensure(m));
+    CUDA_TRY(d_pc_sub_len.ensure(m));
+    CUDA_TRY(d_pc_sub_offsets.ensure(m + 1));
+    CUDA_TRY(d_pc_sub_bytes.ensure(total_bytes + 64));
+    pieces_sub_list_kernel<<<static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (n + 255) / 256)), 256, 0, st>>>(
+        d_pc_flag.p, d_pc_pos.p, d_offsets.p, n32, d_pc_sub_of.p, d_pc_sub_start.p, d_pc_sub_len.p);
+    CUDA_TRY(cudaGetLastError());
+    ++last_launches;
+    SPM_TRY(scan_total(d_pc_sub_len.p, m, 0, d_ctrl64.p + 2, st));
+    SPM_TRY(scan_gather<uint8_t>(d_pc_sub_len.p, m, d_pc_sub_offsets.p, d_pc_sub_start.p, d_bytes.p - base,
+                                 d_pc_sub_bytes.p, d_pc_sub_bytes.cap, 0, 0ull, st));
+    // (the whole batch's byte count bounds the subset's: it only sizes the spans run's temporary buffers)
+    uint64_t sub_tot = 0, sub_norm = 0;
+    const uint64_t launches = last_launches;  // run_device starts its own count
+    rc = run_device(d_pc_sub_bytes.p, reinterpret_cast<const uint64_t *>(d_pc_sub_offsets.p), m, total_bytes, true,
+                    nullptr, 0, nullptr, &sub_tot, &sub_norm, st);
+    if (rc) return rc;
+    last_launches += launches;
+    deferred += last_deferred;
+    P->sub_of = d_pc_sub_of.p;
+    P->sub_ids = d_ids.p;
+    P->sub_tok_end = d_tok_end.p;
+    P->sub_id_offsets = d_id_offsets.p;
+    P->norm = d_norm.p;
+    P->norm_offsets = d_norm_offsets.p;
+  }
+  last_deferred = deferred;
+  last_unk_detour = m;
+  return SPM_OK;
+}
+
 // EncodeAsPieces for a host batch:
 //   1. raw ids from the kernels spm_encode_ids runs (lane / BPE-lane2 kernels, deferred and long kernels), frame off;
 //   2. without unk_piece: the sentences whose raw ids hold the unknown id are packed on the device and run through the
 //      spans path, which gives their token ends in the normalized text (the surfaces of their unknown tokens);
 //   3. K9 (pieces_kernel.cuh): size pass, scans, write pass -- the frame, reverse, unk_piece and sep applied once, to
 //      pieces and ids alike.
+// Steps 1 and 2 are spm_engine::raw_segmentation.
 static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, const char *unk_piece,
                                 size_t unk_len, int sep, const char **text, const uint64_t **text_offsets,
                                 const uint32_t **piece_end, const int32_t **ids, const uint64_t **id_offsets) {
@@ -3391,7 +3484,6 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   if (unk_len > 0xFFFFFFull) { e->set_error("unk_piece too long"); return SPM_ERR_ARG; }
   if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
   CUDA_TRY(cudaSetDevice(e->device));
-  cudaStream_t st = e->stream;
   e->last_unk_detour = 0;
   CUDA_TRY(e->h_pc_text_offsets.ensure(n + 1));
   CUDA_TRY(e->h_id_offsets.ensure(n + 1));
@@ -3406,92 +3498,18 @@ static int encode_pieces_locked(spm_engine *e, const char *bytes, const uint64_t
   }
   for (size_t i = 0; i < n; ++i)
     if (offsets[i + 1] < offsets[i]) { e->set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
-  const uint64_t base = offsets[0];
-  const uint64_t total_bytes = offsets[n] - base;
-  if (e->model.model_type == SPM_UNIGRAM) e->batch_fast_words = e->pick_fast_words_host(bytes, offsets, n);
-  { const int rc = e->ensure_piece_tables(); if (rc) return rc; }
-  CUDA_TRY(e->d_bytes.ensure(total_bytes + 64));
-  CUDA_TRY(e->d_offsets.ensure(n + 1));
-  CUDA_TRY(cudaEventRecord(e->ev[3], st));
-  if (total_bytes) CUDA_TRY(cudaMemcpyAsync(e->d_bytes.p, bytes + base, total_bytes, cudaMemcpyHostToDevice, st));
-  CUDA_TRY(cudaMemcpyAsync(e->d_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-  e->last_h2d = total_bytes + (n + 1) * sizeof(uint64_t) + unk_len;
-  // ---- 1. raw ids: the frame is written once, by K9 ----
-  uint64_t raw_tot = 0;
-  int rc;
-  {
-    struct FrameOff {
-      spm_engine *e;
-      uint32_t np, ns;
-      bool rev;
-      explicit FrameOff(spm_engine *x) : e(x), np(x->frame_np), ns(x->frame_ns), rev(x->frame_rev) {
-        x->frame_np = x->frame_ns = 0;
-        x->frame_rev = false;
-      }
-      ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
-    } off(e);
-    rc = e->run_device(e->d_bytes.p - base, e->d_offsets.p, n, total_bytes, false, nullptr, 0, nullptr, &raw_tot, nullptr, st,
-                       &e->d_pc_ids, &e->d_pc_id_offsets);
-  }
-  if (rc) return rc;
-  float main_ms = 0.f;
-  if (cudaEventElapsedTime(&main_ms, e->ev[0], e->ev[1]) != cudaSuccess) main_ms = 0.f;
-  uint64_t deferred = e->last_deferred;
-  const uint32_t n32 = static_cast<uint32_t>(n);
-  const int wgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  SPM_TRY(e->ensure_piece_tables());
   KPieces P{};
-  P.n = n32;
-  P.ids = e->d_pc_ids.p;
-  P.id_offsets = e->d_pc_id_offsets.p;
+  uint64_t raw_ids = 0;
+  float main_ms = 0.f;
+  SPM_TRY(e->raw_segmentation(bytes, offsets, n, !unk_piece, &P, &raw_ids, &main_ms));
+  e->last_h2d += unk_len;
   P.sep = sep;
   P.F = e->kframe();
-  // ---- 2. unknown surfaces: only the sentences that hold the unknown id take the spans path ----
-  uint32_t m = 0;
-  if (!unk_piece && e->unk_id >= 0) {
-    CUDA_TRY(e->d_pc_flag.ensure(n));
-    CUDA_TRY(e->d_pc_pos.ensure(n + 1));
-    pieces_unk_flag_kernel<<<wgrid, 256, 0, st>>>(e->d_pc_ids.p, e->d_pc_id_offsets.p, n32, e->unk_id, e->d_pc_flag.p);
-    CUDA_TRY(cudaGetLastError());
-    ++e->last_launches;
-    SPM_TRY(e->scan_total(e->d_pc_flag.p, n32, 0, e->d_ctrl64.p + 2, st));
-    SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_flag.p, n32, e->d_pc_pos.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
-    SPM_TRY(e->read_status(st, 0, 4));
-    m = static_cast<uint32_t>(e->h_ctrl64.p[2]);
-  }
-  if (m) {
-    CUDA_TRY(e->d_pc_sub_of.ensure(n));
-    CUDA_TRY(e->d_pc_sub_start.ensure(m));
-    CUDA_TRY(e->d_pc_sub_len.ensure(m));
-    CUDA_TRY(e->d_pc_sub_offsets.ensure(m + 1));
-    CUDA_TRY(e->d_pc_sub_bytes.ensure(total_bytes + 64));
-    pieces_sub_list_kernel<<<static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256)), 256, 0, st>>>(
-        e->d_pc_flag.p, e->d_pc_pos.p, e->d_offsets.p, n32, e->d_pc_sub_of.p, e->d_pc_sub_start.p, e->d_pc_sub_len.p);
-    CUDA_TRY(cudaGetLastError());
-    ++e->last_launches;
-    SPM_TRY(e->scan_total(e->d_pc_sub_len.p, m, 0, e->d_ctrl64.p + 2, st));
-    SPM_TRY(e->scan_gather<uint8_t>(e->d_pc_sub_len.p, m, e->d_pc_sub_offsets.p, e->d_pc_sub_start.p, e->d_bytes.p - base,
-                                    e->d_pc_sub_bytes.p, e->d_pc_sub_bytes.cap, 0, 0ull, st));
-    // (the whole batch's byte count bounds the subset's: it only sizes the spans run's temporary buffers)
-    uint64_t sub_tot = 0, sub_norm = 0;
-    const uint64_t launches = e->last_launches;  // run_device starts its own count
-    rc = e->run_device(e->d_pc_sub_bytes.p, reinterpret_cast<const uint64_t *>(e->d_pc_sub_offsets.p), m, total_bytes, true,
-                       nullptr, 0, nullptr, &sub_tot, &sub_norm, st);
-    if (rc) return rc;
-    e->last_launches += launches;
-    deferred += e->last_deferred;
-    P.sub_of = e->d_pc_sub_of.p;
-    P.sub_ids = e->d_ids.p;
-    P.sub_tok_end = e->d_tok_end.p;
-    P.sub_id_offsets = e->d_id_offsets.p;
-    P.norm = e->d_norm.p;
-    P.norm_offsets = e->d_norm_offsets.p;
-  }
   // ---- 3. K9: sizes, offsets, pieces ----
   uint64_t d2h = 0;
   SPM_TRY(e->write_pieces(P, unk_piece, unk_len, text, text_offsets, piece_end, ids, id_offsets, &d2h));
   e->last_d2h = d2h;
-  e->last_deferred = deferred;
-  e->last_unk_detour = m;
   e->last_main_ms = main_ms;
   float all = 0.f;
   e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : main_ms;
@@ -3506,6 +3524,161 @@ int spm_encode_pieces(spm_engine *e, const char *bytes, const uint64_t *offsets,
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_pieces_locked(e, bytes, offsets, n, unk_piece, unk_piece_len, sep, text, text_offsets, piece_end, ids,
                               id_offsets);
+}
+
+// EncodeAsImmutableProto's ids, offsets and (text != NULL) pieces for a host batch:
+//   1. the raw segmentation, with the unknown detour whatever unk_piece is: K11 needs the extents of unknown tokens;
+//   2. K11 (offsets_kernel.cuh) in chunks of at most kNormChunkSlab slab elements, as spm_normalize: each chunk
+//      normalizes its sentences into slabs and writes begin / end (and, without pieces, the framed ids) in place.
+//      The chunks need no totals, so they are queued back to back;
+//   3. with pieces: K9 as spm_encode_pieces, which also writes the ids.
+static int encode_offsets_locked(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int32_t eos_id,
+                                 const char *unk_piece, size_t unk_len, int sep, const int32_t **ids,
+                                 const uint64_t **id_offsets, const uint32_t **begin, const uint32_t **end,
+                                 const char **text, const uint64_t **text_offsets, const uint32_t **piece_end) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!offsets || !ids || !id_offsets || !begin || !end || (text && (!text_offsets || !piece_end)) ||
+      (unk_len && !unk_piece) || (n && !bytes && offsets[n] != offsets[0])) {
+    e->set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (sep < -1 || sep > 255) { e->set_error("sep must be -1 or a byte value"); return SPM_ERR_ARG; }
+  if (unk_len > 0xFFFFFFull) { e->set_error("unk_piece too long"); return SPM_ERR_ARG; }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  for (size_t i = 0; i < n; ++i)
+    if (offsets[i + 1] < offsets[i]) { e->set_error("offsets must be non-decreasing"); return SPM_ERR_ARG; }
+  const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
+  for (size_t i = 0; i < n; ++i)
+    if (norm_slab_start(offsets[i + 1] - offsets[i], 1, expand) > 0x7FFFFF00ull) {
+      e->set_error("sentence too long for the device path");
+      return SPM_ERR_UNSUPPORTED;
+    }
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = e->stream;
+  e->last_unk_detour = 0;
+  if (n == 0) {
+    e->last_launches = e->last_deferred = e->last_h2d = e->last_d2h = 0;
+    e->last_main_ms = e->last_ms = 0.f;
+    CUDA_TRY(e->h_ids.ensure(1)); CUDA_TRY(e->h_id_offsets.ensure(1));
+    CUDA_TRY(e->h_off_begin.ensure(1)); CUDA_TRY(e->h_off_end.ensure(1));
+    e->h_id_offsets.p[0] = 0;
+    *ids = e->h_ids.p; *id_offsets = e->h_id_offsets.p; *begin = e->h_off_begin.p; *end = e->h_off_end.p;
+    if (text) {
+      CUDA_TRY(e->h_pc_text.ensure(1)); CUDA_TRY(e->h_pc_text_offsets.ensure(1)); CUDA_TRY(e->h_pc_end.ensure(1));
+      e->h_pc_text.p[0] = 0;
+      e->h_pc_text_offsets.p[0] = 0;
+      *text = e->h_pc_text.p; *text_offsets = e->h_pc_text_offsets.p; *piece_end = e->h_pc_end.p;
+    }
+    return SPM_OK;
+  }
+  SPM_TRY(e->ensure_piece_tables());
+  KPieces P{};
+  uint64_t raw_ids = 0;
+  float main_ms = 0.f;
+  SPM_TRY(e->raw_segmentation(bytes, offsets, n, true, &P, &raw_ids, &main_ms));
+  e->last_h2d += unk_len;
+  P.sep = sep;
+  P.F = e->kframe();
+  P.pc_off = e->d_pc_off.p;
+  P.pc_bytes = e->d_pc_bytes.p;
+  P.unk_id = e->unk_id;
+  const uint64_t tids = raw_ids + static_cast<uint64_t>(n) * (P.F.np + P.F.ns);
+  // ---- 2. K11 ----
+  std::vector<size_t> cut{0};  // chunk c is sentences [cut[c], cut[c + 1])
+  unsigned long long slab_max = 0;
+  while (cut.back() < n) {
+    const size_t lo = cut.back();
+    size_t hi = lo + 1;
+    while (hi < n && norm_slab_start(offsets[hi + 1] - offsets[lo], static_cast<uint32_t>(hi + 1 - lo), expand) <= kNormChunkSlab)
+      ++hi;
+    slab_max = std::max(slab_max, norm_slab_start(offsets[hi] - offsets[lo], static_cast<uint32_t>(hi - lo), expand));
+    cut.push_back(hi);
+  }
+  CUDA_TRY(e->d_tmp_norm.ensure(slab_max + 16));
+  CUDA_TRY(e->d_tmp_n2o.ensure(slab_max + 16));
+  CUDA_TRY(e->d_off_begin.ensure(tids + 1));
+  CUDA_TRY(e->d_off_end.ensure(tids + 1));
+  if (!text) {
+    CUDA_TRY(e->d_pc_out_ids.ensure(tids + 1));
+    CUDA_TRY(e->d_pc_out_id_offsets.ensure(n + 1));
+  }
+  CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, sizeof(uint32_t), st));
+  KModel M = e->km;
+  M.hot_link = M.hot_val = 0;
+  KOffsets A{};
+  A.P = P;
+  A.offsets = e->d_offsets.p;
+  A.expand = expand;
+  A.slab_text = e->d_tmp_norm.p;
+  A.slab_n2o = e->d_tmp_n2o.p;
+  A.eos_id = eos_id;
+  A.begin = e->d_off_begin.p;
+  A.end = e->d_off_end.p;
+  A.out_ids = text ? nullptr : e->d_pc_out_ids.p;
+  A.out_id_offsets = text ? nullptr : e->d_pc_out_id_offsets.p;
+  A.status = e->d_ctrl32.p;
+  CUDA_TRY(cudaEventRecord(e->ev[0], st));  // (raw_segmentation has read ev[0] / ev[1])
+  for (size_t c = 0; c + 1 < cut.size(); ++c) {
+    A.first = static_cast<uint32_t>(cut[c]);
+    A.n = static_cast<uint32_t>(cut[c + 1] - cut[c]);
+    A.bytes = e->d_bytes.p + (offsets[cut[c]] - offsets[0]);
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (A.n + 7) / 8));
+    offsets_kernel<<<grid, 256, 0, st>>>(M, A);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  CUDA_TRY(cudaEventRecord(e->ev[1], st));
+  CUDA_TRY(e->h_off_begin.ensure(tids + 1));
+  CUDA_TRY(e->h_off_end.ensure(tids + 1));
+  if (tids) {
+    CUDA_TRY(cudaMemcpyAsync(e->h_off_begin.p, e->d_off_begin.p, tids * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(e->h_off_end.p, e->d_off_end.p, tids * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  }
+  SPM_TRY(e->copy_status(st, 1, 0));
+  uint64_t d2h = tids * 8;
+  // ---- 3. the ids: K9 with the pieces, or K11's ----
+  if (text) {
+    uint64_t d2h_pieces = 0;
+    SPM_TRY(e->write_pieces(P, unk_piece, unk_len, text, text_offsets, piece_end, ids, id_offsets, &d2h_pieces));
+    d2h += d2h_pieces;
+  } else {
+    CUDA_TRY(e->h_ids.ensure(tids + 1));
+    CUDA_TRY(e->h_id_offsets.ensure(n + 1));
+    if (tids) CUDA_TRY(cudaMemcpyAsync(e->h_ids.p, e->d_pc_out_ids.p, tids * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(e->h_id_offsets.p, e->d_pc_out_id_offsets.p, (n + 1) * sizeof(uint64_t),
+                             cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaEventRecord(e->ev[2], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    d2h += tids * 4 + (n + 1) * 8;
+    *ids = e->h_ids.p;
+    *id_offsets = e->h_id_offsets.p;
+  }
+  if (e->h_ctrl32.p[0] & 2u) {
+    set_error("encode offsets: a sentence normalized to more bytes than its bound");
+    return SPM_ERR_ENCODE;
+  }
+  if (e->h_ctrl32.p[0]) {
+    set_error("encode offsets: all normalized characters are not consumed");
+    return SPM_ERR_ENCODE;
+  }
+  *begin = e->h_off_begin.p;
+  *end = e->h_off_end.p;
+  e->last_d2h = d2h;
+  float k_ms = 0.f, all = 0.f;
+  e->last_main_ms = main_ms + (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess ? k_ms : 0.f);
+  e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : e->last_main_ms;
+  (void)cudaGetLastError();
+  return SPM_OK;
+}
+
+int spm_encode_offsets(spm_engine *e, const char *bytes, const uint64_t *offsets, size_t n, int32_t eos_id,
+                       const char *unk_piece, size_t unk_piece_len, int sep, const int32_t **ids,
+                       const uint64_t **id_offsets, const uint32_t **begin, const uint32_t **end, const char **text,
+                       const uint64_t **text_offsets, const uint32_t **piece_end) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  return encode_offsets_locked(e, bytes, offsets, n, eos_id, unk_piece, unk_piece_len, sep, ids, id_offsets, begin, end,
+                               text, text_offsets, piece_end);
 }
 
 // unk_piece / sep as spm_encode_pieces takes them

@@ -420,6 +420,62 @@ util::Status SentencePieceProcessor::SampleEncodePiecesPacked(const char *bytes,
                                                       text_offsets, piece_end, &ids, id_offsets));
 }
 
+util::Status SentencePieceProcessor::EncodeOffsetsPacked(const char *bytes, const uint64_t *offsets, size_t n,
+                                                         const int32_t **ids, const uint64_t **id_offsets,
+                                                         const uint32_t **begin, const uint32_t **end, const char **text,
+                                                         const uint64_t **text_offsets,
+                                                         const uint32_t **piece_end) const {
+  if (!engine_) return status();
+  const std::string *up = UnkPiece();
+  return FromEngine(engine_, spm_encode_offsets(engine_, bytes, offsets, n, eos_id(), up ? up->data() : nullptr,
+                                                up ? up->size() : 0, -1, ids, id_offsets, begin, end, text,
+                                                text_offsets, piece_end));
+}
+
+util::Status SentencePieceProcessor::EncodeWithOffsets(const std::vector<std::string_view> &inputs,
+                                                       std::vector<std::vector<PieceSpan>> *pieces) const {
+  if (!engine_) return status();
+  if (!pieces) return Internal("output container is null");
+  pieces->clear();
+  std::string bytes;
+  std::vector<uint64_t> offs;
+  Pack(inputs, &bytes, &offs);
+  const int32_t *ids;
+  const uint64_t *ido, *to;
+  const uint32_t *b, *e, *pe;
+  const char *text;
+  const auto st = EncodeOffsetsPacked(bytes.data(), offs.data(), inputs.size(), &ids, &ido, &b, &e, &text, &to, &pe);
+  if (!st.ok()) return st;
+  pieces->resize(inputs.size());
+  ParallelFor(inputs.size(), [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) {
+      auto &v = (*pieces)[i];
+      v.resize(ido[i + 1] - ido[i]);
+      const char *t = text + to[i];
+      for (uint64_t k = ido[i]; k < ido[i + 1]; ++k) {
+        PieceSpan &s = v[k - ido[i]];
+        const uint32_t p0 = k > ido[i] ? pe[k - 1] : 0u;
+        s.piece.assign(t + p0, t + pe[k]);
+        s.id = ids[k];
+        s.surface.assign(inputs[i].data() + b[k], e[k] - b[k]);
+        s.begin = b[k];
+        s.end = e[k];
+      }
+    }
+  });
+  return util::OkStatus();
+}
+
+util::Status SentencePieceProcessor::EncodeWithOffsets(std::string_view input, std::vector<PieceSpan> *pieces) const {
+  if (!engine_) return status();
+  if (!pieces) return Internal("output container is null");
+  std::vector<std::vector<PieceSpan>> v;
+  const auto st = EncodeWithOffsets(std::vector<std::string_view>{input}, &v);
+  if (!st.ok()) return st;
+  *pieces = std::move(v[0]);
+  return util::OkStatus();
+}
+
 namespace {
 // list j of a packed pieces result (sep = -1) as strings
 std::vector<std::string> PieceList(const char *text, const uint64_t *to, const uint32_t *ends, const uint64_t *ido,

@@ -125,6 +125,27 @@ class SentencePieceProcessor {
                                         int sep, const char **text, const uint64_t **text_offsets,
                                         const uint32_t **piece_end, const uint64_t **id_offsets) const;
 
+  // ---- Encode with offsets: what SentencePieceText (EncodeAsImmutableProto) holds per token, without protobuf.
+  //      begin / end are byte offsets into the input (the reference's, before any ConvertToUnicodeSpans), surface is
+  //      input[begin, end); the extra options apply as for EncodeAsPieces: bos / eos entries get (0, 0) and
+  //      (size, size), reverse reverses the offsets with the pieces, unk replaces the piece string only. ----
+  struct PieceSpan {
+    std::string piece;
+    int id = 0;
+    std::string surface;
+    uint32_t begin = 0, end = 0;
+  };
+  util::Status EncodeWithOffsets(std::string_view input, std::vector<PieceSpan> *pieces) const;
+  // one device call for all sentences
+  util::Status EncodeWithOffsets(const std::vector<std::string_view> &inputs,
+                                 std::vector<std::vector<PieceSpan>> *pieces) const;
+  // zero-copy form, the layout of spm_encode_offsets with the pieces (sep = -1): token k of sentence i is ids[k] with
+  // begin[k] / end[k] relative to offsets[i], for k in [id_offsets[i], id_offsets[i+1]); owned by the engine until the
+  // next call
+  util::Status EncodeOffsetsPacked(const char *bytes, const uint64_t *offsets, size_t n, const int32_t **ids,
+                                   const uint64_t **id_offsets, const uint32_t **begin, const uint32_t **end,
+                                   const char **text, const uint64_t **text_offsets, const uint32_t **piece_end) const;
+
   // ---- Normalize (sentencepiece_processor.h:621-631): the model's normalizer, on the device (spm_normalize).
   //      norm_to_orig as the reference returns it: empty for empty input and for input that is all heading
   //      whitespace, else one entry per normalized byte and one for the end. ----

@@ -106,6 +106,106 @@ def unicode_alignment(orig, orig_offs, norm, norm_offs, n2o):
     return offsets, values
 
 
+def unicode_spans(buf, offs, begin, end, id_offsets):
+    """ConvertToUnicodeSpans (sentencepiece_processor.cc:63-91) of spm_encode_offsets' byte offsets, for a whole batch ->
+    (begin, end) int64 character indices.  Each offset is clipped to [0, len(input)] and mapped through char_index; an
+    empty input keeps its offsets, which are all 0, as the reference does.  A malformed input whose last character's
+    lead byte claims more bytes than remain ends at its length instead of reading past it."""
+    offs = np.asarray(offs, np.int64)
+    n = len(offs) - 1
+    ci = char_index(buf, offs)
+    sent = np.repeat(np.arange(n), np.diff(np.asarray(id_offsets, np.int64)))
+    lens = np.diff(offs)[sent]
+    base = (offs[:-1] - offs[0] + np.arange(n))[sent]
+
+    def conv(x):
+        return ci[base + np.minimum(np.asarray(x, np.int64), lens)]
+    return conv(begin), conv(end)
+
+
+class ImmutableSentencePiece:
+    """One token of an ImmutableSentencePieceText: piece, id, surface (input[begin:end]), begin, end (read-only)."""
+    __slots__ = ("_piece", "_id", "_surface", "_begin", "_end")
+
+    def __init__(self, piece, id, surface, begin, end):
+        self._piece, self._id, self._surface, self._begin, self._end = piece, id, surface, begin, end
+
+    piece_as_bytes = property(lambda self: self._piece)
+    piece = property(lambda self: self._piece.decode("utf-8", errors="replace"))
+    surface_as_bytes = property(lambda self: self._surface)
+    surface = property(lambda self: self._surface.decode("utf-8", errors="replace"))
+    id = property(lambda self: self._id)
+    begin = property(lambda self: self._begin)
+    end = property(lambda self: self._end)
+
+    def __eq__(self, other):
+        if not isinstance(other, ImmutableSentencePiece):
+            return NotImplemented
+        return (self.piece, self.id, self.surface, self.begin, self.end) == \
+            (other.piece, other.id, other.surface, other.begin, other.end)
+
+    def __hash__(self):
+        return hash((self._piece, self._id, self._surface, self._begin, self._end))
+
+    def __repr__(self):
+        return f'piece: "{self.piece}"\nid: {self.id}\nsurface: "{self.surface}"\nbegin: {self.begin}\nend: {self.end}\n'
+
+
+class ImmutableSentencePieceText:
+    """EncodeAsImmutableProto's result for one input: text, pieces (a tuple of ImmutableSentencePiece); len(),
+    indexing and iteration go over the pieces (read-only)."""
+    __slots__ = ("_text", "_pieces")
+
+    def __init__(self, text, pieces):
+        self._text, self._pieces = text, tuple(pieces)
+
+    text_as_bytes = property(lambda self: self._text)
+    text = property(lambda self: self._text.decode("utf-8", errors="replace"))
+    pieces = property(lambda self: self._pieces)
+
+    def __len__(self):
+        return len(self._pieces)
+
+    def __getitem__(self, k):
+        return self._pieces[k]
+
+    def __iter__(self):
+        return iter(self._pieces)
+
+    def __eq__(self, other):
+        if not isinstance(other, ImmutableSentencePieceText):
+            return NotImplemented
+        return self.text_as_bytes == other.text_as_bytes and self.pieces == other.pieces
+
+    def __hash__(self):
+        return hash((self._text, self._pieces))
+
+    def __repr__(self):
+        return "".join(f"pieces {{\n{p!r}}}\n" for p in self._pieces) + f'text: "{self.text}"\n'
+
+
+def immutable_protos(items, buf, offs, r):
+    """The ImmutableSentencePieceText of every input from spm_encode_offsets' result r (with pieces): offsets in
+    characters (unicode_spans), surfaces cut from the input by byte offsets."""
+    raw = bytes(np.ascontiguousarray(buf, np.uint8))
+    text = bytes(r["text"])
+    ob = np.asarray(offs, np.int64) - int(offs[0])
+    ido, to = r["id_offsets"].tolist(), r["text_offsets"].tolist()
+    cb, ce = unicode_spans(buf, offs, r["begin"], r["end"], r["id_offsets"])
+    ids, pe, bb, be = r["ids"].tolist(), r["piece_end"].tolist(), r["begin"].tolist(), r["end"].tolist()
+    cb, ce = cb.tolist(), ce.tolist()
+    out = []
+    for i in range(len(items)):
+        s = raw[ob[i]:ob[i + 1]]
+        t = text[to[i]:to[i + 1]]
+        pieces, prev = [], 0
+        for k in range(ido[i], ido[i + 1]):
+            pieces.append(ImmutableSentencePiece(t[prev:pe[k]], ids[k], s[bb[k]:be[k]], cb[k], ce[k]))
+            prev = pe[k]
+        out.append(ImmutableSentencePieceText(s, pieces))
+    return out
+
+
 def pack_sentences(sentences):
     """list[bytes|str] -> (uint8[total], uint64[n+1])"""
     bs = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in sentences]
@@ -239,6 +339,33 @@ class Engine:
         self._check(self._lib.spm_encode_pieces(self._h, buf.ctypes.data, offs.ctypes.data, n, *self._unk(unk_piece), sep,
                                                 *[ctypes.byref(x) for x in p]))
         return self._pieces_result(p, n)
+
+    def encode_offsets(self, buf, offs, eos_id=-1, unk_piece=None, sep=-1, pieces=True):
+        """spm_encode_offsets: the ids of every token and its byte range in the input, the encode frame applied ->
+        dict(ids int32[], id_offsets uint64[n+1], begin uint32[], end uint32[]), begin / end relative to the sentence's
+        start; frame entries equal to eos_id get (len, len), the others (0, 0).  pieces: also text, text_offsets and
+        piece_end, exactly as encode_pieces with the same unk_piece and sep."""
+        n = len(offs) - 1
+        buf = np.ascontiguousarray(buf, dtype=np.uint8)
+        offs = np.ascontiguousarray(offs, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(7)]
+        self._check(self._lib.spm_encode_offsets(self._h, buf.ctypes.data, offs.ctypes.data, n, eos_id, *self._unk(unk_piece),
+                                                 sep, *[ctypes.byref(x) for x in p[:4]],
+                                                 *([ctypes.byref(x) for x in p[4:]] if pieces else [None] * 3)))
+        ido = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+        tot = int(ido[n])
+
+        def arr(ptr, ct):
+            return np.ctypeslib.as_array(ctypes.cast(ptr, ctypes.POINTER(ct)), (max(tot, 1),))[:tot].copy()
+        r = dict(ids=arr(p[0], ctypes.c_int32), id_offsets=ido, begin=arr(p[2], ctypes.c_uint32),
+                 end=arr(p[3], ctypes.c_uint32))
+        if pieces:
+            to = np.ctypeslib.as_array(ctypes.cast(p[5], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+            tt = int(to[n])
+            r["text"] = np.ctypeslib.as_array(ctypes.cast(p[4], ctypes.POINTER(ctypes.c_uint8)), (max(tt, 1),))[:tt].copy()
+            r["text_offsets"] = to
+            r["piece_end"] = arr(p[6], ctypes.c_uint32)
+        return r
 
     @staticmethod
     def _pieces_result(p, lists):
@@ -568,11 +695,35 @@ class SentencePieceProcessor:
         out = split_pieces(r["text"], r["text_offsets"], r["piece_end"], r["id_offsets"])
         return out[0] if single else out
 
+    # sentencepiece.i _EncodeAsImmutableProto (:420-434): SetEncodeExtraOptions' options apply, then ConvertToUnicodeSpans
+    def EncodeAsImmutableProto(self, input, enable_sampling=False, nbest_size=-1, alpha=0.1, add_bos=False,
+                               add_eos=False, reverse=False, emit_unk_piece=False):
+        """One str / bytes or a list of them -> ImmutableSentencePieceText (or a list): every token's piece, id,
+        surface and begin / end in characters of the input.  add_bos / add_eos / reverse / emit_unk_piece are refused
+        as in the reference (RewriteIds, sentencepiece.i:167-182); sampled protos are not offered."""
+        self._require()
+        if add_bos or add_eos or reverse or emit_unk_piece:
+            raise RuntimeError("add_bos, add_eos, reverse, and emit_unk_piece is not supported in proto API")
+        if enable_sampling:
+            raise NotImplementedError("EncodeAsImmutableProto with enable_sampling is not offered by the device path")
+        single = not isinstance(input, list)
+        items = [input] if single else input
+        buf, offs = pack_sentences(items)
+        unk = self._pieces_frame(False, False, False, False)
+        r = self._engine.encode_offsets(buf, offs, eos_id=self._specials()["eos_id"], unk_piece=unk)
+        out = immutable_protos(items, buf, offs, r)
+        return out[0] if single else out
+
+    encode_as_immutable_proto = EncodeAsImmutableProto
+
     def encode(self, input, out_type=int, enable_sampling=False, nbest_size=-1, alpha=0.1, add_bos=False, add_eos=False,
                reverse=False, emit_unk_piece=False):
-        """python/src/sentencepiece/__init__.py Encode: out_type int | str; enable_sampling uses SampleEncode.
-        add_bos / add_eos / reverse apply after SetEncodeExtraOptions' options, in the order reverse, bos, eos."""
+        """python/src/sentencepiece/__init__.py Encode: out_type int | str | 'immutable_proto'; enable_sampling uses
+        SampleEncode.  add_bos / add_eos / reverse apply after SetEncodeExtraOptions' options, in the order reverse,
+        bos, eos."""
         kw = dict(add_bos=add_bos, add_eos=add_eos, reverse=reverse, emit_unk_piece=emit_unk_piece)
+        if out_type == "immutable_proto":
+            return self.EncodeAsImmutableProto(input, enable_sampling, nbest_size, alpha, **kw)
         if enable_sampling:
             if out_type is int:
                 return self.SampleEncodeAsIds(input, nbest_size, alpha, **kw)
