@@ -330,6 +330,18 @@ int spm_sample_encode_and_score_pieces(spm_engine *e, const char *bytes, const u
 int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
                    const uint64_t **text_offsets);
 
+/* Replaces SentencePieceProcessor::Decode(const std::vector<int>& ids, SentencePieceText*) /
+ * DecodeIdsAsImmutableProto (src/sentencepiece_processor.cc:766-925) for n id lists: the text and where every token's
+ * surface lies in it.  text / text_offsets are byte for byte what spm_decode_ids returns for the same lists;
+ * tok_end[k - id_offsets[0]] is the end of token k's surface, relative to text_offsets[i] of its list.  The surfaces
+ * tile the text in token order (SetSurface, :822-828), so token k begins where token k-1 ends and the first token of a
+ * list at 0: a CONTROL token's surface is empty, an UNKNOWN token's is unk_surface, and in a run of BYTE pieces the
+ * first c-1 tokens of a valid c-byte character get an empty surface and the last one the whole character, while an
+ * invalid byte's token gets U+FFFD.  Outputs are engine-owned pinned memory, valid until the next call.  Arguments,
+ * errors and refusals are those of spm_decode_ids; n == 0 succeeds. */
+int spm_decode_offsets(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
+                       const uint64_t **text_offsets, const uint32_t **tok_end);
+
 /* Decode of device-resident id rows, e.g. a generation output tensor [n, >= row_len] still on the GPU: row i starts at
  * element i * row_stride of d_ids (int32 when id_bytes == 4, int64 when 8 -- a cast of int64 ids to int32 would wrap
  * large values silently) and holds min(row_len, d_lengths[i]) ids (row_len when d_lengths is NULL; a negative length is

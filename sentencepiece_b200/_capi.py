@@ -18,6 +18,7 @@ EXPORTS = [
     "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
     "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
     "spm_encode_ids_device_padded", "spm_decode_ids_device", "spm_normalize", "spm_encode_offsets",
+    "spm_decode_offsets",
 ]
 
 # spm_normalize: the n2o entry of a sentence whose reference norm_to_orig is empty
@@ -91,6 +92,7 @@ def load():
     L.spm_set_random_seed.argtypes = [vp, ctypes.c_uint32]
     L.spm_sample_encode_ids.argtypes = [vp, vp, vp, sz, ctypes.c_int, ctypes.c_float, P(vp), P(vp)]
     L.spm_decode_ids.argtypes = [vp, vp, vp, sz, P(vp), P(vp)]
+    L.spm_decode_offsets.argtypes = [vp, vp, vp, sz, P(vp), P(vp), P(vp)]
     L.spm_engine_set_unk_surface.argtypes = [vp, cp, sz]
     L.spm_calculate_entropy.argtypes = [vp, vp, vp, sz, ctypes.c_float, P(vp)]
     L.spm_sample_encode_and_score.argtypes = [vp, vp, vp, sz, ctypes.c_int, ctypes.c_float, ctypes.c_int, ctypes.c_int,

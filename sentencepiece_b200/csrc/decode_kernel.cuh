@@ -51,6 +51,10 @@ struct KDecode {
   // range is also stored whole, sign-extended, at cursor[1]
   unsigned long long row_stride;
   const uint32_t *row_len;  // [n]
+  // ENDS mode (decode_warp_kernel<int32_t, false, true>): tok_end[k] = the end of id k's surface in its list's text, for
+  // every k in [id_offsets[0], id_offsets[n]) (indexed like ids).  The surfaces tile the text in token order
+  // (SetSurface, :822-828), so the end of token k-1 is the begin of token k.
+  uint32_t *tok_end;
 };
 
 // IsValidDecodeUTF8 (src/util.h:173-176 over DecodeUTF8, src/util.cc:51-84): bytes consumed by one valid character
@@ -75,8 +79,10 @@ __device__ __forceinline__ uint32_t dec_utf8_valid(const uint32_t *b, uint32_t a
 }
 
 // Sequential restatement for one list (lists with BYTE pieces); WRITE = false only counts.  IdT: the ids' type (every
-// id has been checked to lie in [0, vocab) before).
-template <bool WRITE, typename IdT = int32_t>
+// id has been checked to lie in [0, vocab) before).  ENDS (with WRITE): also the end of every token's surface, as
+// ProcessBytePieces sets them: the first c-1 byte tokens of a valid c-byte character end where they begin and the last
+// one after the character, an invalid byte's token after its U+FFFD.
+template <bool WRITE, typename IdT = int32_t, bool ENDS = false>
 __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, unsigned long long a, uint32_t L, uint8_t *out) {
   const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   uint32_t n = 0;  // bytes of text so far
@@ -100,9 +106,11 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
       if (c == 0) {
         if (WRITE) { out[n] = 0xEF; out[n + 1] = 0xBF; out[n + 2] = 0xBD; }
         n += 3;
+        if constexpr (ENDS) D.tok_end[a + i] = n;
         i += 1;
       } else {
         if (WRITE) for (uint32_t k = 0; k < c; ++k) out[n + k] = static_cast<uint8_t>(b[k]);
+        if constexpr (ENDS) for (uint32_t k = 0; k < c; ++k) D.tok_end[a + i + k] = k + 1 == c ? n + c : n;
         n += c;
         i += c;
       }
@@ -120,6 +128,7 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
     len -= skip;
     if (WRITE) for (uint32_t k = 0; k < len; ++k) out[n + k] = __ldg(D.dec_bytes + off + skip + k);
     n += len;
+    if constexpr (ENDS) D.tok_end[a + i] = n;
     bos_ws_seen = has_bos_ws;
     ++i;
   }
@@ -127,11 +136,12 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
 }
 
 // IdT, ROWS: the ids are int32 or int64, and list i is either [id_offsets[i], id_offsets[i+1]) (packed) or row_len[i]
-// ids from i * row_stride (rows of a padded [n, row_stride] tensor).  Template flags, so that the packed int32
-// instantiation keeps its code.
-template <typename IdT = int32_t, bool ROWS = false>
+// ids from i * row_stride (rows of a padded [n, row_stride] tensor).  ENDS: also write D.tok_end (packed lists only).
+// Template flags, so that the packed int32 instantiation keeps its code.
+template <typename IdT = int32_t, bool ROWS = false, bool ENDS = false>
 __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
   static_assert(ROWS || sizeof(IdT) == 4, "packed lists are int32");
+  static_assert(!(ROWS && ENDS), "token ends are written for packed lists only");
   const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
@@ -182,7 +192,7 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
         total = decode_list_sequential<false, IdT>(D, a, L, nullptr);
         pos = atomicAdd(D.cursor, static_cast<unsigned long long>(total));
         if (pos + total > D.tmp_cap) { atomicOr(D.status + 2, 1u); total = 0; }
-        else decode_list_sequential<true, IdT>(D, a, L, D.tmp + pos);
+        else decode_list_sequential<true, IdT, ENDS>(D, a, L, D.tmp + pos);
         D.sent_start[sent] = pos;
         D.sent_count[sent] = total;
       }
@@ -221,6 +231,7 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
           if (lane >= static_cast<uint32_t>(d)) incl += v;
         }
         if (pass == 1) {
+          if constexpr (ENDS) if (valid) D.tok_end[a + t] = run + incl;
           uint8_t *dst = D.tmp + pos + run + (incl - len);
           const uint8_t *src = D.dec_bytes + off + skip;
           const uint32_t mx = __reduce_max_sync(0xFFFFFFFFu, len);

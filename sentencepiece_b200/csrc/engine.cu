@@ -359,8 +359,10 @@ struct spm_engine {
   DevBuf<uint8_t> d_dec_bytes, d_dec_tmp, d_dec_text;
   DevBuf<int32_t> d_dec_ids;
   DevBuf<unsigned long long> d_dec_text_offsets;
+  DevBuf<uint32_t> d_dec_tok_end;  // spm_decode_offsets: decode_warp_kernel's ENDS mode
   PinBuf<char> h_dec_text;
   PinBuf<uint64_t> h_dec_text_offsets;
+  PinBuf<uint32_t> h_dec_tok_end;
   bool dec_ready = false;
   int ensure_decode_tables();
   // decode_warp_kernel's arguments for n id lists (ids indexed by the values of id_offsets), results in d_dec_tmp
@@ -401,16 +403,19 @@ struct spm_engine {
   DevBuf<int32_t> p_dec_ids[2];
   DevBuf<uint8_t> p_dec_text[2];
   DevBuf<unsigned long long> p_dec_toff[2];
+  DevBuf<uint32_t> p_dec_tok_end[2];
   PinBuf<uint8_t> h_stage[2];
+  // tok_end != NULL: the ENDS mode, and the token ends are copied back too
   int decode_host_pipelined(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
-                            const uint64_t **text_offsets);
+                            const uint64_t **text_offsets, const uint32_t **tok_end);
   DevBuf<uint32_t> d_row_len;  // spm_decode_ids_device: the length of every row
   // The decode of n lists on st after the caller's checks: launch(tmp_cap) queues decode_warp_kernel, which is run again
   // with the exact temporary size if it overflowed; then the text is put into list order and copied into the pinned
-  // results, and the call waits for it.  rows: launch runs the ROWS mode (for decode_error).
+  // results, and the call waits for it.  rows: launch runs the ROWS mode (for decode_error).  tok_end != NULL: launch
+  // runs the ENDS mode into d_dec_tok_end, whose n_tok entries are copied back too.
   template <typename Launch>
   int decode_text(uint32_t n, unsigned long long tmp_cap, bool rows, cudaStream_t st, Launch &&launch, const char **text,
-                  const uint64_t **text_offsets) {
+                  const uint64_t **text_offsets, const uint32_t **tok_end = nullptr, uint64_t n_tok = 0) {
     CUDA_TRY(d_sent_start.ensure(n));
     CUDA_TRY(d_sent_count.ensure(n));
     CUDA_TRY(d_dec_text_offsets.ensure(n + 1));
@@ -441,11 +446,16 @@ struct spm_engine {
     CUDA_TRY(h_dec_text.ensure(tot + 1));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_dec_text.p, d_dec_text.p, tot, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(h_dec_text_offsets.p, d_dec_text_offsets.p, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+    if (tok_end) {
+      CUDA_TRY(h_dec_tok_end.ensure(n_tok + 1));
+      if (n_tok) CUDA_TRY(cudaMemcpyAsync(h_dec_tok_end.p, d_dec_tok_end.p, n_tok * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    }
     CUDA_TRY(cudaStreamSynchronize(st));
-    last_d2h = tot + (n + 1) * sizeof(uint64_t);
+    last_d2h = tot + (n + 1) * sizeof(uint64_t) + (tok_end ? n_tok * sizeof(uint32_t) : 0);
     h_dec_text.p[tot] = 0;
     *text = h_dec_text.p;
     *text_offsets = h_dec_text_offsets.p;
+    if (tok_end) *tok_end = h_dec_tok_end.p;
     return SPM_OK;
   }
   // EncodeAsPieces (K9): per-id piece bytes, built on first use; the raw ids of the lane kernels, the unknown-surface
@@ -1941,7 +1951,7 @@ void parallel_memcpy(void *dst, const void *src, size_t bytes) {
 // Decode of a large host batch: chunks of id lists flow through H2D (staged when the caller's memory is pageable),
 // decode + scan + gather, and D2H of the text on three streams; inputs and outputs are double buffered.
 int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
-                                      const uint64_t **text_offsets) {
+                                      const uint64_t **text_offsets, const uint32_t **tok_end) {
   { const int rc = ensure_copy_streams(); if (rc) return rc; }
   cudaStream_t st = stream;
   const TraceClock trace;
@@ -1955,9 +1965,11 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
     CUDA_TRY(p_dec_ids[k].ensure(max_ids + 1));
     CUDA_TRY(p_offsets[k].ensure(chunk + 1));
     CUDA_TRY(p_dec_toff[k].ensure(chunk + 1));
+    if (tok_end) CUDA_TRY(p_dec_tok_end[k].ensure(max_ids + 1));
     if (!pinned_in) CUDA_TRY(h_stage[k].ensure(max_ids * sizeof(int32_t) + 64));
   }
   CUDA_TRY(h_dec_text_offsets.ensure(n + 1));
+  if (tok_end) CUDA_TRY(h_dec_tok_end.ensure(total_ids + 1));
   CUDA_TRY(h_dec_text.ensure(std::max<size_t>(h_dec_text.cap, total_ids * 5 + 16 * n + 4096)));
   CUDA_TRY(d_sent_start.ensure(chunk));
   CUDA_TRY(d_sent_count.ensure(chunk));
@@ -1999,7 +2011,13 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
       CUDA_TRY(cudaMemsetAsync(d_ctrl64.p, 0, 8 * sizeof(unsigned long long), st));
       CUDA_TRY(cudaEventRecord(ev[0], st));
       const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (m + 7) / 8));
-      decode_warp_kernel<<<grid, 256, 0, st>>>(decode_args(p_dec_ids[k].p - id_offsets[lo], p_offsets[k].p, m, tmp_cap));
+      KDecode D = decode_args(p_dec_ids[k].p - id_offsets[lo], p_offsets[k].p, m, tmp_cap);
+      if (tok_end) {
+        D.tok_end = p_dec_tok_end[k].p - id_offsets[lo];
+        decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D);
+      } else {
+        decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+      }
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaEventRecord(ev[1], st));
       ++last_launches;
@@ -2033,6 +2051,9 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
     CUDA_TRY(cudaStreamWaitEvent(s_d2h, ev_out[k], 0));
     if (tot) CUDA_TRY(cudaMemcpyAsync(h_dec_text.p + text_base, p_dec_text[k].p, tot, cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaMemcpyAsync(h_dec_text_offsets.p + lo, p_dec_toff[k].p, (m + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, s_d2h));
+    if (tok_end && cnt)
+      CUDA_TRY(cudaMemcpyAsync(h_dec_tok_end.p + (id_offsets[lo] - id_offsets[0]), p_dec_tok_end[k].p, cnt * sizeof(uint32_t),
+                               cudaMemcpyDeviceToHost, s_d2h));
     CUDA_TRY(cudaEventRecord(ev_d2h[k], s_d2h));
     text_base += tot;
   }
@@ -2046,9 +2067,10 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
   last_main_ms = main_ms;
   last_ms = main_ms + all_ms;
   last_h2d = total_ids * sizeof(int32_t) + (n + C) * sizeof(uint64_t);
-  last_d2h = text_base + (n + C) * sizeof(uint64_t);
+  last_d2h = text_base + (n + C) * sizeof(uint64_t) + (tok_end ? total_ids * sizeof(uint32_t) : 0);
   *text = h_dec_text.p;
   *text_offsets = h_dec_text_offsets.p;
+  if (tok_end) *tok_end = h_dec_tok_end.p;
   return SPM_OK;
 }
 
@@ -2640,8 +2662,10 @@ int spm_engine_set_unk_surface(spm_engine *e, const char *surface, size_t bytes)
   return SPM_OK;
 }
 
-int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
-                   const uint64_t **text_offsets) {
+namespace {
+// spm_decode_ids and spm_decode_offsets: tok_end == NULL decodes the text only
+int decode_host(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
+                const uint64_t **text_offsets, const uint32_t **tok_end) {
   if (!e || !id_offsets || !text || !text_offsets) return SPM_ERR_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   auto set_error = [&](const std::string &m) { e->set_error(m); };
@@ -2657,7 +2681,7 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
   }
   CUDA_TRY(cudaSetDevice(e->device));
   { const int rc = e->ensure_decode_tables(); if (rc) return rc; }
-  if (n >= e->pipeline_min_sentences) return e->decode_host_pipelined(ids, id_offsets, n, text, text_offsets);
+  if (n >= e->pipeline_min_sentences) return e->decode_host_pipelined(ids, id_offsets, n, text, text_offsets, tok_end);
   cudaStream_t st = e->stream;
   e->last_launches = 0;
   CUDA_TRY(e->h_dec_text_offsets.ensure(n + 1));
@@ -2666,6 +2690,10 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
     e->h_dec_text_offsets.p[0] = 0;
     *text = e->h_dec_text.p;
     *text_offsets = e->h_dec_text_offsets.p;
+    if (tok_end) {
+      CUDA_TRY(e->h_dec_tok_end.ensure(1));
+      *tok_end = e->h_dec_tok_end.p;
+    }
     return SPM_OK;
   }
   CUDA_TRY(e->d_dec_ids.ensure(total_ids + 1));
@@ -2675,14 +2703,32 @@ int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets
   e->last_h2d = total_ids * sizeof(int32_t) + (n + 1) * sizeof(uint64_t);
   const uint32_t n32 = static_cast<uint32_t>(n);
   const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  if (tok_end) CUDA_TRY(e->d_dec_tok_end.ensure(total_ids + 1));
   SPM_TRY(e->decode_text(n32, total_ids * 6 + 16ull * n + (1u << 20), false, st,  // retried with the exact size on overflow
                          [&](unsigned long long tmp_cap) {
-                           decode_warp_kernel<<<grid, 256, 0, st>>>(
-                               e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap));
+                           KDecode D = e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap);
+                           if (tok_end) {
+                             D.tok_end = e->d_dec_tok_end.p - base;
+                             decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D);
+                           } else {
+                             decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+                           }
                          },
-                         text, text_offsets));
+                         text, text_offsets, tok_end, total_ids));
   finish_timing(e);
   return SPM_OK;
+}
+}  // namespace
+
+int spm_decode_ids(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
+                   const uint64_t **text_offsets) {
+  return decode_host(e, ids, id_offsets, n, text, text_offsets, nullptr);
+}
+
+int spm_decode_offsets(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
+                       const uint64_t **text_offsets, const uint32_t **tok_end) {
+  if (!tok_end) return SPM_ERR_ARG;
+  return decode_host(e, ids, id_offsets, n, text, text_offsets, tok_end);
 }
 
 int spm_decode_ids_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, uint64_t row_stride, size_t n,

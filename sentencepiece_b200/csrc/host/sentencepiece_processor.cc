@@ -261,6 +261,13 @@ std::string SentencePieceProcessor::DecodeIds(const std::vector<int> &ids) const
   return out;
 }
 
+util::Status SentencePieceProcessor::DecodeOffsetsPacked(const int32_t *ids, const uint64_t *id_offsets, size_t n,
+                                                         const char **text, const uint64_t **text_offsets,
+                                                         const uint32_t **tok_end) const {
+  if (!engine_) return status();
+  return FromEngine(engine_, spm_decode_offsets(engine_, ids, id_offsets, n, text, text_offsets, tok_end));
+}
+
 namespace {
 // runs fn(lo, hi) over [0, n) on a few host threads (the container conversions around a batch call are the only
 // per-sentence host work left; the reference's Python layer uses a thread pool for the same reason,
@@ -472,6 +479,60 @@ util::Status SentencePieceProcessor::EncodeWithOffsets(std::string_view input, s
   std::vector<std::vector<PieceSpan>> v;
   const auto st = EncodeWithOffsets(std::vector<std::string_view>{input}, &v);
   if (!st.ok()) return st;
+  *pieces = std::move(v[0]);
+  return util::OkStatus();
+}
+
+util::Status SentencePieceProcessor::DecodeWithOffsets(const std::vector<std::vector<int>> &ids,
+                                                       std::vector<std::string> *text,
+                                                       std::vector<std::vector<PieceSpan>> *pieces) const {
+  if (!engine_) return status();
+  if (!text || !pieces) return Internal("output container is null");
+  text->clear();
+  pieces->clear();
+  std::vector<int32_t> packed;
+  std::vector<uint64_t> offs(1, 0);
+  for (const auto &l : ids) {
+    packed.insert(packed.end(), l.begin(), l.end());
+    offs.push_back(packed.size());
+  }
+  const char *t;
+  const uint64_t *to;
+  const uint32_t *te;
+  const auto st = DecodeOffsetsPacked(packed.data(), offs.data(), ids.size(), &t, &to, &te);
+  if (!st.ok()) return st;
+  text->resize(ids.size());
+  pieces->resize(ids.size());
+  ParallelFor(ids.size(), [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; ++i) {
+      std::string &s = (*text)[i];
+      s.assign(t + to[i], t + to[i + 1]);
+      auto &v = (*pieces)[i];
+      v.resize(offs[i + 1] - offs[i]);
+      uint32_t begin = 0;
+      for (uint64_t k = offs[i]; k < offs[i + 1]; ++k) {
+        PieceSpan &p = v[k - offs[i]];
+        p.id = packed[k];
+        p.piece = IdToPiece(p.id);
+        p.begin = begin;
+        p.end = te[k];
+        p.surface.assign(s, p.begin, p.end - p.begin);
+        begin = p.end;
+      }
+    }
+  });
+  return util::OkStatus();
+}
+
+util::Status SentencePieceProcessor::DecodeWithOffsets(const std::vector<int> &ids, std::string *text,
+                                                       std::vector<PieceSpan> *pieces) const {
+  if (!engine_) return status();
+  if (!text || !pieces) return Internal("output container is null");
+  std::vector<std::string> t;
+  std::vector<std::vector<PieceSpan>> v;
+  const auto st = DecodeWithOffsets(std::vector<std::vector<int>>{ids}, &t, &v);
+  if (!st.ok()) return st;
+  *text = std::move(t[0]);
   *pieces = std::move(v[0]);
   return util::OkStatus();
 }

@@ -167,6 +167,19 @@ class SentencePieceProcessor {
   util::Status Decode(const std::vector<std::vector<int>> &ids, std::vector<std::string> *detokenized) const;
   std::string DecodeIds(const std::vector<int> &ids) const;
 
+  // ---- Decode with offsets: what SentencePieceText (DecodeIdsAsImmutableProto) holds per token, without protobuf.
+  //      piece is IdToPiece(id), surface is text[begin, end) (byte offsets into the decoded text, before any
+  //      ConvertToUnicodeSpans); the surfaces tile the text in token order.  Errors as Decode. ----
+  util::Status DecodeWithOffsets(const std::vector<int> &ids, std::string *text, std::vector<PieceSpan> *pieces) const;
+  // one device call for all lists
+  util::Status DecodeWithOffsets(const std::vector<std::vector<int>> &ids, std::vector<std::string> *text,
+                                 std::vector<std::vector<PieceSpan>> *pieces) const;
+  // zero-copy form, the layout of spm_decode_offsets: list i is text[text_offsets[i] .. text_offsets[i+1]), token k of it
+  // ends at tok_end[k - id_offsets[0]] relative to text_offsets[i] and begins where token k-1 ends (0 for the first
+  // token of a list); owned by the engine until the next call
+  util::Status DecodeOffsetsPacked(const int32_t *ids, const uint64_t *id_offsets, size_t n, const char **text,
+                                   const uint64_t **text_offsets, const uint32_t **tok_end) const;
+
   // ---- vocabulary accessors used by callers of the encode path ----
   int GetPieceSize() const;
   int PieceToId(std::string_view piece) const;

@@ -206,6 +206,28 @@ def immutable_protos(items, buf, offs, r):
     return out
 
 
+def decode_protos(pieces, ids, id_offsets, text, text_offsets, tok_end):
+    """The ImmutableSentencePieceText of every list from spm_decode_offsets' result: .text is the decoded text, piece
+    is pieces[id], surface is text[begin:end], begin / end in characters of the text (unicode_spans)."""
+    raw = bytes(np.ascontiguousarray(text, np.uint8))
+    ido = np.asarray(id_offsets, np.int64)
+    ido = ido - ido[0]
+    te = np.asarray(tok_end, np.int64)
+    tb = te.copy()  # each token begins where the one before it in its list ends, the first one at 0
+    if len(tb):
+        tb[1:] = te[:-1]
+        tb[ido[:-1][ido[:-1] < ido[1:]]] = 0
+    cb, ce = unicode_spans(text, text_offsets, tb, te, ido)
+    to, ido = np.asarray(text_offsets, np.int64).tolist(), ido.tolist()
+    ids, tb, te, cb, ce = np.asarray(ids).tolist(), tb.tolist(), te.tolist(), cb.tolist(), ce.tolist()
+    out = []
+    for i in range(len(to) - 1):
+        t = raw[to[i]:to[i + 1]]
+        out.append(ImmutableSentencePieceText(t, [ImmutableSentencePiece(pieces[ids[k]], ids[k], t[tb[k]:te[k]], cb[k], ce[k])
+                                                  for k in range(ido[i], ido[i + 1])]))
+    return out
+
+
 def pack_sentences(sentences):
     """list[bytes|str] -> (uint8[total], uint64[n+1])"""
     bs = [s.encode("utf-8") if isinstance(s, str) else bytes(s) for s in sentences]
@@ -444,6 +466,21 @@ class Engine:
         t = np.frombuffer(ctypes.string_at(text, tot), dtype=np.uint8) if tot else np.zeros(0, np.uint8)
         return t, o
 
+    def decode_offsets(self, ids, id_offsets):
+        """spm_decode_offsets: Decode of packed id lists with every token's surface -> (text uint8[], text_offsets
+        uint64[n+1], tok_end uint32[]): text and text_offsets as decode_packed, tok_end[k - id_offsets[0]] the end of
+        token k's surface relative to its list's text; token k begins where token k-1 of its list ends, the first at 0."""
+        n = len(id_offsets) - 1
+        ids = np.ascontiguousarray(ids, dtype=np.int32)
+        ido = np.ascontiguousarray(id_offsets, dtype=np.uint64)
+        p = [ctypes.c_void_p() for _ in range(3)]
+        self._check(self._lib.spm_decode_offsets(self._h, ids.ctypes.data, ido.ctypes.data, n, *[ctypes.byref(x) for x in p]))
+        to = np.ctypeslib.as_array(ctypes.cast(p[1], ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).copy()
+        tt, tot = int(to[n]), int(ido[n]) - int(ido[0])
+        text = np.ctypeslib.as_array(ctypes.cast(p[0], ctypes.POINTER(ctypes.c_uint8)), (max(tt, 1),))[:tt].copy()
+        te = np.ctypeslib.as_array(ctypes.cast(p[2], ctypes.POINTER(ctypes.c_uint32)), (max(tot, 1),))[:tot].copy()
+        return text, to, te
+
     def set_random_seed(self, seed):
         self._check(self._lib.spm_set_random_seed(self._h, seed))
 
@@ -595,6 +632,17 @@ class Engine:
         return [raw[o[i]:o[i + 1]].decode("utf-8", errors="replace") for i in range(n)]
 
 
+def _id_lists(input):
+    """One id list or a list of id lists -> (single, (ids int32[], id_offsets uint64[n+1]))"""
+    single = len(input) == 0 or not isinstance(input[0], (list, tuple, np.ndarray))
+    lists = [input] if single else list(input)
+    ido = np.zeros(len(lists) + 1, dtype=np.uint64)
+    if lists:
+        ido[1:] = np.cumsum([len(x) for x in lists], dtype=np.uint64)
+    ids = np.concatenate([np.asarray(x, dtype=np.int32) for x in lists]) if int(ido[-1]) else np.zeros(0, np.int32)
+    return single, (ids, ido)
+
+
 class SentencePieceProcessor:
     """Mirror of the reference's encode API (same method names / argument meaning as
     python/src/sentencepiece/__init__.py and src/sentencepiece_processor.h for this path)."""
@@ -616,6 +664,7 @@ class SentencePieceProcessor:
         self._model_bytes = bytes(serialized)
         self._engine = Engine(self._model_bytes, device=device)
         self._special = None
+        self._pieces = None
         self._extra = []
         return True
 
@@ -661,18 +710,58 @@ class SentencePieceProcessor:
             raise RuntimeError("Model is not initialized.")  # sentencepiece_processor.cc:293-299
 
     # sentencepiece_processor.h:458 + python batch entry sentencepiece.i:439-446
-    def DecodeIds(self, input):
-        """Decode(ids) (src/sentencepiece_processor.h, python __init__.py DecodeIds): one id list or a list of lists."""
+    def DecodeIds(self, input, out_type=str):
+        """Decode(ids) (src/sentencepiece_processor.h, python __init__.py DecodeIds): one id list or a list of lists;
+        out_type str, bytes or 'immutable_proto' as in Decode."""
         self._require()
-        single = len(input) == 0 or not isinstance(input[0], (list, tuple, np.ndarray))
-        lists = [input] if single else list(input)
-        ido = np.zeros(len(lists) + 1, dtype=np.uint64)
-        if lists:
-            ido[1:] = np.cumsum([len(x) for x in lists], dtype=np.uint64)
-        ids = np.concatenate([np.asarray(x, dtype=np.int32) for x in lists]) if int(ido[-1]) else np.zeros(0, np.int32)
-        text, to = self._engine.decode_packed(ids, ido)
-        raw = text.tobytes()
-        out = [raw[int(to[i]):int(to[i + 1])].decode("utf-8", errors="replace") for i in range(len(lists))]
+        if out_type is str:
+            return self._decode(input, str)
+        return self.Decode(input, out_type=out_type)
+
+    # python/src/sentencepiece/__init__.py Decode (:776-868)
+    def Decode(self, input, out_type=str):
+        """An id, a list of ids or a list of id lists -> str, bytes or ImmutableSentencePieceText (out_type str, bytes or
+        'immutable_proto'), one or a list.  Empty input returns '' as in the reference, whose `if not input` test also
+        catches the single id 0.  Pieces (str input) are not decoded by the device path: NotImplementedError."""
+        self._require()
+        if not isinstance(input, np.ndarray) and not input:
+            return ""
+        if out_type is not str and out_type is not bytes and out_type != "immutable_proto":
+            raise RuntimeError("unknown output or input type")
+        first = input
+        while isinstance(first, (list, tuple, np.ndarray)) and len(first):
+            first = first[0]
+        if isinstance(first, str):
+            raise NotImplementedError("Decode of piece strings (DecodePieces) is not offered by the device path")
+        if isinstance(input, (int, np.integer)):
+            input = [int(input)]
+        return self._decode(input, out_type)
+
+    decode = Decode
+
+    # sentencepiece.i _DecodeIdsAsImmutableProto (:506-512, 541-545): Decode(ids, SentencePieceText*), then
+    # ConvertToUnicodeSpans over the decoded text
+    def DecodeIdsAsImmutableProto(self, input):
+        """One id list or a list of lists -> ImmutableSentencePieceText (or a list): the decoded text and every token's
+        piece, id, surface (text[begin:end]) and begin / end in characters of that text."""
+        return self.Decode(input, out_type="immutable_proto")
+
+    decode_ids_as_immutable_proto = DecodeIdsAsImmutableProto
+
+    def _decode(self, input, out_type):
+        single, (ids, ido) = _id_lists(input)
+        if out_type == "immutable_proto":
+            text, to, te = self._engine.decode_offsets(ids, ido)
+            if self._pieces is None:
+                from . import _modelinfo
+                self._pieces = [p.encode("utf-8") for p in _modelinfo.pieces_and_types(self._model_bytes)[0]]
+            out = decode_protos(self._pieces, ids, ido, text, to, te)
+        else:
+            text, to = self._engine.decode_packed(ids, ido)
+            raw = text.tobytes()
+            out = [raw[int(to[i]):int(to[i + 1])] for i in range(len(ido) - 1)]
+            if out_type is str:
+                out = [o.decode("utf-8", errors="replace") for o in out]
         return out[0] if single else out
 
     def EncodeAsIds(self, input, add_bos=False, add_eos=False, reverse=False, emit_unk_piece=False):
