@@ -230,6 +230,34 @@ int spm_encode_ids_device_padded(spm_engine *e, const char *d_bytes, const uint6
                                  int32_t pad_id, uint32_t flags, int32_t *d_lengths, uint32_t *width_out,
                                  void *stream);
 
+/* The padded rows of spm_encode_ids_device_padded together with every token's begin / end in its input, aligned cell
+ * for cell (what other fast tokenizers call an offsets mapping): the ids and offsets a token-classification, span or
+ * question-answering model consumes, for a batch already in device memory.
+ *   d_ids (int32 [n, w], capacity out_capacity cells), d_lengths and *width_out: exactly what
+ *     spm_encode_ids_device_padded writes for the same batch, encode frame, width, pad_id and SPM_PAD_TRUNCATE /
+ *     SPM_PAD_LEFT flags, including both SPM_ERR_CAPACITY cases (nothing written; *width_out the longest row or the
+ *     width used).
+ *   d_spans (int32 [n, w, 2], room for 2 * out_capacity int32, 8-byte aligned): cell (i, j) holds (begin, end) of the token in
+ *     d_ids[i, j]: for a real cell what spm_encode_offsets returns for that token with the same eos_id; frame entries
+ *     equal to eos_id get (len, len) and other frame entries (0, 0); a reversing frame reverses the offsets with the
+ *     body; truncation keeps exactly the cells the id row keeps; pad cells get (0, 0).
+ *   Units: byte offsets in the sentence's input (relative to d_offsets[i]); with SPM_OFFSETS_CHARS every offset p
+ *     becomes the index of the character that holds byte min(p, len) (len: the number of characters), the table of
+ *     the reference's ConvertToUnicodeSpans, characters being stepped by their lead byte's length as the reference
+ *     does, malformed input included.  The rows then hold exactly EncodeAsImmutableProto's begin / end.
+ * Argument rules, stream, "returns after the work is done on `stream`" and n == 0 as spm_encode_ids_device_padded;
+ * flags other than these three bits are SPM_ERR_ARG.  Sentences whose offsets do not add up to their normalized
+ * length ("all normalized characters are not consumed") give SPM_ERR_ENCODE, and a sentence too long for the offsets
+ * path SPM_ERR_UNSUPPORTED, as in spm_encode_offsets.  Sentences that hold the unknown id are encoded a second time by
+ * the spans path (spm_engine_info.last_unk_detour).  No per-sentence data crosses PCIe: the host reads back a fixed
+ * number of status words (the detour count, the longest row, the chunk plan). */
+enum { SPM_OFFSETS_CHARS = 4 };
+int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                                     uint64_t total_bytes, int32_t eos_id,
+                                     int32_t *d_ids, int32_t *d_spans, uint64_t out_capacity, uint32_t width,
+                                     int32_t pad_id, uint32_t flags, int32_t *d_lengths, uint32_t *width_out,
+                                     void *stream);
+
 /* ------------------------------------------------------------------------
  * N-best and sampling (unigram models; BASELINE.json config 5).
  *

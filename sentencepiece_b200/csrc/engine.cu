@@ -18,6 +18,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <random>
 #include <thread>
@@ -41,6 +42,7 @@
 #include "nbest_kernel.cuh"
 #include "normalize_kernel.cuh"
 #include "offsets_kernel.cuh"
+#include "chars_kernel.cuh"
 #include "lattice_kernel.cuh"
 #include "trie_builder.h"
 
@@ -481,9 +483,20 @@ struct spm_engine {
   // kernel's time.
   int raw_segmentation(const char *bytes, const uint64_t *offsets, size_t n, bool detour, KPieces *P, uint64_t *raw_ids,
                        float *main_ms);
+  // Its device part, for a batch at d_bytes_base + d_offs[i] on st (the unigram kernel choice already made): the encode
+  // with the frame off, the unknown flags, the subset pack and the spans run.  at_read (may be empty) is called after
+  // the encode, while d_sent_count still holds its raw counts, to queue more work and copies on st; they complete in the
+  // status read that gives the detour count, or in a read of their own when no detour count is read.
+  int raw_segmentation_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n, uint64_t total_bytes,
+                              bool detour, KPieces *P, uint64_t *raw_ids, float *main_ms, cudaStream_t st,
+                              const std::function<int()> &at_read);
   // spm_encode_offsets (K11): begin / end of the framed tokens
   DevBuf<uint32_t> d_off_begin, d_off_end;
   PinBuf<uint32_t> h_off_begin, h_off_end;
+  // spm_encode_offsets_device_padded: the longest row, the longest sentence and the K11 chunk plan
+  // (offsets_plan_kernel), and their pinned copy
+  DevBuf<unsigned long long> d_opad;
+  PinBuf<unsigned long long> h_opad;
   // n-best / sampling; pieces: the candidates' token ends and the exported normalized texts (NbestOut)
   DevBuf<uint8_t> d_nb_scratch, d_nb_norm;
   DevBuf<uint32_t> d_nb_end;
@@ -3439,7 +3452,15 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
   CUDA_TRY(cudaEventRecord(ev[3], st));
   if (total_bytes) CUDA_TRY(cudaMemcpyAsync(d_bytes.p, bytes + base, total_bytes, cudaMemcpyHostToDevice, st));
   CUDA_TRY(cudaMemcpyAsync(d_offsets.p, offsets, (n + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, st));
-  last_h2d = total_bytes + (n + 1) * sizeof(uint64_t);
+  const uint64_t h2d = total_bytes + (n + 1) * sizeof(uint64_t);
+  SPM_TRY(raw_segmentation_device(d_bytes.p - base, d_offsets.p, n, total_bytes, detour, P, raw_ids, main_ms, st, {}));
+  last_h2d = h2d;
+  return SPM_OK;
+}
+
+int spm_engine::raw_segmentation_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n,
+                                        uint64_t total_bytes, bool detour, KPieces *P, uint64_t *raw_ids,
+                                        float *main_ms, cudaStream_t st, const std::function<int()> &at_read) {
   // ---- 1. raw ids: the frame is written once, by K9 / K11 ----
   int rc;
   {
@@ -3453,7 +3474,7 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
       }
       ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
     } off(this);
-    rc = run_device(d_bytes.p - base, d_offsets.p, n, total_bytes, false, nullptr, 0, nullptr, raw_ids, nullptr, st,
+    rc = run_device(d_bytes_base, d_offs, n, total_bytes, false, nullptr, 0, nullptr, raw_ids, nullptr, st,
                     &d_pc_ids, &d_pc_id_offsets);
   }
   if (rc) return rc;
@@ -3464,6 +3485,7 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
   P->n = n32;
   P->ids = d_pc_ids.p;
   P->id_offsets = d_pc_id_offsets.p;
+  if (at_read) SPM_TRY(at_read());
   // ---- 2. unknown extents: only the sentences that hold the unknown id take the spans path ----
   uint32_t m = 0;
   if (detour && unk_id >= 0) {
@@ -3476,6 +3498,8 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
     SPM_TRY(scan_gather<uint8_t>(d_pc_flag.p, n32, d_pc_pos.p, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
     SPM_TRY(read_status(st, 0, 4));
     m = static_cast<uint32_t>(h_ctrl64.p[2]);
+  } else if (at_read) {
+    CUDA_TRY(cudaStreamSynchronize(st));
   }
   if (m) {
     CUDA_TRY(d_pc_sub_of.ensure(n));
@@ -3484,11 +3508,11 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
     CUDA_TRY(d_pc_sub_offsets.ensure(m + 1));
     CUDA_TRY(d_pc_sub_bytes.ensure(total_bytes + 64));
     pieces_sub_list_kernel<<<static_cast<int>(std::min<size_t>(static_cast<size_t>(sm_count) * 8, (n + 255) / 256)), 256, 0, st>>>(
-        d_pc_flag.p, d_pc_pos.p, d_offsets.p, n32, d_pc_sub_of.p, d_pc_sub_start.p, d_pc_sub_len.p);
+        d_pc_flag.p, d_pc_pos.p, d_offs, n32, d_pc_sub_of.p, d_pc_sub_start.p, d_pc_sub_len.p);
     CUDA_TRY(cudaGetLastError());
     ++last_launches;
     SPM_TRY(scan_total(d_pc_sub_len.p, m, 0, d_ctrl64.p + 2, st));
-    SPM_TRY(scan_gather<uint8_t>(d_pc_sub_len.p, m, d_pc_sub_offsets.p, d_pc_sub_start.p, d_bytes.p - base,
+    SPM_TRY(scan_gather<uint8_t>(d_pc_sub_len.p, m, d_pc_sub_offsets.p, d_pc_sub_start.p, d_bytes_base,
                                  d_pc_sub_bytes.p, d_pc_sub_bytes.cap, 0, 0ull, st));
     // (the whole batch's byte count bounds the subset's: it only sizes the spans run's temporary buffers)
     uint64_t sub_tot = 0, sub_norm = 0;
@@ -3725,6 +3749,169 @@ int spm_encode_offsets(spm_engine *e, const char *bytes, const uint64_t *offsets
   std::lock_guard<std::mutex> lk(e->mu);
   return encode_offsets_locked(e, bytes, offsets, n, eos_id, unk_piece, unk_piece_len, sep, ids, id_offsets, begin, end,
                                text, text_offsets, piece_end);
+}
+
+// spm_encode_offsets for a device batch, as padded rows:
+//   1. the raw segmentation on st, with the unknown detour; behind its encode, row_max_kernel (the longest framed row)
+//      and offsets_plan_kernel (the K11 chunk cuts, the longest sentence) fill d_opad, which comes back in the status
+//      read of the detour count;
+//   2. the width and capacity checks of spm_encode_ids_device_padded;
+//   3. offsets_padded_kernel (K11's padded mode) per chunk, writing every cell of the rows;
+//   4. with SPM_OFFSETS_CHARS, spans_to_chars_kernel over all rows.
+// Host synchronisations: pick_fast_words_device's (unigram), encode_stage's status reads (one, and one more per
+// deferral stage that runs), run_device's total, the detour count (with d_opad), the detour's spans run when a
+// sentence holds the unknown id (its encode_stage reads and its total), the rest of the cuts when there are more than
+// kOpadInlineCuts chunks, and the final one.
+static constexpr uint32_t kOpadInlineCuts = 32;
+static constexpr size_t kOpadHead = 4;
+
+int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                                     uint64_t total_bytes, int32_t eos_id, int32_t *d_ids, int32_t *d_spans,
+                                     uint64_t out_capacity, uint32_t width, int32_t pad_id, uint32_t flags,
+                                     int32_t *d_lengths, uint32_t *width_out, void *stream) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!d_offsets || !width_out || (n && (!d_ids || !d_spans || !d_lengths)) || (n && !d_bytes && total_bytes)) {
+    e->set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  if (reinterpret_cast<uintptr_t>(d_spans) % 8u) {  // (the kernels store (begin, end) as one 8-byte pair)
+    e->set_error("d_spans must be 8-byte aligned");
+    return SPM_ERR_ARG;
+  }
+  if (flags & ~static_cast<uint32_t>(SPM_PAD_TRUNCATE | SPM_PAD_LEFT | SPM_OFFSETS_CHARS)) {
+    e->set_error("unknown flags");
+    return SPM_ERR_ARG;
+  }
+  const bool truncate = flags & SPM_PAD_TRUNCATE;
+  const uint32_t frame = e->frame_np + e->frame_ns;
+  if (truncate && width && width < frame) {
+    e->set_error("width " + std::to_string(width) + " is shorter than the encode frame (" + std::to_string(frame) + " ids)");
+    return SPM_ERR_ARG;
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  *width_out = 0;
+  if (n == 0) {
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SPM_OK;
+  }
+  e->last_h2d = e->last_d2h = 0;
+  e->last_unk_detour = 0;
+  SPM_TRY(e->ensure_piece_tables());
+  const uint8_t *d_base = reinterpret_cast<const uint8_t *>(d_bytes);
+  if (e->model.model_type == SPM_UNIGRAM) SPM_TRY(e->pick_fast_words_device(d_base, d_offsets, n, st, &e->batch_fast_words));
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
+  const size_t head = kOpadHead + 2 * kOpadInlineCuts;
+  CUDA_TRY(e->d_opad.ensure(std::max(head, kOpadHead + 2 * (n + 1))));
+  CUDA_TRY(e->h_opad.ensure(e->d_opad.cap));
+  uint64_t d2h = 0;
+  auto at_read = [&]() -> int {
+    CUDA_TRY(cudaMemsetAsync(e->d_opad.p, 0, kOpadHead * sizeof(unsigned long long), st));
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256));
+    row_max_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, frame, e->d_opad.p + 3);
+    offsets_plan_kernel<<<grid, 256, 0, st>>>(d_offsets, n32, expand, kNormChunkSlab, static_cast<uint32_t>((e->d_opad.cap - kOpadHead) / 2),
+                                              e->d_opad.p);
+    CUDA_TRY(cudaGetLastError());
+    e->last_launches += 2;
+    CUDA_TRY(cudaMemcpyAsync(e->h_opad.p, e->d_opad.p, head * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+    d2h += head * sizeof(unsigned long long);
+    return SPM_OK;
+  };
+  KPieces P{};
+  uint64_t raw_ids = 0;
+  float main_ms = 0.f;
+  CUDA_TRY(cudaEventRecord(e->ev[3], st));
+  SPM_TRY(e->raw_segmentation_device(d_base, d_offsets, n, total_bytes, true, &P, &raw_ids, &main_ms, st, at_read));
+  const unsigned long long *plan = e->h_opad.p;
+  const uint64_t chunks = plan[0], slab_max = plan[1], longest_input = plan[2], longest = plan[3];
+  if (norm_slab_start(longest_input, 1, expand) > 0x7FFFFF00ull) {
+    set_error("sentence too long for the device path");
+    return SPM_ERR_UNSUPPORTED;
+  }
+  // ---- the longest framed row decides the width, or whether the call fails ----
+  if (longest > 0xFFFFFFFFull) { set_error("a row is longer than 2^32 - 1 ids"); return SPM_ERR_UNSUPPORTED; }
+  if (width && !truncate && longest > width) {
+    *width_out = static_cast<uint32_t>(longest);
+    set_error("a row of " + std::to_string(longest) + " ids does not fit width " + std::to_string(width));
+    return SPM_ERR_CAPACITY;
+  }
+  const uint32_t w = width ? width : static_cast<uint32_t>(longest);
+  *width_out = w;
+  if (static_cast<unsigned long long>(n) * w > out_capacity) {
+    set_error("out_capacity too small: need " + std::to_string(static_cast<unsigned long long>(n) * w));
+    return SPM_ERR_CAPACITY;
+  }
+  if (chunks > kOpadInlineCuts) {  // (over 2^32 slab elements of input)
+    const size_t rest = 2 * (chunks - kOpadInlineCuts);
+    CUDA_TRY(cudaMemcpyAsync(e->h_opad.p + head, e->d_opad.p + head, rest * sizeof(unsigned long long),
+                             cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    d2h += rest * sizeof(unsigned long long);
+  }
+  // ---- K11, padded: the rows ----
+  P.F = e->kframe();
+  P.pc_off = e->d_pc_off.p;
+  P.pc_bytes = e->d_pc_bytes.p;
+  P.unk_id = e->unk_id;
+  CUDA_TRY(e->d_tmp_norm.ensure(slab_max + 16));
+  CUDA_TRY(e->d_tmp_n2o.ensure(slab_max + 16));
+  CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, sizeof(uint32_t), st));
+  KModel M = e->km;
+  M.hot_link = M.hot_val = 0;
+  KOffsets A{};
+  A.P = P;
+  A.offsets = d_offsets;
+  A.expand = expand;
+  A.slab_text = e->d_tmp_norm.p;
+  A.slab_n2o = e->d_tmp_n2o.p;
+  A.eos_id = eos_id;
+  A.status = e->d_ctrl32.p;
+  A.pad_ids = d_ids;
+  A.spans = reinterpret_cast<int2 *>(d_spans);
+  A.lengths = d_lengths;
+  A.w = w;
+  A.pad_id = pad_id;
+  A.truncate = truncate ? 1u : 0u;
+  A.left = (flags & SPM_PAD_LEFT) ? 1u : 0u;
+  CUDA_TRY(cudaEventRecord(e->ev[0], st));  // (raw_segmentation_device has read ev[0] / ev[1])
+  for (uint64_t c = 0; c < chunks; ++c) {
+    A.first = static_cast<uint32_t>(plan[kOpadHead + 2 * c]);
+    A.n = static_cast<uint32_t>((c + 1 < chunks ? plan[kOpadHead + 2 * (c + 1)] : n) - A.first);
+    A.bytes = d_base + plan[kOpadHead + 2 * c + 1];
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (A.n + 7) / 8));
+    offsets_padded_kernel<<<grid, 256, 0, st>>>(M, A);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  if (flags & SPM_OFFSETS_CHARS) {
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+    spans_to_chars_kernel<<<grid, 256, 0, st>>>(d_base, d_offsets, n32, A.spans, d_lengths, w, P.F, eos_id, A.left);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  CUDA_TRY(cudaEventRecord(e->ev[1], st));
+  SPM_TRY(e->copy_status(st, 1, 0));
+  CUDA_TRY(cudaEventRecord(e->ev[2], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  d2h += sizeof(uint32_t);
+  if (e->h_ctrl32.p[0] & 2u) {
+    set_error("encode offsets: a sentence normalized to more bytes than its bound");
+    return SPM_ERR_ENCODE;
+  }
+  if (e->h_ctrl32.p[0]) {
+    set_error("encode offsets: all normalized characters are not consumed");
+    return SPM_ERR_ENCODE;
+  }
+  e->last_d2h = d2h;
+  float k_ms = 0.f, all = 0.f;
+  e->last_main_ms = main_ms + (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess ? k_ms : 0.f);
+  e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : e->last_main_ms;
+  (void)cudaGetLastError();
+  return SPM_OK;
 }
 
 // unk_piece / sep as spm_encode_pieces takes them

@@ -21,6 +21,12 @@
 // are not consumed", which the reference reports as an error): status bit 0 otherwise.  Status bit 1: a sentence
 // normalized to more bytes than its slab holds (the bound of normalize_kernel.cuh says it cannot).
 //
+// Padded mode (offsets_padded_kernel, spm_encode_offsets_device_padded): the same walk, but the warp owns row `sent` of
+// an [n, w] id tensor and its [n, w, 2] begin / end tensor and writes every cell of it, as write_padded_kernel
+// (padded_kernel.cuh) lays the row out: the frame's prefix, body positions k < B (k = L - 1 - q under a reversing frame,
+// else q; B = L, or min(L, w - np - ns) when truncating), the suffix, all shifted by w - real when padding on the left,
+// and pad_id / (0, 0) in the other cells.  Tokens past B are walked (the lengths still have to add up) but not stored.
+//
 // The byte-fallback grouping assumes the normalized text is valid UTF-8, so that every unknown piece is exactly one
 // character.  The normalizer guarantees that for every input (a malformed byte becomes U+FFFD) as long as the
 // model's charsmap targets are valid UTF-8; the engine refuses models whose targets are not.
@@ -55,9 +61,18 @@ struct KOffsets {
   int32_t *out_ids;                    // null: the ids are written by K9
   unsigned long long *out_id_offsets;  // with out_ids
   uint32_t *status;  // bit 0: lengths do not add up; bit 1: slab overflow
+  // padded mode: rows of width w at pad_ids + sent * w and (begin, end) pairs at spans + sent * w; lengths[sent] =
+  // the row's real cells
+  int32_t *pad_ids;
+  int2 *spans;
+  int32_t *lengths;
+  uint32_t w;
+  int32_t pad_id;
+  uint32_t truncate, left;
 };
 
-__global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const KOffsets A) {
+template <bool PADDED>
+__device__ __forceinline__ void offsets_walk(const KModel &M, const KOffsets &A) {
   const Tile T;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   const KPieces &P = A.P;
@@ -79,7 +94,23 @@ __global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const K
     const unsigned long long out = raw + static_cast<unsigned long long>(sent) * fr;
     const bool overflow = r.n > tm.ncap;
     bool bad = overflow || L != P.id_offsets[sent + 1] - raw;
-    if (A.out_ids && T.lane == 0) {
+    // padded mode: the row's kept body B, its real cells and the pad cells before them
+    [[maybe_unused]] uint32_t B = L, lead = 0;
+    [[maybe_unused]] int32_t *row_ids = nullptr;
+    [[maybe_unused]] int2 *row_sp = nullptr;
+    if constexpr (PADDED) {
+      B = A.truncate ? min(L, A.w - fr) : L;
+      const uint32_t real = B + fr;
+      lead = A.left ? A.w - real : 0u;
+      row_ids = A.pad_ids + static_cast<unsigned long long>(sent) * A.w;
+      row_sp = A.spans + static_cast<unsigned long long>(sent) * A.w;
+      for (uint32_t t = T.lane; t < A.w; t += 32)
+        if (t - lead >= real) {  // (wraps for the leading pad cells)
+          __stcs(row_ids + t, A.pad_id);
+          __stcs(row_sp + t, make_int2(0, 0));
+        }
+      if (T.lane == 0) A.lengths[sent] = static_cast<int32_t>(real);
+    } else if (A.out_ids && T.lane == 0) {
       if (sent == 0) A.out_id_offsets[0] = 0;
       A.out_id_offsets[sent + 1] = P.id_offsets[sent + 1] + static_cast<unsigned long long>(sent + 1) * fr;
     }
@@ -87,10 +118,16 @@ __global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const K
     for (uint32_t t = T.lane; t < fr; t += 32) {
       const int32_t id = P.F.ids[t];
       const uint32_t o = id == A.eos_id ? len : 0u;
-      const unsigned long long k = out + (t < P.F.np ? t : L + t);
-      A.begin[k] = o;
-      A.end[k] = o;
-      if (A.out_ids) A.out_ids[k] = id;
+      if constexpr (PADDED) {
+        const uint32_t c = lead + (t < P.F.np ? t : B + t);
+        __stcs(row_ids + c, id);
+        __stcs(row_sp + c, make_int2(static_cast<int32_t>(o), static_cast<int32_t>(o)));
+      } else {
+        const unsigned long long k = out + (t < P.F.np ? t : L + t);
+        A.begin[k] = o;
+        A.end[k] = o;
+        if (A.out_ids) A.out_ids[k] = id;
+      }
     }
     // the body
     uint32_t c0 = 0;      // normalized bytes before this trip
@@ -131,10 +168,18 @@ __global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const K
         } else {
           const uint32_t b = tm.n2o[byte ? head : c];
           const uint32_t e = byte && next_cont ? b : tm.n2o[c1];
-          const unsigned long long k = out + P.F.np + (P.F.reverse ? L - 1u - q : q);
-          A.begin[k] = b;
-          A.end[k] = e;
-          if (A.out_ids) A.out_ids[k] = id;
+          if constexpr (PADDED) {
+            const uint32_t k = P.F.reverse ? L - 1u - q : q;
+            if (k < B) {
+              __stcs(row_ids + lead + P.F.np + k, id);
+              __stcs(row_sp + lead + P.F.np + k, make_int2(static_cast<int32_t>(b), static_cast<int32_t>(e)));
+            }
+          } else {
+            const unsigned long long k = out + P.F.np + (P.F.reverse ? L - 1u - q : q);
+            A.begin[k] = b;
+            A.end[k] = e;
+            if (A.out_ids) A.out_ids[k] = id;
+          }
         }
       }
       bad = T.ballot(bad) != 0u;
@@ -143,6 +188,65 @@ __global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const K
     }
     if (!bad && c0 != r.n) bad = true;
     if (bad && T.lane == 0) atomicOr(A.status, overflow ? 2u : 1u);
+  }
+}
+
+__global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const KOffsets A) { offsets_walk<false>(M, A); }
+
+__global__ void __launch_bounds__(256, 1) offsets_padded_kernel(const KModel M, const KOffsets A) {
+  offsets_walk<true>(M, A);
+}
+
+// The chunk plan of a device batch (spm_encode_offsets_device_padded): the cuts spm_encode_offsets makes on the host
+// -- chunk c is the longest run of sentences from its first whose slabs (norm_slab_start) stay within chunk_slab, at
+// least one sentence -- found by warp 0 of block 0 with a 32-way search per cut (the slab of a run grows with its end).
+// plan[0] = the chunks, plan[1] = the largest chunk slab, plan[2] = the longest sentence in bytes (every block);
+// plan[4 + 2c] / plan[5 + 2c] = chunk c's first sentence and its byte offset, for c < max_cuts.  plan[0..3) are zeroed
+// by the caller.  n > 0.
+__global__ void __launch_bounds__(256) offsets_plan_kernel(const uint64_t *offs, uint32_t n, uint32_t expand,
+                                                           unsigned long long chunk_slab, uint32_t max_cuts,
+                                                           unsigned long long *plan) {
+  unsigned long long longest = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x)
+    longest = max(longest, static_cast<unsigned long long>(offs[i + 1] - offs[i]));
+  longest = __reduce_max_sync(0xFFFFFFFFu, static_cast<unsigned>(min(longest, 0xFFFFFFFFull)));
+  if ((threadIdx.x & 31) == 0) atomicMax(plan + 2, longest);
+  if (blockIdx.x != 0 || threadIdx.x >= 32) return;
+  const uint32_t lane = threadIdx.x;
+  uint32_t chunks = 0;
+  unsigned long long slab_max = 0;
+  for (uint32_t lo = 0; lo < n;) {
+    const uint64_t base = offs[lo];
+    // the largest hi in [lo + 1, n] whose run [lo, hi) fits, or lo + 1.  It lies in [a, b]; lane j probes
+    // h_j = a + ceil((b - a)(j + 1) / 32), which rises with j to h_31 = b, and `fits` falls as h rises
+    uint32_t a = lo + 1, b = n;
+    while (a < b) {
+      const unsigned long long span = b - a;
+      const uint32_t h = a + static_cast<uint32_t>((span * (lane + 1) + 31u) / 32u);
+      const uint32_t m = __ballot_sync(0xFFFFFFFFu, norm_slab_start(offs[h] - base, h - lo, expand) <= chunk_slab);
+      const uint32_t h0 = a + static_cast<uint32_t>((span + 31u) / 32u);
+      if (!m) {
+        b = h0 - 1u;
+      } else {
+        const uint32_t last = 31u - __clz(m);
+        const uint32_t ha = __shfl_sync(0xFFFFFFFFu, h, last);
+        const uint32_t hb = __shfl_sync(0xFFFFFFFFu, h, last < 31u ? last + 1u : 31u);
+        a = ha;
+        b = last < 31u ? hb - 1u : b;
+      }
+    }
+    const uint32_t hi = a;
+    if (lane == 0 && chunks < max_cuts) {
+      plan[4 + 2 * chunks] = lo;
+      plan[5 + 2 * chunks] = base;
+    }
+    slab_max = max(slab_max, norm_slab_start(offs[hi] - base, hi - lo, expand));
+    ++chunks;
+    lo = hi;
+  }
+  if (lane == 0) {
+    plan[0] = chunks;
+    plan[1] = slab_max;
   }
 }
 

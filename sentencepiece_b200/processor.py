@@ -609,6 +609,63 @@ class Engine:
             self._pad_guess = max(w, 1)  # (an all-empty batch gives 0, and zero cells have no device pointer)
         return cells.view(-1)[:n * w].view(n, w), lengths
 
+    def encode_offsets_device_padded(self, d_bytes, d_offsets, width=0, pad_id=None, truncate=False, pad_left=False,
+                                     unit="byte", eos_id=None, out=None):
+        """spm_encode_offsets_device_padded: the rows of encode_device_padded with every token's begin / end in its
+        input -> (ids int32 [n, w], spans int32 [n, w, 2], lengths int32 [n]).  spans[i, j] is (begin, end) of the
+        token in ids[i, j], as encode_offsets gives it; frame entries equal to eos_id (None = the model's eos_id())
+        get (len, len), other frame entries and pad cells (0, 0).  unit "byte": offsets in bytes of the sentence's
+        input; "char": in characters, as ConvertToUnicodeSpans converts them (EncodeAsImmutableProto's begin / end).
+        Arguments, errors and the width-0 retry as encode_device_padded; out: a contiguous int32 tensor of at least
+        3 * n * w + 1 cells, which take the ids and then the spans (at an even cell, as the spans must be 8-byte
+        aligned)."""
+        import torch
+        if unit not in ("byte", "char"):
+            raise ValueError('unit must be "byte" or "char"')
+        if pad_id is None:
+            pad_id = self.pad_id()
+            if pad_id < 0:
+                raise ValueError("the model defines no pad piece (trainer_spec.pad_piece): pass pad_id explicitly")
+        if eos_id is None:
+            from . import _modelinfo
+            eos_id = _modelinfo.special_pieces(self._model_bytes)["eos_id"]
+        st = self._stream(d_bytes, d_offsets, out)
+        if d_bytes.dtype != torch.uint8 or d_bytes.dim() != 1 or not d_bytes.is_contiguous():
+            raise ValueError("d_bytes must be a contiguous 1-D uint8 tensor")
+        if d_offsets.dtype not in (torch.int64, torch.uint64) or d_offsets.dim() != 1 or not d_offsets.is_contiguous():
+            raise ValueError("d_offsets must be a contiguous 1-D int64 or uint64 tensor of n + 1 offsets")
+        if out is not None and (out.dtype != torch.int32 or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int32 tensor")
+        n = d_offsets.numel() - 1
+        flags = (_capi.PAD_TRUNCATE if truncate else 0) | (_capi.PAD_LEFT if pad_left else 0) | \
+            (_capi.OFFSETS_CHARS if unit == "char" else 0)
+        lengths = torch.empty(n, dtype=torch.int32, device=d_bytes.device)
+
+        def call(cells):
+            cap = max(cells.numel() - 1, 0) // 3
+            at = cap + (cap & 1)  # first cell of the spans
+            w = ctypes.c_uint32()
+            rc = self._lib.spm_encode_offsets_device_padded(self._h, d_bytes.data_ptr(), d_offsets.data_ptr(), n,
+                                                            d_bytes.numel(), eos_id, cells.data_ptr(),
+                                                            cells.data_ptr() + 4 * at, cap, width, pad_id, flags,
+                                                            lengths.data_ptr(), ctypes.byref(w), st)
+            return rc, w.value, at
+
+        cells = out if out is not None else torch.empty(3 * n * (width or self._pad_guess) + 1, dtype=torch.int32,
+                                                        device=d_bytes.device)
+        rc, w, at = call(cells)
+        too_long = width and not truncate and w > width
+        if rc == _capi.SPM_ERR_CAPACITY and out is None and not too_long:
+            cells = torch.empty(3 * n * w + 1, dtype=torch.int32, device=d_bytes.device)
+            rc, w, at = call(cells)
+        if rc == _capi.SPM_ERR_CAPACITY:
+            raise ValueError(self._lib.spm_last_error(self._h).decode())
+        self._check(rc)
+        if not width and n:
+            self._pad_guess = max(w, 1)
+        flat = cells.view(-1)
+        return flat[:n * w].view(n, w), flat[at:at + 2 * n * w].view(n, w, 2), lengths
+
     def decode_device(self, ids2d, lengths=None, stop_id=-1):
         """spm_decode_ids_device: the rows of an int32 or int64 [n, L] CUDA tensor (any row stride, e.g. a column slice;
         each row contiguous) -> list of n str.  Row i holds min(L, lengths[i]) ids (lengths: int32 [n], or None for L),
@@ -907,12 +964,15 @@ class SentencePieceProcessor:
     # ---- padded id tensors on the device (no reference counterpart): a model's [batch, seq_len] input, and the text
     #      of a [batch, T] generation output ----
     def encode_padded(self, input, max_len=None, pad_id=None, truncate=False, pad_left=False, add_bos=False,
-                      add_eos=False, reverse=False):
+                      add_eos=False, reverse=False, return_offsets=False):
         """EncodeAsIds of a batch as padded rows on the GPU -> (ids int32 [n, w], lengths int32 [n]) on the engine's
         device.  input: a list of str / bytes (packed and uploaded through pinned memory) or a (bytes, offsets) pair of
         CUDA tensors as Engine.encode_device_padded takes them.  max_len = None: w is the longest row; otherwise rows
         longer than max_len fail (ValueError) unless truncate, which keeps bos / eos and cuts the ids between them.
-        pad_id = None: the model's pad_id(), and ValueError when it has none."""
+        pad_id = None: the model's pad_id(), and ValueError when it has none.
+        return_offsets: -> (ids, lengths, offsets int32 [n, w, 2]), offsets[i, j] the (begin, end) of the token in
+        ids[i, j] in characters of input i, as ConvertToUnicodeSpans counts them (EncodeAsImmutableProto's begin /
+        end; eos gets (len, len), bos and pad cells (0, 0))."""
         self._require()
         if isinstance(input, tuple):
             d_bytes, d_offs = input
@@ -923,6 +983,11 @@ class SentencePieceProcessor:
             d_bytes = torch.from_numpy(np.require(buf, requirements="W")).pin_memory().to(dev, non_blocking=True)
             d_offs = torch.from_numpy(offs.view(np.int64)).pin_memory().to(dev, non_blocking=True)
         self._set_frame(add_bos, add_eos, reverse)
+        if return_offsets:
+            ids, spans, lengths = self._engine.encode_offsets_device_padded(
+                d_bytes, d_offs, width=max_len or 0, pad_id=pad_id, truncate=truncate, pad_left=pad_left, unit="char",
+                eos_id=self._specials()["eos_id"])
+            return ids, lengths, spans
         return self._engine.encode_device_padded(d_bytes, d_offs, width=max_len or 0, pad_id=pad_id, truncate=truncate,
                                                  pad_left=pad_left)
 
