@@ -258,6 +258,39 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
                                      int32_t pad_id, uint32_t flags, int32_t *d_lengths, uint32_t *width_out,
                                      void *stream);
 
+/* A device batch as overlapping windows of one width (what other fast tokenizers call overflowing tokens with a
+ * stride): long inputs for extractive QA, long-document classification, token classification or retrieval chunks,
+ * with every token kept.
+ * For sentence i: F_i = prefix ++ body_i ++ suffix is the framed list spm_encode_ids_device returns (body_i already
+ * reversed when the frame reverses), np / ns the prefix and suffix sizes, L_i = |body_i|.  For width w and an overlap
+ * `stride`: B = w - np - ns, which must satisfy B >= 1 and 0 <= stride < B (else SPM_ERR_ARG); step = B - stride.
+ *   Sentence i gets m_i = 1 row if L_i <= B, else 1 + ceil((L_i - B) / step) rows.  Window j holds
+ *   prefix ++ body_i[j*step : min(j*step + B, L_i)] ++ suffix: every window carries the whole frame, every window after
+ *   the first starts step tokens later and holds at least one token the one before it does not, and an empty sentence
+ *   gets one row that holds the frame only.
+ *   Rows are ordered by sentence, then window; R = sum m_i.  Row r is written at d_ids + r * w with pad_id in the other
+ *   cells (SPM_PAD_LEFT: the real cells at the end of the row); d_lengths[r] = its real cells; d_row_sentence[r] = i
+ *   (the overflow-to-sample mapping); d_row_first[r] = j*step, the index in body_i of the window's first body token.
+ *   d_spans (optional, int32 [R, w, 2], 8-byte aligned; NULL = no offsets): cell (r, c) holds the (begin, end)
+ *   spm_encode_offsets_device_padded gives the same token with the same eos_id; frame entries equal to eos_id get
+ *   (len, len), other frame entries and pad cells (0, 0); SPM_OFFSETS_CHARS gives characters as there.  Without
+ *   d_spans, no normalizer walk runs: the ids cost what spm_encode_ids_device_padded's cost.
+ * When every L_i <= B the result is exactly spm_encode_ids_device_padded / spm_encode_offsets_device_padded with width
+ * w: the same rows, lengths and spans, R = n, row_sentence = 0..n-1, row_first = 0.
+ * R is known only after the encode and comes back with the call's status words: if R > rows_capacity the call returns
+ * SPM_ERR_CAPACITY with *rows_out = R and writes nothing to any output (a retry with room encodes the batch again);
+ * on success *rows_out = R.  SPM_ERR_ARG: width == 0, SPM_PAD_TRUNCATE (windows never drop tokens), SPM_OFFSETS_CHARS
+ * without d_spans, other flags, null pointers, a misaligned d_spans.  SPM_ERR_UNSUPPORTED: a body longer than
+ * 2^31 - 1 ids, or R over 2^31 - 1.  With d_spans: a sentence too long for the offsets path, SPM_ERR_ENCODE on
+ * unconsumed characters and the unknown-id detour (spm_engine_info.last_unk_detour) as in
+ * spm_encode_offsets_device_padded.  Stream, "returns after the work is done on `stream`" and n == 0 (*rows_out = 0)
+ * as the padded calls.  No per-token data crosses PCIe: the host reads back a fixed number of status words. */
+int spm_encode_windows_device(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                              uint64_t total_bytes, uint32_t width, uint32_t stride, int32_t pad_id, uint32_t flags,
+                              int32_t eos_id, int32_t *d_ids, int32_t *d_spans, uint64_t rows_capacity,
+                              int32_t *d_lengths, int32_t *d_row_sentence, int32_t *d_row_first,
+                              uint64_t *rows_out, void *stream);
+
 /* ------------------------------------------------------------------------
  * N-best and sampling (unigram models; BASELINE.json config 5).
  *

@@ -79,10 +79,55 @@ struct CharSweep {
   }
 };
 
+// One list's offsets in place: its body of B tokens at cells np + (B - 1 - q reversed, else q) for raw position q, its
+// frame at cells [0, np) and [np + B, np + B + ns).  Cells: get(c) / set(c, v) of the (begin, end) at cell c.
+template <typename Cells>
+__device__ __forceinline__ void list_to_chars(CharSweep &sw, Cells cells, uint32_t B, const KFrame &F, int32_t eos_id,
+                                              uint32_t lane) {
+  const uint32_t fr = F.np + F.ns;
+  for (uint32_t r0 = 0; r0 < B; r0 += 32) {
+    const uint32_t q = r0 + lane;  // raw order
+    const bool act = q < B;
+    const uint32_t cell = F.np + (F.reverse ? B - 1u - q : q);
+    int2 v = act ? cells.get(cell) : make_int2(0, 0);
+    const uint32_t b = min(static_cast<uint32_t>(v.x), sw.len), e = min(static_cast<uint32_t>(v.y), sw.len);
+    const uint32_t lo = __reduce_min_sync(0xFFFFFFFFu, act ? min(b, e) : 0xFFFFFFFFu);
+    const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, act ? max(b, e) : 0u);
+    if (lo < sw.base) sw.reset();
+    uint32_t cb = 0, ce = 0;
+    for (;;) {
+      if (!sw.have) sw.block(lane);
+      if (b - sw.base < 32u) cb = sw.index(b);
+      if (e - sw.base < 32u) ce = sw.index(e);
+      if (hi < sw.base + 32u) break;
+      sw.advance();
+    }
+    if (act) cells.set(cell, make_int2(static_cast<int32_t>(cb), static_cast<int32_t>(ce)));
+  }
+  bool eos = false;
+  for (uint32_t t = 0; t < fr; ++t) eos |= F.ids[t] == eos_id;
+  if (!eos) return;
+  // the number of characters: the sweep to the block that holds len
+  if (sw.len < sw.base) sw.reset();
+  for (;;) {
+    if (!sw.have) sw.block(lane);
+    if (sw.len < sw.base + 32u) break;
+    sw.advance();
+  }
+  const int32_t chars = static_cast<int32_t>(sw.index(sw.len));
+  for (uint32_t t = lane; t < fr; t += 32)
+    if (F.ids[t] == eos_id) cells.set(t < F.np ? t : B + t, make_int2(chars, chars));
+}
+
 // One warp per row of the [n, w] spans tensor that the padded K11 wrote (byte offsets), rewritten in place.
 __global__ void __launch_bounds__(256) spans_to_chars_kernel(const uint8_t *bytes, const uint64_t *offsets, uint32_t n,
                                                              int2 *spans, const int32_t *lengths, uint32_t w, KFrame F,
                                                              int32_t eos_id, uint32_t left) {
+  struct Row {
+    int2 *r;
+    __device__ __forceinline__ int2 get(uint32_t c) const { return r[c]; }
+    __device__ __forceinline__ void set(uint32_t c, int2 v) const { r[c] = v; }
+  };
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   const uint32_t fr = F.np + F.ns;
@@ -93,43 +138,39 @@ __global__ void __launch_bounds__(256) spans_to_chars_kernel(const uint8_t *byte
     sw.reset();
     sw.mask = sw.next = 0u;
     const uint32_t real = static_cast<uint32_t>(lengths[row]);
-    const uint32_t B = real - fr;
-    int2 *r = spans + static_cast<unsigned long long>(row) * w + (left ? w - real : 0u);
-    for (uint32_t r0 = 0; r0 < B; r0 += 32) {
-      const uint32_t q = r0 + lane;  // raw order
-      const bool act = q < B;
-      int2 *cell = r + F.np + (F.reverse ? B - 1u - q : q);
-      int2 v = act ? *cell : make_int2(0, 0);
-      const uint32_t b = min(static_cast<uint32_t>(v.x), sw.len), e = min(static_cast<uint32_t>(v.y), sw.len);
-      const uint32_t lo = __reduce_min_sync(0xFFFFFFFFu, act ? min(b, e) : 0xFFFFFFFFu);
-      const uint32_t hi = __reduce_max_sync(0xFFFFFFFFu, act ? max(b, e) : 0u);
-      if (lo < sw.base) sw.reset();
-      uint32_t cb = 0, ce = 0;
-      for (;;) {
-        if (!sw.have) sw.block(lane);
-        if (b - sw.base < 32u) cb = sw.index(b);
-        if (e - sw.base < 32u) ce = sw.index(e);
-        if (hi < sw.base + 32u) break;
-        sw.advance();
-      }
-      if (act) *cell = make_int2(static_cast<int32_t>(cb), static_cast<int32_t>(ce));
+    list_to_chars(sw, Row{spans + static_cast<unsigned long long>(row) * w + (left ? w - real : 0u)}, real - fr, F,
+                  eos_id, lane);
+  }
+}
+
+// One warp per sentence of K11's framed, packed output (begin / end at id_offsets[i], byte offsets), rewritten in
+// place: the character offsets of spm_encode_windows_device, converted once per sentence before the window rows
+// copy them.
+__global__ void __launch_bounds__(256) lists_to_chars_kernel(const uint8_t *bytes, const uint64_t *offsets, uint32_t n,
+                                                             uint32_t *begin, uint32_t *end,
+                                                             const unsigned long long *id_offsets, KFrame F,
+                                                             int32_t eos_id) {
+  struct List {
+    uint32_t *b, *e;
+    __device__ __forceinline__ int2 get(uint32_t c) const {
+      return make_int2(static_cast<int32_t>(b[c]), static_cast<int32_t>(e[c]));
     }
-    bool eos = false;
-    for (uint32_t t = 0; t < fr; ++t) eos |= F.ids[t] == eos_id;
-    if (!eos) continue;
-    // the number of characters: the sweep to the block that holds len
-    if (sw.len < sw.base) sw.reset();
-    for (;;) {
-      if (!sw.have) sw.block(lane);
-      if (sw.len < sw.base + 32u) break;
-      sw.advance();
+    __device__ __forceinline__ void set(uint32_t c, int2 v) const {
+      b[c] = static_cast<uint32_t>(v.x);
+      e[c] = static_cast<uint32_t>(v.y);
     }
-    const int32_t chars = static_cast<int32_t>(sw.index(sw.len));
-    for (uint32_t t = lane; t < fr; t += 32)
-      if (F.ids[t] == eos_id) {
-        const uint32_t c = t < F.np ? t : B + t;
-        r[c] = make_int2(chars, chars);
-      }
+  };
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+  const uint32_t fr = F.np + F.ns;
+  for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += warps) {
+    CharSweep sw;
+    sw.s = bytes + offsets[i];
+    sw.len = static_cast<uint32_t>(offsets[i + 1] - offsets[i]);
+    sw.reset();
+    sw.mask = sw.next = 0u;
+    const unsigned long long o = id_offsets[i];
+    list_to_chars(sw, List{begin + o, end + o}, static_cast<uint32_t>(id_offsets[i + 1] - o) - fr, F, eos_id, lane);
   }
 }
 

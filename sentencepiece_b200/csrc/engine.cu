@@ -497,6 +497,11 @@ struct spm_engine {
   // (offsets_plan_kernel), and their pinned copy
   DevBuf<unsigned long long> d_opad;
   PinBuf<unsigned long long> h_opad;
+  // spm_encode_windows_device: the rows R, the longest body, then the first row of each sentence (d_win), their
+  // pinned copy (the first two words) and the windows per sentence
+  DevBuf<unsigned long long> d_win;
+  PinBuf<unsigned long long> h_win;
+  DevBuf<uint32_t> d_win_count;
   // n-best / sampling; pieces: the candidates' token ends and the exported normalized texts (NbestOut)
   DevBuf<uint8_t> d_nb_scratch, d_nb_norm;
   DevBuf<uint32_t> d_nb_end;
@@ -3765,6 +3770,82 @@ int spm_encode_offsets(spm_engine *e, const char *bytes, const uint64_t *offsets
 static constexpr uint32_t kOpadInlineCuts = 32;
 static constexpr size_t kOpadHead = 4;
 
+// offsets_plan_kernel behind a device batch's encode, into d_opad (sized and its head zeroed here); the caller copies
+// the head back (into h_opad, sized here too).
+static int queue_offsets_plan(spm_engine *e, const uint64_t *d_offsets, uint32_t n32, uint32_t expand, cudaStream_t st) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  CUDA_TRY(e->d_opad.ensure(std::max<size_t>(kOpadHead + 2 * kOpadInlineCuts, kOpadHead + 2 * (size_t{n32} + 1))));
+  CUDA_TRY(e->h_opad.ensure(e->d_opad.cap));
+  CUDA_TRY(cudaMemsetAsync(e->d_opad.p, 0, kOpadHead * sizeof(unsigned long long), st));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n32 + 255) / 256));
+  offsets_plan_kernel<<<grid, 256, 0, st>>>(d_offsets, n32, expand, kNormChunkSlab,
+                                            static_cast<uint32_t>((e->d_opad.cap - kOpadHead) / 2), e->d_opad.p);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  return SPM_OK;
+}
+
+// K11 over a device batch in the chunks that offsets_plan_kernel cut (its head already read into h_opad): fetches the
+// cuts past the first kOpadInlineCuts, then queues one launch per chunk on st, behind ev[0].  A's outputs (packed or
+// padded mode, as `padded` says) are set by the caller; P is the raw segmentation, which gets the frame and the piece
+// table here.
+static int offsets_device_chunks(spm_engine *e, bool padded, KPieces P, KOffsets &A, const uint8_t *d_base,
+                                 const uint64_t *d_offsets, size_t n, uint32_t expand, int32_t eos_id, cudaStream_t st,
+                                 uint64_t *d2h) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  const size_t head = kOpadHead + 2 * kOpadInlineCuts;
+  const unsigned long long *plan = e->h_opad.p;
+  const uint64_t chunks = plan[0], slab_max = plan[1];
+  if (chunks > kOpadInlineCuts) {  // (over 2^32 slab elements of input)
+    const size_t rest = 2 * (chunks - kOpadInlineCuts);
+    CUDA_TRY(cudaMemcpyAsync(e->h_opad.p + head, e->d_opad.p + head, rest * sizeof(unsigned long long),
+                             cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *d2h += rest * sizeof(unsigned long long);
+  }
+  P.F = e->kframe();
+  P.pc_off = e->d_pc_off.p;
+  P.pc_bytes = e->d_pc_bytes.p;
+  P.unk_id = e->unk_id;
+  CUDA_TRY(e->d_tmp_norm.ensure(slab_max + 16));
+  CUDA_TRY(e->d_tmp_n2o.ensure(slab_max + 16));
+  CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, sizeof(uint32_t), st));
+  KModel M = e->km;
+  M.hot_link = M.hot_val = 0;
+  A.P = P;
+  A.offsets = d_offsets;
+  A.expand = expand;
+  A.slab_text = e->d_tmp_norm.p;
+  A.slab_n2o = e->d_tmp_n2o.p;
+  A.eos_id = eos_id;
+  A.status = e->d_ctrl32.p;
+  CUDA_TRY(cudaEventRecord(e->ev[0], st));  // (raw_segmentation_device has read ev[0] / ev[1])
+  for (uint64_t c = 0; c < chunks; ++c) {
+    A.first = static_cast<uint32_t>(plan[kOpadHead + 2 * c]);
+    A.n = static_cast<uint32_t>((c + 1 < chunks ? plan[kOpadHead + 2 * (c + 1)] : n) - A.first);
+    A.bytes = d_base + plan[kOpadHead + 2 * c + 1];
+    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (A.n + 7) / 8));
+    if (padded) offsets_padded_kernel<<<grid, 256, 0, st>>>(M, A);
+    else offsets_kernel<<<grid, 256, 0, st>>>(M, A);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  return SPM_OK;
+}
+
+// K11's status word, read back: its errors as spm_encode_offsets reports them.
+static int offsets_status(spm_engine *e) {
+  if (e->h_ctrl32.p[0] & 2u) {
+    e->set_error("encode offsets: a sentence normalized to more bytes than its bound");
+    return SPM_ERR_ENCODE;
+  }
+  if (e->h_ctrl32.p[0]) {
+    e->set_error("encode offsets: all normalized characters are not consumed");
+    return SPM_ERR_ENCODE;
+  }
+  return SPM_OK;
+}
+
 int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
                                      uint64_t total_bytes, int32_t eos_id, int32_t *d_ids, int32_t *d_spans,
                                      uint64_t out_capacity, uint32_t width, int32_t pad_id, uint32_t flags,
@@ -3806,17 +3887,13 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
   const uint32_t n32 = static_cast<uint32_t>(n);
   const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
   const size_t head = kOpadHead + 2 * kOpadInlineCuts;
-  CUDA_TRY(e->d_opad.ensure(std::max(head, kOpadHead + 2 * (n + 1))));
-  CUDA_TRY(e->h_opad.ensure(e->d_opad.cap));
   uint64_t d2h = 0;
   auto at_read = [&]() -> int {
-    CUDA_TRY(cudaMemsetAsync(e->d_opad.p, 0, kOpadHead * sizeof(unsigned long long), st));
+    SPM_TRY(queue_offsets_plan(e, d_offsets, n32, expand, st));
     const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 255) / 256));
     row_max_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, frame, e->d_opad.p + 3);
-    offsets_plan_kernel<<<grid, 256, 0, st>>>(d_offsets, n32, expand, kNormChunkSlab, static_cast<uint32_t>((e->d_opad.cap - kOpadHead) / 2),
-                                              e->d_opad.p);
     CUDA_TRY(cudaGetLastError());
-    e->last_launches += 2;
+    ++e->last_launches;
     CUDA_TRY(cudaMemcpyAsync(e->h_opad.p, e->d_opad.p, head * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
     d2h += head * sizeof(unsigned long long);
     return SPM_OK;
@@ -3827,7 +3904,7 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
   CUDA_TRY(cudaEventRecord(e->ev[3], st));
   SPM_TRY(e->raw_segmentation_device(d_base, d_offsets, n, total_bytes, true, &P, &raw_ids, &main_ms, st, at_read));
   const unsigned long long *plan = e->h_opad.p;
-  const uint64_t chunks = plan[0], slab_max = plan[1], longest_input = plan[2], longest = plan[3];
+  const uint64_t longest_input = plan[2], longest = plan[3];
   if (norm_slab_start(longest_input, 1, expand) > 0x7FFFFF00ull) {
     set_error("sentence too long for the device path");
     return SPM_ERR_UNSUPPORTED;
@@ -3845,31 +3922,8 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
     set_error("out_capacity too small: need " + std::to_string(static_cast<unsigned long long>(n) * w));
     return SPM_ERR_CAPACITY;
   }
-  if (chunks > kOpadInlineCuts) {  // (over 2^32 slab elements of input)
-    const size_t rest = 2 * (chunks - kOpadInlineCuts);
-    CUDA_TRY(cudaMemcpyAsync(e->h_opad.p + head, e->d_opad.p + head, rest * sizeof(unsigned long long),
-                             cudaMemcpyDeviceToHost, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    d2h += rest * sizeof(unsigned long long);
-  }
   // ---- K11, padded: the rows ----
-  P.F = e->kframe();
-  P.pc_off = e->d_pc_off.p;
-  P.pc_bytes = e->d_pc_bytes.p;
-  P.unk_id = e->unk_id;
-  CUDA_TRY(e->d_tmp_norm.ensure(slab_max + 16));
-  CUDA_TRY(e->d_tmp_n2o.ensure(slab_max + 16));
-  CUDA_TRY(cudaMemsetAsync(e->d_ctrl32.p, 0, sizeof(uint32_t), st));
-  KModel M = e->km;
-  M.hot_link = M.hot_val = 0;
   KOffsets A{};
-  A.P = P;
-  A.offsets = d_offsets;
-  A.expand = expand;
-  A.slab_text = e->d_tmp_norm.p;
-  A.slab_n2o = e->d_tmp_n2o.p;
-  A.eos_id = eos_id;
-  A.status = e->d_ctrl32.p;
   A.pad_ids = d_ids;
   A.spans = reinterpret_cast<int2 *>(d_spans);
   A.lengths = d_lengths;
@@ -3877,19 +3931,11 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
   A.pad_id = pad_id;
   A.truncate = truncate ? 1u : 0u;
   A.left = (flags & SPM_PAD_LEFT) ? 1u : 0u;
-  CUDA_TRY(cudaEventRecord(e->ev[0], st));  // (raw_segmentation_device has read ev[0] / ev[1])
-  for (uint64_t c = 0; c < chunks; ++c) {
-    A.first = static_cast<uint32_t>(plan[kOpadHead + 2 * c]);
-    A.n = static_cast<uint32_t>((c + 1 < chunks ? plan[kOpadHead + 2 * (c + 1)] : n) - A.first);
-    A.bytes = d_base + plan[kOpadHead + 2 * c + 1];
-    const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (A.n + 7) / 8));
-    offsets_padded_kernel<<<grid, 256, 0, st>>>(M, A);
-    CUDA_TRY(cudaGetLastError());
-    ++e->last_launches;
-  }
+  SPM_TRY(offsets_device_chunks(e, true, P, A, d_base, d_offsets, n, expand, eos_id, st, &d2h));
   if (flags & SPM_OFFSETS_CHARS) {
     const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
-    spans_to_chars_kernel<<<grid, 256, 0, st>>>(d_base, d_offsets, n32, A.spans, d_lengths, w, P.F, eos_id, A.left);
+    spans_to_chars_kernel<<<grid, 256, 0, st>>>(d_base, d_offsets, n32, A.spans, d_lengths, w, e->kframe(), eos_id,
+                                                A.left);
     CUDA_TRY(cudaGetLastError());
     ++e->last_launches;
   }
@@ -3898,14 +3944,175 @@ int spm_encode_offsets_device_padded(spm_engine *e, const char *d_bytes, const u
   CUDA_TRY(cudaEventRecord(e->ev[2], st));
   CUDA_TRY(cudaStreamSynchronize(st));
   d2h += sizeof(uint32_t);
-  if (e->h_ctrl32.p[0] & 2u) {
-    set_error("encode offsets: a sentence normalized to more bytes than its bound");
-    return SPM_ERR_ENCODE;
+  SPM_TRY(offsets_status(e));
+  e->last_d2h = d2h;
+  float k_ms = 0.f, all = 0.f;
+  e->last_main_ms = main_ms + (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess ? k_ms : 0.f);
+  e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : e->last_main_ms;
+  (void)cudaGetLastError();
+  return SPM_OK;
+}
+
+// spm_encode_windows_device: a device batch as overlapping windows of one width.
+//   1. the encode: encode_stage (ids only), or the raw segmentation with the unknown detour (offsets);
+//   2. behind it, while d_sent_count holds the raw counts, windows_plan: the windows per sentence, their exclusive scan
+//      (each sentence's first row, R in total) and the longest body, read back in the call's one status read (with
+//      offsets, the detour count's, which also brings the K11 chunk plan);
+//   3. the checks on the longest body and R, then window_rows_kernel (row_sentence / row_first);
+//   4. ids only: write_windows_kernel from the raw ids, as the padded call writes its rows.  Offsets: K11 in packed
+//      mode (framed ids, begin, end; each token walked once), lists_to_chars_kernel with SPM_OFFSETS_CHARS, then
+//      write_window_spans_kernel gathers every row from the packed lists.
+static int windows_plan(spm_engine *e, uint32_t n32, uint32_t B, uint32_t step, cudaStream_t st, uint64_t *d2h) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  CUDA_TRY(e->d_win.ensure(size_t{n32} + 3));
+  CUDA_TRY(e->h_win.ensure(2));
+  CUDA_TRY(e->d_win_count.ensure(n32));
+  CUDA_TRY(cudaMemsetAsync(e->d_win.p + 1, 0, sizeof(unsigned long long), st));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n32 + 255) / 256));
+  row_max_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, 0u, e->d_win.p + 1);
+  window_count_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, B, step, e->d_win_count.p);
+  CUDA_TRY(cudaGetLastError());
+  e->last_launches += 2;
+  SPM_TRY(e->scan_total(e->d_win_count.p, n32, 0, e->d_win.p, st));
+  SPM_TRY(e->scan_gather<uint8_t>(e->d_win_count.p, n32, e->d_win.p + 2, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  CUDA_TRY(cudaMemcpyAsync(e->h_win.p, e->d_win.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  *d2h += 2 * sizeof(unsigned long long);
+  return SPM_OK;
+}
+
+int spm_encode_windows_device(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                              uint64_t total_bytes, uint32_t width, uint32_t stride, int32_t pad_id, uint32_t flags,
+                              int32_t eos_id, int32_t *d_ids, int32_t *d_spans, uint64_t rows_capacity,
+                              int32_t *d_lengths, int32_t *d_row_sentence, int32_t *d_row_first, uint64_t *rows_out,
+                              void *stream) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!d_offsets || !rows_out || (n && (!d_ids || !d_lengths || !d_row_sentence || !d_row_first)) ||
+      (n && !d_bytes && total_bytes)) {
+    set_error("null argument");
+    return SPM_ERR_ARG;
   }
-  if (e->h_ctrl32.p[0]) {
-    set_error("encode offsets: all normalized characters are not consumed");
-    return SPM_ERR_ENCODE;
+  if (n >= 0xFFFFFFF0ull) { set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  if (reinterpret_cast<uintptr_t>(d_spans) % 8u) {  // (the kernels store (begin, end) as one 8-byte pair)
+    set_error("d_spans must be 8-byte aligned");
+    return SPM_ERR_ARG;
   }
+  if (flags & SPM_PAD_TRUNCATE) { set_error("windows keep every token: SPM_PAD_TRUNCATE does not apply"); return SPM_ERR_ARG; }
+  if (flags & ~static_cast<uint32_t>(SPM_PAD_LEFT | SPM_OFFSETS_CHARS)) { set_error("unknown flags"); return SPM_ERR_ARG; }
+  if ((flags & SPM_OFFSETS_CHARS) && !d_spans) { set_error("SPM_OFFSETS_CHARS needs d_spans"); return SPM_ERR_ARG; }
+  if (width == 0) { set_error("windows need a fixed width"); return SPM_ERR_ARG; }
+  const uint32_t frame = e->frame_np + e->frame_ns;
+  if (width <= frame) {
+    set_error("width " + std::to_string(width) + " leaves no body next to the encode frame (" + std::to_string(frame) +
+              " ids)");
+    return SPM_ERR_ARG;
+  }
+  const uint32_t B = width - frame;
+  if (stride >= B) {
+    set_error("stride " + std::to_string(stride) + " must be less than the window's body of " + std::to_string(B) + " ids");
+    return SPM_ERR_ARG;
+  }
+  const uint32_t step = B - stride;
+  const uint32_t left = (flags & SPM_PAD_LEFT) ? 1u : 0u;
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  *rows_out = 0;
+  if (n == 0) {
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SPM_OK;
+  }
+  e->last_h2d = e->last_d2h = 0;
+  const bool spans = d_spans != nullptr;
+  const uint8_t *d_base = reinterpret_cast<const uint8_t *>(d_bytes);
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
+  if (spans) {
+    e->last_unk_detour = 0;
+    SPM_TRY(e->ensure_piece_tables());
+  }
+  if (e->model.model_type == SPM_UNIGRAM) SPM_TRY(e->pick_fast_words_device(d_base, d_offsets, n, st, &e->batch_fast_words));
+  uint64_t d2h = 0;
+  KPieces P{};
+  uint64_t raw_ids = 0;
+  float main_ms = 0.f;
+  if (!spans) {
+    SPM_TRY(e->encode_stage(d_base, d_offsets, n, total_bytes, false, st));
+    SPM_TRY(windows_plan(e, n32, B, step, st, &d2h));
+    CUDA_TRY(cudaStreamSynchronize(st));
+  } else {
+    const size_t head = kOpadHead + 2 * kOpadInlineCuts;
+    auto at_read = [&]() -> int {
+      SPM_TRY(queue_offsets_plan(e, d_offsets, n32, expand, st));
+      CUDA_TRY(cudaMemcpyAsync(e->h_opad.p, e->d_opad.p, head * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      d2h += head * sizeof(unsigned long long);
+      return windows_plan(e, n32, B, step, st, &d2h);
+    };
+    CUDA_TRY(cudaEventRecord(e->ev[3], st));
+    SPM_TRY(e->raw_segmentation_device(d_base, d_offsets, n, total_bytes, true, &P, &raw_ids, &main_ms, st, at_read));
+    if (norm_slab_start(e->h_opad.p[2], 1, expand) > 0x7FFFFF00ull) {
+      set_error("sentence too long for the device path");
+      return SPM_ERR_UNSUPPORTED;
+    }
+  }
+  // ---- the rows: their number decides whether the call fails ----
+  const unsigned long long R = e->h_win.p[0], longest = e->h_win.p[1];
+  if (longest > 0x7FFFFFFFull) {
+    set_error("a sentence of " + std::to_string(longest) + " ids is longer than 2^31 - 1 ids");
+    return SPM_ERR_UNSUPPORTED;
+  }
+  if (R > 0x7FFFFFFFull) { set_error(std::to_string(R) + " rows do not fit int32"); return SPM_ERR_UNSUPPORTED; }
+  *rows_out = R;
+  if (R > rows_capacity) {
+    set_error("rows_capacity too small: need " + std::to_string(R) + " rows");
+    return SPM_ERR_CAPACITY;
+  }
+  const uint32_t R32 = static_cast<uint32_t>(R);
+  const int sgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  const int rgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (R + 7) / 8));
+  window_rows_kernel<<<sgrid, 256, 0, st>>>(e->d_win.p + 2, n32, step, d_row_sentence, d_row_first);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  if (!spans) {
+    write_windows_kernel<<<rgrid, 256, 0, st>>>(e->d_sent_count.p, e->d_sent_start.p, e->d_tmp_ids.p, R32, e->kframe(),
+                                                width, pad_id, left, d_ids, d_lengths, d_row_sentence, d_row_first);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+    CUDA_TRY(cudaEventRecord(e->ev[2], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    e->last_d2h = d2h;
+    finish_timing(e);
+    return SPM_OK;
+  }
+  // ---- K11, packed: every token's begin / end once, then the rows ----
+  const uint64_t tids = raw_ids + static_cast<uint64_t>(n) * frame;
+  CUDA_TRY(e->d_off_begin.ensure(tids + 1));
+  CUDA_TRY(e->d_off_end.ensure(tids + 1));
+  CUDA_TRY(e->d_pc_out_ids.ensure(tids + 1));
+  CUDA_TRY(e->d_pc_out_id_offsets.ensure(n + 1));
+  KOffsets A{};
+  A.begin = e->d_off_begin.p;
+  A.end = e->d_off_end.p;
+  A.out_ids = e->d_pc_out_ids.p;
+  A.out_id_offsets = e->d_pc_out_id_offsets.p;
+  SPM_TRY(offsets_device_chunks(e, false, P, A, d_base, d_offsets, n, expand, eos_id, st, &d2h));
+  if (flags & SPM_OFFSETS_CHARS) {
+    lists_to_chars_kernel<<<sgrid, 256, 0, st>>>(d_base, d_offsets, n32, A.begin, A.end, A.out_id_offsets, e->kframe(),
+                                                 eos_id);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  write_window_spans_kernel<<<rgrid, 256, 0, st>>>(A.out_ids, A.begin, A.end, A.out_id_offsets, R32, d_row_sentence,
+                                                   d_row_first, e->frame_np, frame, width, pad_id, left, d_ids,
+                                                   reinterpret_cast<int2 *>(d_spans), d_lengths);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  CUDA_TRY(cudaEventRecord(e->ev[1], st));
+  SPM_TRY(e->copy_status(st, 1, 0));
+  CUDA_TRY(cudaEventRecord(e->ev[2], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  d2h += sizeof(uint32_t);
+  SPM_TRY(offsets_status(e));
   e->last_d2h = d2h;
   float k_ms = 0.f, all = 0.f;
   e->last_main_ms = main_ms + (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess ? k_ms : 0.f);

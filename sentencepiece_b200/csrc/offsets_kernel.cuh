@@ -27,6 +27,9 @@
 // else q; B = L, or min(L, w - np - ns) when truncating), the suffix, all shifted by w - real when padding on the left,
 // and pad_id / (0, 0) in the other cells.  Tokens past B are walked (the lengths still have to add up) but not stored.
 //
+// Windows (spm_encode_windows_device) run K11 in packed mode, once per sentence, and write_window_spans_kernel gathers
+// each window row from the packed lists: a token that lies in several windows is walked once.
+//
 // The byte-fallback grouping assumes the normalized text is valid UTF-8, so that every unknown piece is exactly one
 // character.  The normalizer guarantees that for every input (a malformed byte becomes U+FFFD) as long as the
 // model's charsmap targets are valid UTF-8; the engine refuses models whose targets are not.
@@ -195,6 +198,43 @@ __global__ void __launch_bounds__(256, 1) offsets_kernel(const KModel M, const K
 
 __global__ void __launch_bounds__(256, 1) offsets_padded_kernel(const KModel M, const KOffsets A) {
   offsets_walk<true>(M, A);
+}
+
+// The offset rows of spm_encode_windows_device: one warp per window row, gathered from K11's framed, packed output
+// (ids, begin, end; sentence i's list at id_offsets[i], np + L + ns entries).  Window f of sentence i takes the list's
+// entries [0, np), [np + f, np + f + b) and [np + L, np + L + ns), b = min(L - f, w - np - ns), laid out as
+// write_windows_kernel (padded_kernel.cuh) lays out its id rows, and pad_id / (0, 0) in the other cells.
+__global__ void __launch_bounds__(256) write_window_spans_kernel(const int32_t *ids, const uint32_t *begin,
+                                                                 const uint32_t *end,
+                                                                 const unsigned long long *id_offsets, uint32_t rows,
+                                                                 const int32_t *row_sentence, const int32_t *row_first,
+                                                                 uint32_t np, uint32_t fr, uint32_t w, int32_t pad_id,
+                                                                 uint32_t left, int32_t *out, int2 *spans,
+                                                                 int32_t *lengths) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+    const uint32_t i = static_cast<uint32_t>(row_sentence[row]), f = static_cast<uint32_t>(row_first[row]);
+    const unsigned long long o = id_offsets[i];
+    const uint32_t L = static_cast<uint32_t>(id_offsets[i + 1] - o) - fr;
+    const uint32_t body = min(L - f, w - fr);
+    const uint32_t real = body + fr;
+    const uint32_t lead = left ? w - real : 0u;
+    int32_t *ro = out + static_cast<unsigned long long>(row) * w;
+    int2 *rs = spans + static_cast<unsigned long long>(row) * w;
+    for (uint32_t t = lane; t < w; t += 32) {
+      const uint32_t k = t - lead;  // wraps past `real` for the leading pad cells
+      if (k < real) {
+        const unsigned long long q = o + (k < np ? k : k < np + body ? k + f : k + L - body);
+        __stcs(ro + t, ids[q]);
+        __stcs(rs + t, make_int2(static_cast<int32_t>(begin[q]), static_cast<int32_t>(end[q])));
+      } else {
+        __stcs(ro + t, pad_id);
+        __stcs(rs + t, make_int2(0, 0));
+      }
+    }
+    if (lane == 0) lengths[row] = static_cast<int32_t>(real);
+  }
 }
 
 // The chunk plan of a device batch (spm_encode_offsets_device_padded): the cuts spm_encode_offsets makes on the host

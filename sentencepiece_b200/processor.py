@@ -251,6 +251,7 @@ class Engine:
         self.device = device
         self._model_bytes = model_bytes
         self._pad_guess = 64  # cells per row encode_device_padded(width=0) allocates first: the last such call's width
+        self._win_ratio = 1.0  # rows per sentence encode_device_windows allocates first: the last call's R / n
         self._pad = None  # pad_id(), read from the model on first use
 
     def close(self):
@@ -666,6 +667,77 @@ class Engine:
         flat = cells.view(-1)
         return flat[:n * w].view(n, w), flat[at:at + 2 * n * w].view(n, w, 2), lengths
 
+    def encode_device_windows(self, d_bytes, d_offsets, width, stride=0, pad_id=None, pad_left=False, unit=None,
+                              eos_id=None, out=None):
+        """spm_encode_windows_device: a batch already on the GPU as overlapping windows of `width` cells, each holding
+        the encode frame and up to B = width - np - ns body ids; every window after a sentence's first starts
+        B - stride ids later, so long sentences keep every token -> (ids int32 [R, w], lengths int32 [R],
+        row_sentence int32 [R], row_first int32 [R]), plus spans int32 [R, w, 2] when unit is "byte" or "char" (None:
+        no offsets).  row_sentence[r] is the sentence of row r, row_first[r] the index of its first body id in the
+        sentence's body.  Cells, pad_id, pad_left, eos_id and the spans as encode_offsets_device_padded gives them.
+        Without `out`, the rows go to max(n, guess) new rows, guess scaling the previous call's R / n; when R is larger,
+        the call is repeated into exactly R rows, which encodes the batch a second time.  out: a contiguous int32 tensor
+        of at least R * w cells (3 * R * w + 1 with spans: the ids, then the spans at an even cell) plus 3 * R for the
+        lengths and the two row maps (ValueError when too small)."""
+        import torch
+        if unit not in (None, "byte", "char"):
+            raise ValueError('unit must be None, "byte" or "char"')
+        if pad_id is None:
+            pad_id = self.pad_id()
+            if pad_id < 0:
+                raise ValueError("the model defines no pad piece (trainer_spec.pad_piece): pass pad_id explicitly")
+        if eos_id is None:
+            from . import _modelinfo
+            eos_id = _modelinfo.special_pieces(self._model_bytes)["eos_id"]
+        st = self._stream(d_bytes, d_offsets, out)
+        if d_bytes.dtype != torch.uint8 or d_bytes.dim() != 1 or not d_bytes.is_contiguous():
+            raise ValueError("d_bytes must be a contiguous 1-D uint8 tensor")
+        if d_offsets.dtype not in (torch.int64, torch.uint64) or d_offsets.dim() != 1 or not d_offsets.is_contiguous():
+            raise ValueError("d_offsets must be a contiguous 1-D int64 or uint64 tensor of n + 1 offsets")
+        if out is not None and (out.dtype != torch.int32 or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int32 tensor")
+        n = d_offsets.numel() - 1
+        flags = (_capi.PAD_LEFT if pad_left else 0) | (_capi.OFFSETS_CHARS if unit == "char" else 0)
+        per_row = 3 * width + 3 if unit else width + 3  # cells a row takes: ids (and spans), length, sentence, first
+
+        def layout(cells):
+            rows = max(cells.numel() - (1 if unit else 0), 0) // per_row
+            sp_at = rows * width + ((rows * width) & 1)  # the spans start at an even cell (8-byte aligned)
+            len_at = sp_at + 2 * rows * width if unit else rows * width
+            return rows, sp_at, len_at
+
+        def call(cells):
+            rows, sp_at, len_at = layout(cells)
+            p = cells.data_ptr()
+            r = ctypes.c_uint64()
+            rc = self._lib.spm_encode_windows_device(self._h, d_bytes.data_ptr(), d_offsets.data_ptr(), n,
+                                                     d_bytes.numel(), width, stride, pad_id, flags, eos_id, p,
+                                                     p + 4 * sp_at if unit else None, rows, p + 4 * len_at,
+                                                     p + 4 * (len_at + rows), p + 4 * (len_at + 2 * rows),
+                                                     ctypes.byref(r), st)
+            return rc, r.value
+
+        def alloc(rows):
+            return torch.empty(rows * per_row + (1 if unit else 0), dtype=torch.int32, device=d_bytes.device)
+
+        cells = out if out is not None else alloc(max(n, int(n * self._win_ratio + 0.5), 1))
+        rc, R = call(cells)
+        if rc == _capi.SPM_ERR_CAPACITY and out is None:
+            cells = alloc(R)
+            rc, R = call(cells)
+        if rc == _capi.SPM_ERR_CAPACITY:
+            raise ValueError(self._lib.spm_last_error(self._h).decode())
+        self._check(rc)
+        if n:
+            self._win_ratio = R / n
+        rows, sp_at, len_at = layout(cells)
+        flat = cells.view(-1)
+        res = (flat[:R * width].view(R, width), flat[len_at:len_at + R], flat[len_at + rows:len_at + rows + R],
+               flat[len_at + 2 * rows:len_at + 2 * rows + R])
+        if unit:
+            res += (flat[sp_at:sp_at + 2 * R * width].view(R, width, 2),)
+        return res
+
     def decode_device(self, ids2d, lengths=None, stop_id=-1):
         """spm_decode_ids_device: the rows of an int32 or int64 [n, L] CUDA tensor (any row stride, e.g. a column slice;
         each row contiguous) -> list of n str.  Row i holds min(L, lengths[i]) ids (lengths: int32 [n], or None for L),
@@ -974,14 +1046,7 @@ class SentencePieceProcessor:
         ids[i, j] in characters of input i, as ConvertToUnicodeSpans counts them (EncodeAsImmutableProto's begin /
         end; eos gets (len, len), bos and pad cells (0, 0))."""
         self._require()
-        if isinstance(input, tuple):
-            d_bytes, d_offs = input
-        else:
-            import torch
-            buf, offs = pack_sentences(input)
-            dev = torch.device("cuda", self._engine.device)
-            d_bytes = torch.from_numpy(np.require(buf, requirements="W")).pin_memory().to(dev, non_blocking=True)
-            d_offs = torch.from_numpy(offs.view(np.int64)).pin_memory().to(dev, non_blocking=True)
+        d_bytes, d_offs = self._device_batch(input)
         self._set_frame(add_bos, add_eos, reverse)
         if return_offsets:
             ids, spans, lengths = self._engine.encode_offsets_device_padded(
@@ -990,6 +1055,34 @@ class SentencePieceProcessor:
             return ids, lengths, spans
         return self._engine.encode_device_padded(d_bytes, d_offs, width=max_len or 0, pad_id=pad_id, truncate=truncate,
                                                  pad_left=pad_left)
+
+    def _device_batch(self, input):
+        """A list of str / bytes packed and uploaded through pinned memory, or a (bytes, offsets) pair of CUDA tensors
+        as it is."""
+        if isinstance(input, tuple):
+            return input
+        import torch
+        buf, offs = pack_sentences(input)
+        dev = torch.device("cuda", self._engine.device)
+        d_bytes = torch.from_numpy(np.require(buf, requirements="W")).pin_memory().to(dev, non_blocking=True)
+        d_offs = torch.from_numpy(offs.view(np.int64)).pin_memory().to(dev, non_blocking=True)
+        return d_bytes, d_offs
+
+    def encode_windows(self, input, max_len, stride=0, pad_id=None, pad_left=False, add_bos=False, add_eos=False,
+                       reverse=False, return_offsets=False):
+        """EncodeAsIds of a batch as overlapping windows of max_len cells on the GPU, for inputs longer than a model's
+        width: each window holds bos / eos and up to B = max_len - (bos + eos) ids, and a sentence's windows start
+        B - stride ids apart, so no token is dropped -> (ids int32 [R, w], lengths int32 [R], row_sentence int32 [R],
+        row_first int32 [R]) on the engine's device.  row_sentence[r] is the input row r comes from, row_first[r] the
+        index of its first id in the sentence's ids (without bos / eos).  input, pad_id and pad_left as
+        encode_padded.  return_offsets: -> (ids, lengths, row_sentence, row_first, offsets int32 [R, w, 2]), the
+        offsets in characters as encode_padded(return_offsets=True) gives them."""
+        self._require()
+        d_bytes, d_offs = self._device_batch(input)
+        self._set_frame(add_bos, add_eos, reverse)
+        return self._engine.encode_device_windows(d_bytes, d_offs, max_len, stride=stride, pad_id=pad_id,
+                                                  pad_left=pad_left, unit="char" if return_offsets else None,
+                                                  eos_id=self._specials()["eos_id"])
 
     def decode_padded(self, ids, lengths=None, stop_id=None):
         """DecodeIds of every row of an int32 / int64 [n, L] CUDA tensor -> list of n str: row i holds lengths[i] ids
