@@ -291,6 +291,62 @@ int spm_encode_windows_device(spm_engine *e, const char *d_bytes, const uint64_t
                               int32_t *d_lengths, int32_t *d_row_sentence, int32_t *d_row_first,
                               uint64_t *rows_out, void *stream);
 
+/* Sentence pairs: two inputs per padded row, for cross-encoders and rerankers (query, passage), NLI and paraphrase
+ * classifiers (premise, hypothesis) and extractive QA (question, context).
+ * The device batch holds 2n sentences (d_offsets: 2n + 1 entries): pair i is A_i = sentence i and B_i = sentence n + i,
+ * each as the raw ids spm_encode_ids_device gives it with no frame.  The engine's encode frame does not apply to this
+ * call (it stays set for later calls); the call's own template does: prefix, middle and suffix (host arrays of at most
+ * 64 ids each in [0, vocab); T = n_prefix + n_middle + n_suffix).  The row of pair i before truncation is
+ *   prefix ++ A_i ++ middle ++ B_i ++ suffix
+ * which covers T5's "A </s> B </s>", "<s> A </s></s> B </s>" and "[CLS] A [SEP] B [SEP]".
+ * Truncation (`truncation`), with a = |A_i|, b = |B_i| and the body room Bt = width - T (width > T required):
+ *   SPM_PAIR_TRUNC_NONE: nothing is cut.  width == 0 takes the longest row of the batch as w; a fixed width that some
+ *     row exceeds gives SPM_ERR_CAPACITY with the longest row in *width_out.
+ *   SPM_PAIR_TRUNC_LONGEST_FIRST: while a + b > Bt, the last id of the longer body is dropped (B's on ties); that is
+ *     a' = min(a, max(Bt - b, ceil(Bt / 2))), b' = min(b, Bt - a').
+ *   SPM_PAIR_TRUNC_ONLY_FIRST / _ONLY_SECOND: only that member is cut, from its end, to the room r = Bt - |other|.
+ *   Only right truncation is offered.  These rules are this project's definitions, not a claim of parity with any other
+ *   library's truncation.
+ * SPM_PAIR_OVERFLOW (flag; with ONLY_FIRST / ONLY_SECOND only): the cut member is not dropped but split into windows as
+ *   spm_encode_windows_device splits a body, with room r_i = Bt - |other_i| and step s_i = r_i - stride per pair.  Pair
+ *   i gets 1 row if the member fits, else 1 + ceil((L - r_i) / s_i) rows (L: the member's length); window j holds
+ *   the member's ids [j*s_i, min(j*s_i + r_i, L)), and every row repeats the template and the whole other member.
+ *   Without the flag, stride must be 0.
+ * A pair under ONLY_* that needs cutting but has r_i < 1 (or r_i <= stride under overflow) cannot be laid out: the call
+ * returns SPM_ERR_CAPACITY with *rows_out = 0 and in *width_out the least width at which every pair would pass.
+ * Outputs, for R rows (R = n without the overflow flag; rows ordered by pair, then window) of width w (*width_out):
+ *   d_ids int32 [R, w]: the row, then pad_id (SPM_PAD_LEFT: the real cells at the end of the row).
+ *   d_type_ids int32 [R, w] (required): 0 on the prefix, A's cells and the middle; 1 on B's cells and the suffix; 0 on
+ *     pad cells.
+ *   d_lengths, d_row_pair, d_row_first int32 [R]: the real cells; the pair of the row; the index of the window's first
+ *     id within the windowed member's ids (0 without the overflow flag).
+ *   d_spans (optional, int32 [R, w, 2], 8-byte aligned; NULL = no offsets): an A cell holds its token's (begin, end) in
+ *     A's input, a B cell its token's (begin, end) in B's input, as spm_encode_offsets gives them; template and pad
+ *     cells (0, 0).  SPM_OFFSETS_CHARS counts characters as spm_encode_offsets_device_padded does.  A sentence too long
+ *     for the offsets path, SPM_ERR_ENCODE on unconsumed characters and the unknown-id detour are as there.
+ * Capacities: d_lengths, d_row_pair and d_row_first hold rows_capacity entries, d_ids and d_type_ids cells_capacity
+ * cells and d_spans 2 * cells_capacity.  R > rows_capacity or R * w > cells_capacity gives SPM_ERR_CAPACITY with R in
+ * *rows_out and w in *width_out; like the width failure above, it writes nothing to any output (a retry encodes the
+ * batch again).  On success *rows_out = R, *width_out = w.
+ * SPM_ERR_ARG: null pointers, unknown flags or strategy, SPM_PAD_TRUNCATE, a template list over 64 ids or an id
+ * outside [0, vocab), width 0 or width <= T with any strategy but NONE, the overflow flag with NONE or LONGEST_FIRST,
+ * stride != 0 without it, SPM_OFFSETS_CHARS without d_spans, a misaligned d_spans, 2n over the sentence limit.
+ * SPM_ERR_UNSUPPORTED: a row of 2^32 - 1 ids or more, R over 2^31 - 1.  n == 0 succeeds with *rows_out = 0.  Stream
+ * and "returns after the work is done on `stream`" as the padded calls.  No per-token data crosses PCIe: the template
+ * goes up and a fixed number of status words come back. */
+enum {
+  SPM_PAIR_TRUNC_NONE = 0, SPM_PAIR_TRUNC_LONGEST_FIRST = 1, SPM_PAIR_TRUNC_ONLY_FIRST = 2,
+  SPM_PAIR_TRUNC_ONLY_SECOND = 3
+};
+enum { SPM_PAIR_OVERFLOW = 8 };
+int spm_encode_pairs_device(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                            uint64_t total_bytes, const int32_t *prefix, uint32_t n_prefix, const int32_t *middle,
+                            uint32_t n_middle, const int32_t *suffix, uint32_t n_suffix, uint32_t width,
+                            uint32_t truncation, uint32_t stride, int32_t pad_id, uint32_t flags, int32_t *d_ids,
+                            int32_t *d_type_ids, int32_t *d_spans, uint64_t rows_capacity, uint64_t cells_capacity,
+                            int32_t *d_lengths, int32_t *d_row_pair, int32_t *d_row_first, uint64_t *rows_out,
+                            uint32_t *width_out, void *stream);
+
 /* ------------------------------------------------------------------------
  * N-best and sampling (unigram models; BASELINE.json config 5).
  *

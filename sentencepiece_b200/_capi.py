@@ -18,7 +18,7 @@ EXPORTS = [
     "spm_sample_encode_and_score", "spm_engine_cache_reset", "spm_engine_set_encode_frame", "spm_encode_pieces",
     "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
     "spm_encode_ids_device_padded", "spm_decode_ids_device", "spm_normalize", "spm_encode_offsets",
-    "spm_decode_offsets", "spm_encode_offsets_device_padded", "spm_encode_windows_device",
+    "spm_decode_offsets", "spm_encode_offsets_device_padded", "spm_encode_windows_device", "spm_encode_pairs_device",
 ]
 
 # spm_normalize: the n2o entry of a sentence whose reference norm_to_orig is empty
@@ -26,6 +26,9 @@ NORM_TO_ORIG_EMPTY = 0xFFFFFFFF
 
 # spm_encode_ids_device_padded flags, and spm_encode_offsets_device_padded's character offsets
 PAD_TRUNCATE, PAD_LEFT, OFFSETS_CHARS = 1, 2, 4
+# spm_encode_pairs_device: truncation strategies by name, and the overflow flag
+PAIR_TRUNCATION = {"none": 0, "longest_first": 1, "only_first": 2, "only_second": 3}
+PAIR_OVERFLOW = 8
 SPM_ERR_CAPACITY = 4
 
 
@@ -85,6 +88,9 @@ def load():
                                                    u32, vp, P(u32), vp]
     L.spm_encode_windows_device.argtypes = [vp, vp, vp, sz, u64, u32, u32, ctypes.c_int32, u32, ctypes.c_int32, vp, vp,
                                             u64, vp, vp, vp, P(u64), vp]
+    L.spm_encode_pairs_device.argtypes = [vp, vp, vp, sz, u64, P(ctypes.c_int32), u32, P(ctypes.c_int32), u32,
+                                          P(ctypes.c_int32), u32, u32, u32, u32, ctypes.c_int32, u32, vp, vp, vp, u64,
+                                          u64, vp, vp, vp, P(u64), P(u32), vp]
     L.spm_decode_ids_device.argtypes = [vp, vp, u32, u64, sz, u32, vp, ctypes.c_int64, P(vp), P(vp), vp]
     L.spm_host_alloc.argtypes = [sz]
     L.spm_host_alloc.restype = vp

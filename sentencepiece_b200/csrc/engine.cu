@@ -502,6 +502,11 @@ struct spm_engine {
   DevBuf<unsigned long long> d_win;
   PinBuf<unsigned long long> h_win;
   DevBuf<uint32_t> d_win_count;
+  // spm_encode_pairs_device (which also uses d_win / h_win / d_win_count): the template's ids, each pair's kept ids of
+  // A and B per row and the step between its windows
+  DevBuf<int32_t> d_pair_tmpl;
+  DevBuf<uint2> d_pair_keep;
+  DevBuf<uint32_t> d_pair_step;
   // n-best / sampling; pieces: the candidates' token ends and the exported normalized texts (NbestOut)
   DevBuf<uint8_t> d_nb_scratch, d_nb_norm;
   DevBuf<uint32_t> d_nb_end;
@@ -3463,22 +3468,25 @@ int spm_engine::raw_segmentation(const char *bytes, const uint64_t *offsets, siz
   return SPM_OK;
 }
 
+// The engine's encode frame switched off for the guard's scope, and restored when it ends.
+struct FrameOff {
+  spm_engine *e;
+  uint32_t np, ns;
+  bool rev;
+  explicit FrameOff(spm_engine *x) : e(x), np(x->frame_np), ns(x->frame_ns), rev(x->frame_rev) {
+    x->frame_np = x->frame_ns = 0;
+    x->frame_rev = false;
+  }
+  ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
+};
+
 int spm_engine::raw_segmentation_device(const uint8_t *d_bytes_base, const uint64_t *d_offs, size_t n,
                                         uint64_t total_bytes, bool detour, KPieces *P, uint64_t *raw_ids,
                                         float *main_ms, cudaStream_t st, const std::function<int()> &at_read) {
   // ---- 1. raw ids: the frame is written once, by K9 / K11 ----
   int rc;
   {
-    struct FrameOff {
-      spm_engine *e;
-      uint32_t np, ns;
-      bool rev;
-      explicit FrameOff(spm_engine *x) : e(x), np(x->frame_np), ns(x->frame_ns), rev(x->frame_rev) {
-        x->frame_np = x->frame_ns = 0;
-        x->frame_rev = false;
-      }
-      ~FrameOff() { e->frame_np = np; e->frame_ns = ns; e->frame_rev = rev; }
-    } off(this);
+    FrameOff off(this);
     rc = run_device(d_bytes_base, d_offs, n, total_bytes, false, nullptr, 0, nullptr, raw_ids, nullptr, st,
                     &d_pc_ids, &d_pc_id_offsets);
   }
@@ -4070,7 +4078,7 @@ int spm_encode_windows_device(spm_engine *e, const char *d_bytes, const uint64_t
   const uint32_t R32 = static_cast<uint32_t>(R);
   const int sgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
   const int rgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (R + 7) / 8));
-  window_rows_kernel<<<sgrid, 256, 0, st>>>(e->d_win.p + 2, n32, step, d_row_sentence, d_row_first);
+  window_rows_kernel<<<sgrid, 256, 0, st>>>(e->d_win.p + 2, n32, step, nullptr, d_row_sentence, d_row_first);
   CUDA_TRY(cudaGetLastError());
   ++e->last_launches;
   if (!spans) {
@@ -4105,6 +4113,213 @@ int spm_encode_windows_device(spm_engine *e, const char *d_bytes, const uint64_t
   write_window_spans_kernel<<<rgrid, 256, 0, st>>>(A.out_ids, A.begin, A.end, A.out_id_offsets, R32, d_row_sentence,
                                                    d_row_first, e->frame_np, frame, width, pad_id, left, d_ids,
                                                    reinterpret_cast<int2 *>(d_spans), d_lengths);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  CUDA_TRY(cudaEventRecord(e->ev[1], st));
+  SPM_TRY(e->copy_status(st, 1, 0));
+  CUDA_TRY(cudaEventRecord(e->ev[2], st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  d2h += sizeof(uint32_t);
+  SPM_TRY(offsets_status(e));
+  e->last_d2h = d2h;
+  float k_ms = 0.f, all = 0.f;
+  e->last_main_ms = main_ms + (cudaEventElapsedTime(&k_ms, e->ev[0], e->ev[1]) == cudaSuccess ? k_ms : 0.f);
+  e->last_ms = cudaEventElapsedTime(&all, e->ev[3], e->ev[2]) == cudaSuccess ? all : e->last_main_ms;
+  (void)cudaGetLastError();
+  return SPM_OK;
+}
+
+// spm_encode_pairs_device: 2n sentences as n pair rows (or more, when one member is cut into windows).
+//   1. the encode over the 2n sentences with the engine's frame off for the whole call (FrameOff): encode_stage (ids
+//      only), or the raw segmentation with the unknown detour (offsets);
+//   2. behind it, while d_sent_count holds the raw counts, pairs_plan: pair_plan_kernel (kept ids, rows and step per
+//      pair, the least workable width), the exclusive scan of the rows (R in total), read back in the call's one
+//      status read (with offsets, the detour count's, which also brings the K11 chunk plan);
+//   3. the width and R checks, then window_rows_kernel with the per-pair steps (row_pair / row_first);
+//   4. ids only: write_pair_rows_kernel from the raw ids.  Offsets: K11 in packed mode over the 2n sentences,
+//      lists_to_chars_kernel with SPM_OFFSETS_CHARS, then write_pair_spans_kernel gathers every row.
+static int pairs_plan(spm_engine *e, uint32_t n32, const KPairs &T, uint32_t w, uint32_t trunc, uint32_t overflow,
+                      uint32_t stride, cudaStream_t st, uint64_t *d2h) {
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  CUDA_TRY(e->d_win.ensure(size_t{n32} + 3));
+  CUDA_TRY(e->h_win.ensure(2));
+  CUDA_TRY(e->d_win_count.ensure(n32));
+  CUDA_TRY(e->d_pair_keep.ensure(n32));
+  CUDA_TRY(e->d_pair_step.ensure(n32));
+  CUDA_TRY(cudaMemsetAsync(e->d_win.p + 1, 0, sizeof(unsigned long long), st));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n32 + 255) / 256));
+  pair_plan_kernel<<<grid, 256, 0, st>>>(e->d_sent_count.p, n32, T, w, trunc, overflow, stride, e->d_pair_keep.p,
+                                         e->d_win_count.p, e->d_pair_step.p, e->d_win.p + 1);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  SPM_TRY(e->scan_total(e->d_win_count.p, n32, 0, e->d_win.p, st));
+  SPM_TRY(e->scan_gather<uint8_t>(e->d_win_count.p, n32, e->d_win.p + 2, nullptr, nullptr, nullptr, 0, 0, 0ull, st));
+  CUDA_TRY(cudaMemcpyAsync(e->h_win.p, e->d_win.p, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  *d2h += 2 * sizeof(unsigned long long);
+  return SPM_OK;
+}
+
+int spm_encode_pairs_device(spm_engine *e, const char *d_bytes, const uint64_t *d_offsets, size_t n,
+                            uint64_t total_bytes, const int32_t *prefix, uint32_t n_prefix, const int32_t *middle,
+                            uint32_t n_middle, const int32_t *suffix, uint32_t n_suffix, uint32_t width,
+                            uint32_t truncation, uint32_t stride, int32_t pad_id, uint32_t flags, int32_t *d_ids,
+                            int32_t *d_type_ids, int32_t *d_spans, uint64_t rows_capacity, uint64_t cells_capacity,
+                            int32_t *d_lengths, int32_t *d_row_pair, int32_t *d_row_first, uint64_t *rows_out,
+                            uint32_t *width_out, void *stream) {
+  if (!e) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (!d_offsets || !rows_out || !width_out ||
+      (n && (!d_ids || !d_type_ids || !d_lengths || !d_row_pair || !d_row_first)) || (n && !d_bytes && total_bytes) ||
+      (n_prefix && !prefix) || (n_middle && !middle) || (n_suffix && !suffix)) {
+    set_error("null argument");
+    return SPM_ERR_ARG;
+  }
+  if (n >= 0xFFFFFFF0ull / 2) { set_error("too many sentences in one call"); return SPM_ERR_ARG; }
+  if (reinterpret_cast<uintptr_t>(d_spans) % 8u) {  // (the kernels store (begin, end) as one 8-byte pair)
+    set_error("d_spans must be 8-byte aligned");
+    return SPM_ERR_ARG;
+  }
+  if (flags & SPM_PAD_TRUNCATE) { set_error("pairs truncate by their strategy: SPM_PAD_TRUNCATE does not apply"); return SPM_ERR_ARG; }
+  if (flags & ~static_cast<uint32_t>(SPM_PAD_LEFT | SPM_OFFSETS_CHARS | SPM_PAIR_OVERFLOW)) {
+    set_error("unknown flags");
+    return SPM_ERR_ARG;
+  }
+  if ((flags & SPM_OFFSETS_CHARS) && !d_spans) { set_error("SPM_OFFSETS_CHARS needs d_spans"); return SPM_ERR_ARG; }
+  if (truncation > SPM_PAIR_TRUNC_ONLY_SECOND) { set_error("unknown truncation strategy"); return SPM_ERR_ARG; }
+  const uint32_t overflow = (flags & SPM_PAIR_OVERFLOW) ? 1u : 0u;
+  if (overflow && truncation != SPM_PAIR_TRUNC_ONLY_FIRST && truncation != SPM_PAIR_TRUNC_ONLY_SECOND) {
+    set_error("SPM_PAIR_OVERFLOW needs SPM_PAIR_TRUNC_ONLY_FIRST or SPM_PAIR_TRUNC_ONLY_SECOND");
+    return SPM_ERR_ARG;
+  }
+  if (stride && !overflow) { set_error("a stride needs SPM_PAIR_OVERFLOW"); return SPM_ERR_ARG; }
+  std::vector<int32_t> tmpl;  // prefix, middle, suffix
+  const int32_t V = e->model.vocab_size();
+  for (const auto &[list, len] : {std::pair{prefix, n_prefix}, std::pair{middle, n_middle}, std::pair{suffix, n_suffix}}) {
+    if (len > spm_engine::kMaxFrame) { set_error("a template list holds more than 64 ids"); return SPM_ERR_ARG; }
+    for (uint32_t k = 0; k < len; ++k) {
+      if (list[k] < 0 || list[k] >= V) {
+        set_error("template id " + std::to_string(list[k]) + " is outside [0, " + std::to_string(V) + ")");
+        return SPM_ERR_ARG;
+      }
+      tmpl.push_back(list[k]);
+    }
+  }
+  const uint32_t tsz = n_prefix + n_middle + n_suffix;
+  if (truncation != SPM_PAIR_TRUNC_NONE && width <= tsz) {
+    set_error("width " + std::to_string(width) + " leaves no room next to the template (" + std::to_string(tsz) +
+              " ids)");
+    return SPM_ERR_ARG;
+  }
+  const uint32_t left = (flags & SPM_PAD_LEFT) ? 1u : 0u;
+  CUDA_TRY(cudaSetDevice(e->device));
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  *rows_out = 0;
+  *width_out = 0;
+  if (n == 0) {
+    CUDA_TRY(cudaStreamSynchronize(st));
+    return SPM_OK;
+  }
+  e->last_h2d = e->last_d2h = 0;
+  FrameOff off(e);  // the template replaces the frame: every stage below sees raw ids
+  const bool spans = d_spans != nullptr;
+  const uint8_t *d_base = reinterpret_cast<const uint8_t *>(d_bytes);
+  const size_t n2 = 2 * n;
+  const uint32_t n32 = static_cast<uint32_t>(n), m32 = static_cast<uint32_t>(n2);
+  const uint32_t expand = (e->max_expand_num + e->max_expand_den - 1) / e->max_expand_den;
+  CUDA_TRY(e->d_pair_tmpl.ensure(std::max<size_t>(tsz, 1)));
+  if (tsz) {  // (from pageable memory: the copy is staged before cudaMemcpyAsync returns)
+    CUDA_TRY(cudaMemcpyAsync(e->d_pair_tmpl.p, tmpl.data(), tsz * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    e->last_h2d = tsz * sizeof(int32_t);
+  }
+  const KPairs T{e->d_pair_tmpl.p, n_prefix, n_middle, n_suffix,
+                 overflow ? (truncation == SPM_PAIR_TRUNC_ONLY_FIRST ? 1u : 2u) : 0u};
+  if (spans) {
+    e->last_unk_detour = 0;
+    SPM_TRY(e->ensure_piece_tables());
+  }
+  if (e->model.model_type == SPM_UNIGRAM) SPM_TRY(e->pick_fast_words_device(d_base, d_offsets, n2, st, &e->batch_fast_words));
+  uint64_t d2h = 0;
+  KPieces P{};
+  uint64_t raw_ids = 0;
+  float main_ms = 0.f;
+  if (!spans) {
+    SPM_TRY(e->encode_stage(d_base, d_offsets, n2, total_bytes, false, st));
+    SPM_TRY(pairs_plan(e, n32, T, width, truncation, overflow, stride, st, &d2h));
+    CUDA_TRY(cudaStreamSynchronize(st));
+  } else {
+    const size_t head = kOpadHead + 2 * kOpadInlineCuts;
+    auto at_read = [&]() -> int {
+      SPM_TRY(queue_offsets_plan(e, d_offsets, m32, expand, st));
+      CUDA_TRY(cudaMemcpyAsync(e->h_opad.p, e->d_opad.p, head * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+      d2h += head * sizeof(unsigned long long);
+      return pairs_plan(e, n32, T, width, truncation, overflow, stride, st, &d2h);
+    };
+    CUDA_TRY(cudaEventRecord(e->ev[3], st));
+    SPM_TRY(e->raw_segmentation_device(d_base, d_offsets, n2, total_bytes, true, &P, &raw_ids, &main_ms, st, at_read));
+    if (norm_slab_start(e->h_opad.p[2], 1, expand) > 0x7FFFFF00ull) {
+      set_error("sentence too long for the device path");
+      return SPM_ERR_UNSUPPORTED;
+    }
+  }
+  // ---- the width, then the rows: each decides whether the call fails ----
+  const unsigned long long R = e->h_win.p[0], need = e->h_win.p[1];
+  if (need >= 0xFFFFFFFFull) { set_error("a row is longer than 2^32 - 2 ids"); return SPM_ERR_UNSUPPORTED; }
+  if (width && need > width) {
+    *width_out = static_cast<uint32_t>(need);
+    set_error(truncation == SPM_PAIR_TRUNC_NONE
+                  ? "a row of " + std::to_string(need) + " ids does not fit width " + std::to_string(width)
+                  : "a pair needs width " + std::to_string(need) + " to keep its other member whole and the room " +
+                        "above the stride");
+    return SPM_ERR_CAPACITY;
+  }
+  const uint32_t w = width ? width : static_cast<uint32_t>(need);
+  if (R > 0x7FFFFFFFull) { set_error(std::to_string(R) + " rows do not fit int32"); return SPM_ERR_UNSUPPORTED; }
+  *rows_out = R;
+  *width_out = w;
+  if (R > rows_capacity || R * w > cells_capacity) {
+    set_error("capacity too small: need " + std::to_string(R) + " rows of " + std::to_string(w) + " cells");
+    return SPM_ERR_CAPACITY;
+  }
+  const uint32_t R32 = static_cast<uint32_t>(R);
+  const int pgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  const int rgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (R + 7) / 8));
+  window_rows_kernel<<<pgrid, 256, 0, st>>>(e->d_win.p + 2, n32, 0u, e->d_pair_step.p, d_row_pair, d_row_first);
+  CUDA_TRY(cudaGetLastError());
+  ++e->last_launches;
+  if (!spans) {
+    write_pair_rows_kernel<<<rgrid, 256, 0, st>>>(e->d_sent_count.p, e->d_sent_start.p, e->d_tmp_ids.p, n32, R32, T,
+                                                  e->d_pair_keep.p, d_row_pair, d_row_first, w, pad_id, left, d_ids,
+                                                  d_type_ids, d_lengths);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+    CUDA_TRY(cudaEventRecord(e->ev[2], st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    e->last_d2h = d2h;
+    finish_timing(e);
+    return SPM_OK;
+  }
+  // ---- K11, packed over the 2n sentences: every token's begin / end once, then the rows ----
+  CUDA_TRY(e->d_off_begin.ensure(raw_ids + 1));
+  CUDA_TRY(e->d_off_end.ensure(raw_ids + 1));
+  CUDA_TRY(e->d_pc_out_ids.ensure(raw_ids + 1));
+  CUDA_TRY(e->d_pc_out_id_offsets.ensure(n2 + 1));
+  KOffsets A{};
+  A.begin = e->d_off_begin.p;
+  A.end = e->d_off_end.p;
+  A.out_ids = e->d_pc_out_ids.p;
+  A.out_id_offsets = e->d_pc_out_id_offsets.p;
+  SPM_TRY(offsets_device_chunks(e, false, P, A, d_base, d_offsets, n2, expand, -1, st, &d2h));
+  const int sgrid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n2 + 7) / 8));
+  if (flags & SPM_OFFSETS_CHARS) {
+    lists_to_chars_kernel<<<sgrid, 256, 0, st>>>(d_base, d_offsets, m32, A.begin, A.end, A.out_id_offsets, e->kframe(),
+                                                 -1);
+    CUDA_TRY(cudaGetLastError());
+    ++e->last_launches;
+  }
+  write_pair_spans_kernel<<<rgrid, 256, 0, st>>>(A.out_ids, A.begin, A.end, A.out_id_offsets, n32, R32, T,
+                                                 e->d_pair_keep.p, d_row_pair, d_row_first, w, pad_id, left, d_ids,
+                                                 d_type_ids, reinterpret_cast<int2 *>(d_spans), d_lengths);
   CUDA_TRY(cudaGetLastError());
   ++e->last_launches;
   CUDA_TRY(cudaEventRecord(e->ev[1], st));

@@ -29,6 +29,8 @@
 //
 // Windows (spm_encode_windows_device) run K11 in packed mode, once per sentence, and write_window_spans_kernel gathers
 // each window row from the packed lists: a token that lies in several windows is walked once.
+// Sentence pairs (spm_encode_pairs_device) do the same over their 2n sentences with no frame, and
+// write_pair_spans_kernel gathers each pair row.
 //
 // The byte-fallback grouping assumes the normalized text is valid UTF-8, so that every unknown piece is exactly one
 // character.  The normalizer guarantees that for every input (a malformed byte becomes U+FFFD) as long as the
@@ -41,6 +43,7 @@
 #include "device_model.h"
 #include "kernels.cuh"
 #include "normalize_kernel.cuh"
+#include "padded_kernel.cuh"
 #include "pieces_kernel.cuh"
 
 namespace spm_b200 {
@@ -234,6 +237,51 @@ __global__ void __launch_bounds__(256) write_window_spans_kernel(const int32_t *
       }
     }
     if (lane == 0) lengths[row] = static_cast<int32_t>(real);
+  }
+}
+
+// The rows of spm_encode_pairs_device with offsets: one warp per pair row, gathered from K11's packed output over the
+// 2n sentences with no frame (sentence i's list at id_offsets[i]), laid out as write_pair_rows_kernel
+// (padded_kernel.cuh) lays out its id rows; template and pad cells get (0, 0).
+__global__ void __launch_bounds__(256) write_pair_spans_kernel(const int32_t *ids, const uint32_t *begin,
+                                                               const uint32_t *end,
+                                                               const unsigned long long *id_offsets, uint32_t n,
+                                                               uint32_t rows, KPairs T, const uint2 *keep,
+                                                               const int32_t *row_pair, const int32_t *row_first,
+                                                               uint32_t w, int32_t pad_id, uint32_t left, int32_t *out,
+                                                               int32_t *type_ids, int2 *spans, int32_t *lengths) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < rows; row += warps) {
+    const uint32_t i = static_cast<uint32_t>(row_pair[row]);
+    const unsigned long long oa = id_offsets[i], ob = id_offsets[n + i];
+    const PairRow p = pair_row(T, static_cast<uint32_t>(row_first[row]), keep[i],
+                               static_cast<uint32_t>(id_offsets[i + 1] - oa),
+                               static_cast<uint32_t>(id_offsets[n + i + 1] - ob));
+    const uint32_t lead = left ? w - p.real : 0u;
+    const uint32_t second = T.np + p.ca + T.nm;
+    const unsigned long long at = static_cast<unsigned long long>(row) * w;
+    for (uint32_t t = lane; t < w; t += 32) {
+      const uint32_t k = t - lead;  // wraps past `real` for the leading pad cells
+      int32_t id = pad_id, type = 0;
+      int2 sp = make_int2(0, 0);
+      if (k < p.real) {
+        uint32_t q;
+        const uint32_t c = pair_cell(T, p, k, q);
+        if (c == 0) {
+          id = T.tmpl[q];
+        } else {
+          const unsigned long long g = (c == 1 ? oa : ob) + q;
+          id = ids[g];
+          sp = make_int2(static_cast<int32_t>(begin[g]), static_cast<int32_t>(end[g]));
+        }
+        type = k >= second ? 1 : 0;
+      }
+      __stcs(out + at + t, id);
+      __stcs(type_ids + at + t, type);
+      __stcs(spans + at + t, sp);
+    }
+    if (lane == 0) lengths[row] = static_cast<int32_t>(p.real);
   }
 }
 

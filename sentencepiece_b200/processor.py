@@ -252,6 +252,7 @@ class Engine:
         self._model_bytes = model_bytes
         self._pad_guess = 64  # cells per row encode_device_padded(width=0) allocates first: the last such call's width
         self._win_ratio = 1.0  # rows per sentence encode_device_windows allocates first: the last call's R / n
+        self._pair_guess = (1.0, 64)  # encode_device_pairs' first allocation: the last call's R / n and width
         self._pad = None  # pad_id(), read from the model on first use
 
     def close(self):
@@ -738,6 +739,90 @@ class Engine:
             res += (flat[sp_at:sp_at + 2 * R * width].view(R, width, 2),)
         return res
 
+    def encode_device_pairs(self, d_bytes, d_offsets, prefix=(), middle=(), suffix=(), width=0,
+                            truncation="longest_first", overflow=False, stride=0, pad_id=None, pad_left=False,
+                            unit=None, out=None):
+        """spm_encode_pairs_device: a batch of 2n sentences already on the GPU (d_offsets: the 2n + 1 offsets of the
+        stacked batch) as n pair rows prefix ++ A_i ++ middle ++ B_i ++ suffix, A_i = sentence i, B_i = sentence n + i,
+        cut by `truncation` ("none", "longest_first", "only_first", "only_second") to `width` cells (0: the longest row,
+        "none" only) -> (ids int32 [R, w], lengths int32 [R], type_ids int32 [R, w], row_pair int32 [R], row_first
+        int32 [R]), plus spans int32 [R, w, 2] when unit is "byte" or "char" (None: no offsets).  overflow (with
+        "only_first" / "only_second"): the cut member is split into windows that overlap by `stride` ids instead of
+        being dropped; row_pair[r] is the pair of row r and row_first[r] the window's first id in that member.  The
+        engine's encode frame does not apply.  A pair that cannot be laid out at `width` raises ValueError naming the
+        width it needs.  Without `out`, the rows go to new tensors sized by a guess, and when R or w is larger the call
+        is repeated into exactly R rows of w cells, which encodes the batch a second time.  out (fixed widths only): a
+        contiguous int32 tensor of at least R * (2 * w + 3) cells (R * (4 * w + 3) with spans), 8-byte aligned, that
+        takes the ids, the type ids, the spans, then the lengths and the two row maps (ValueError when too small)."""
+        import torch
+        if unit not in (None, "byte", "char"):
+            raise ValueError('unit must be None, "byte" or "char"')
+        if truncation not in _capi.PAIR_TRUNCATION:
+            raise ValueError("truncation must be one of " + ", ".join(_capi.PAIR_TRUNCATION))
+        if out is not None and not width:
+            raise ValueError("out needs a fixed width")
+        if pad_id is None:
+            pad_id = self.pad_id()
+            if pad_id < 0:
+                raise ValueError("the model defines no pad piece (trainer_spec.pad_piece): pass pad_id explicitly")
+        st = self._stream(d_bytes, d_offsets, out)
+        if d_bytes.dtype != torch.uint8 or d_bytes.dim() != 1 or not d_bytes.is_contiguous():
+            raise ValueError("d_bytes must be a contiguous 1-D uint8 tensor")
+        if d_offsets.dtype not in (torch.int64, torch.uint64) or d_offsets.dim() != 1 or not d_offsets.is_contiguous():
+            raise ValueError("d_offsets must be a contiguous 1-D int64 or uint64 tensor of 2n + 1 offsets")
+        if (d_offsets.numel() - 1) % 2:
+            raise ValueError("d_offsets must hold 2n + 1 offsets: the first members, then the second")
+        if out is not None and (out.dtype != torch.int32 or not out.is_contiguous()):
+            raise ValueError("out must be a contiguous int32 tensor")
+        n = (d_offsets.numel() - 1) // 2
+        flags = (_capi.PAD_LEFT if pad_left else 0) | (_capi.OFFSETS_CHARS if unit == "char" else 0) | \
+            (_capi.PAIR_OVERFLOW if overflow else 0)
+        lists = [(ctypes.c_int32 * len(x))(*x) for x in (prefix, middle, suffix)]
+
+        per_cell = 4 if unit else 2  # int32 per cell: id, type id (and begin, end)
+
+        def layout(total, w):
+            """a flat buffer of `total` cells as rows of w: (rows, cells, type ids at, spans at, lengths at); the spans
+            start at an even cell, 8-byte aligned"""
+            rows = total // (per_cell * w + 3)
+            cells = rows * w
+            return rows, cells, cells, 2 * cells, per_cell * cells
+
+        def call(buf, w):
+            rows, cells, ty_at, sp_at, len_at = layout(buf.numel(), w)
+            p = buf.data_ptr()
+            r, wo = ctypes.c_uint64(), ctypes.c_uint32()
+            rc = self._lib.spm_encode_pairs_device(
+                self._h, d_bytes.data_ptr(), d_offsets.data_ptr(), n, d_bytes.numel(), lists[0], len(prefix), lists[1],
+                len(middle), lists[2], len(suffix), width, _capi.PAIR_TRUNCATION[truncation], stride, pad_id, flags, p,
+                p + 4 * ty_at, p + 4 * sp_at if unit else None, rows, cells, p + 4 * len_at, p + 4 * (len_at + rows),
+                p + 4 * (len_at + 2 * rows), ctypes.byref(r), ctypes.byref(wo), st)
+            return rc, r.value, wo.value
+
+        def alloc(rows, w):
+            return torch.empty(rows * (per_cell * w + 3), dtype=torch.int32, device=d_bytes.device)
+
+        ratio, w_alloc = self._pair_guess
+        w_alloc = width or w_alloc
+        buf = out if out is not None else alloc(max(n, int(n * ratio + 0.5), 1), w_alloc)
+        rc, R, w = call(buf, w_alloc)
+        if rc == _capi.SPM_ERR_CAPACITY and out is None and R:
+            w_alloc = w
+            buf = alloc(R, w)
+            rc, R, w = call(buf, w_alloc)
+        if rc == _capi.SPM_ERR_CAPACITY:
+            raise ValueError(self._lib.spm_last_error(self._h).decode())
+        self._check(rc)
+        if n:
+            self._pair_guess = (R / n, max(w, 1))
+        rows, cells, ty_at, sp_at, len_at = layout(buf.numel(), w_alloc)
+        flat = buf.view(-1)
+        res = (flat[:R * w].view(R, w), flat[len_at:len_at + R], flat[ty_at:ty_at + R * w].view(R, w),
+               flat[len_at + rows:len_at + rows + R], flat[len_at + 2 * rows:len_at + 2 * rows + R])
+        if unit:
+            res += (flat[sp_at:sp_at + 2 * R * w].view(R, w, 2),)
+        return res
+
     def decode_device(self, ids2d, lengths=None, stop_id=-1):
         """spm_decode_ids_device: the rows of an int32 or int64 [n, L] CUDA tensor (any row stride, e.g. a column slice;
         each row contiguous) -> list of n str.  Row i holds min(L, lengths[i]) ids (lengths: int32 [n], or None for L),
@@ -1083,6 +1168,46 @@ class SentencePieceProcessor:
         return self._engine.encode_device_windows(d_bytes, d_offs, max_len, stride=stride, pad_id=pad_id,
                                                   pad_left=pad_left, unit="char" if return_offsets else None,
                                                   eos_id=self._specials()["eos_id"])
+
+    def encode_pairs(self, first, second, max_len=None, truncation=None, stride=None, prefix=(), middle=(), suffix=(),
+                     pad_id=None, pad_left=False, return_offsets=False):
+        """EncodeAsIds of a batch of sentence pairs as padded rows prefix ++ first[i] ++ middle ++ second[i] ++ suffix
+        on the GPU (cross-encoders, NLI, extractive QA) -> (ids int32 [R, w], lengths int32 [R], type_ids int32
+        [R, w]) on the engine's device; type ids are 1 from second[i]'s first cell through the suffix.  first /
+        second: equal-length lists of str / bytes, or two (bytes, offsets) pairs of CUDA tensors as
+        Engine.encode_device_pairs takes one batch; they are stacked into one batch on the device.  max_len = None:
+        w is the longest row and nothing is cut; otherwise truncation ("longest_first" when None, "only_first",
+        "only_second" or "none") fits the pairs to max_len.  stride (an int; with "only_first" / "only_second"): the
+        cut member is split into windows overlapping by stride ids, every row repeating the other member, and the
+        result also holds (row_pair int32 [R], row_first int32 [R]).  return_offsets: offsets int32 [R, w, 2] last, each
+        token's (begin, end) in characters of its own member (EncodeAsImmutableProto's begin / end), (0, 0) on template
+        and pad cells.  The add_bos / add_eos / reverse options do not apply: the template places the special ids."""
+        self._require()
+        if isinstance(first, tuple) != isinstance(second, tuple):
+            raise ValueError("first and second must both be lists or both be (bytes, offsets) pairs")
+        if isinstance(first, tuple):
+            import torch
+            (b1, o1), (b2, o2) = first, second
+            if o1.numel() != o2.numel():
+                raise ValueError("first and second must hold the same number of sentences")
+            o1, o2 = o1.view(torch.int64), o2.view(torch.int64)
+            end1, start2 = int(o1[-1]), int(o2[0])
+            d_bytes = torch.cat([b1[:end1], b2[start2:]])
+            d_offs = torch.cat([o1, o2[1:] - start2 + end1])
+        else:
+            if len(first) != len(second):
+                raise ValueError("first and second must hold the same number of sentences")
+            d_bytes, d_offs = self._device_batch(list(first) + list(second))
+        if truncation is None:
+            truncation = "none" if max_len is None else "longest_first"
+        res = self._engine.encode_device_pairs(d_bytes, d_offs, prefix=prefix, middle=middle, suffix=suffix,
+                                               width=max_len or 0, truncation=truncation, overflow=stride is not None,
+                                               stride=stride or 0, pad_id=pad_id, pad_left=pad_left,
+                                               unit="char" if return_offsets else None)
+        out = (res[0], res[1], res[2])
+        if stride is not None:
+            out += (res[3], res[4])
+        return out + (res[5],) if return_offsets else out
 
     def decode_padded(self, ids, lengths=None, stop_id=None):
         """DecodeIds of every row of an int32 / int64 [n, L] CUDA tensor -> list of n str: row i holds lengths[i] ids
