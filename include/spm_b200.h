@@ -471,6 +471,42 @@ int spm_decode_ids_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, u
                           uint32_t row_len, const int32_t *d_lengths, int64_t stop_id, const char **text,
                           const uint64_t **text_offsets, void *stream);
 
+/* The state of one streamed row of spm_decode_stream_device, in device memory.  16 bytes; all zeros is a fresh row. */
+typedef struct {
+  uint64_t text_bytes; /* bytes of text returned for this row so far */
+  uint32_t ids;        /* ids consumed so far, held ones included */
+  uint8_t flags;       /* bit 0: done; bits 1-2: held byte ids (0..3); bit 3: the leading-U+2581 rule no longer applies
+                          (the reference's is_bos_ws would be false at the next token: bos_ws_seen, or text non-empty) */
+  uint8_t held[3];     /* the byte values of the held BYTE ids, in order */
+} spm_decode_stream_state;
+
+/* Streaming Decode of device-resident generation output: each call takes the next ids of n sequences and returns, per
+ * row, the text those ids settle.  Row i's new ids are read as spm_decode_ids_device reads a row (int32 / int64 at
+ * d_ids + i * row_stride elements, min(row_len, d_lengths[i]) of them, cut before the first stop_id when stop_id >= 0),
+ * so a [n, 1] column slice of one step's sampled ids or a [n, k] block of accepted speculative ids is passed as it is.
+ * d_state[i] (16-byte aligned device memory) carries row i from call to call.
+ * Let S be every id row i has consumed, this call's included.  The held tail of S is empty unless S ends in a run of
+ * BYTE pieces in which a UTF-8 decision is pending: from the first position p of that run whose lead byte b0 needs more
+ * bytes than the run has left (2 for 110xxxxx, 3 for 1110xxxx, 4 for 11110xxx; every other byte needs 1), the rest of
+ * the run is held, at most 3 ids.  Row i's text is Decode(S) from d_state[i].text_bytes up to the end of the last token
+ * before the held tail (that token's end as spm_decode_offsets gives it).  So the texts of all a row's calls, through
+ * the one that finishes it, concatenate to spm_decode_ids of all its ids, and each text is whole UTF-8 characters.
+ * A row finishes in the call where its new ids stop at stop_id, or where d_final[i] != 0 (d_final: nullable int32 [n]):
+ * its held bytes are then decoded as the reference decodes a run at the end of a list (U+FFFD per invalid byte), and
+ * it is marked done.  A done row returns empty text, and its ids are neither read nor validated until the caller zeroes
+ * its state, which starts a new sequence in that slot.
+ * Outputs: engine-owned pinned text and text_offsets[n+1], valid until the next call on this engine.  Errors: an id
+ * outside [0, vocab) gives SPM_ERR_ARG "Invalid id: N" (the whole int64 value), a BYTE piece not of the form <0xXX>
+ * SPM_ERR_ENCODE, a row's id count above 2^32 - 1 SPM_ERR_UNSUPPORTED, as do models with a denormalizer_spec charsmap.
+ * On any error no state changes and no text is returned: the new states are written to engine scratch and copied over
+ * d_state on `stream` only after the call's status words read back clean.  n == 0 succeeds.  No per-row data goes to
+ * the device; the text, its offsets and the status words come back.  `stream` as in spm_encode_ids_device; the call
+ * returns after the text and the new states have arrived.  decode_extra_options are not applied. */
+int spm_decode_stream_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, uint64_t row_stride, size_t n,
+                             uint32_t row_len, const int32_t *d_lengths, int64_t stop_id, const int32_t *d_final,
+                             spm_decode_stream_state *d_state, const char **text, const uint64_t **text_offsets,
+                             void *stream);
+
 /* TrainerSpec.unk_surface (src/sentencepiece_model.proto:228, read at sentencepiece_processor.cc:771-773) for
  * engines created from an spm_model_desc; engines created from a serialized ModelProto take it from the proto. */
 int spm_engine_set_unk_surface(spm_engine *e, const char *surface, size_t bytes);

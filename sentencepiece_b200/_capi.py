@@ -19,6 +19,7 @@ EXPORTS = [
     "spm_nbest_encode_pieces", "spm_sample_encode_pieces", "spm_sample_encode_and_score_pieces",
     "spm_encode_ids_device_padded", "spm_decode_ids_device", "spm_normalize", "spm_encode_offsets",
     "spm_decode_offsets", "spm_encode_offsets_device_padded", "spm_encode_windows_device", "spm_encode_pairs_device",
+    "spm_decode_stream_device",
 ]
 
 # spm_normalize: the n2o entry of a sentence whose reference norm_to_orig is empty
@@ -30,6 +31,8 @@ PAD_TRUNCATE, PAD_LEFT, OFFSETS_CHARS = 1, 2, 4
 PAIR_TRUNCATION = {"none": 0, "longest_first": 1, "only_first": 2, "only_second": 3}
 PAIR_OVERFLOW = 8
 SPM_ERR_CAPACITY = 4
+# spm_decode_stream_state: bytes per row, and the byte and bit of its done flag
+STREAM_STATE_BYTES, STREAM_FLAGS_BYTE, STREAM_DONE = 16, 12, 1
 
 
 class ModelDesc(ctypes.Structure):
@@ -92,6 +95,7 @@ def load():
                                           P(ctypes.c_int32), u32, u32, u32, u32, ctypes.c_int32, u32, vp, vp, vp, u64,
                                           u64, vp, vp, vp, P(u64), P(u32), vp]
     L.spm_decode_ids_device.argtypes = [vp, vp, u32, u64, sz, u32, vp, ctypes.c_int64, P(vp), P(vp), vp]
+    L.spm_decode_stream_device.argtypes = [vp, vp, u32, u64, sz, u32, vp, ctypes.c_int64, vp, vp, P(vp), P(vp), vp]
     L.spm_host_alloc.argtypes = [sz]
     L.spm_host_alloc.restype = vp
     L.spm_host_free.argtypes = [vp]

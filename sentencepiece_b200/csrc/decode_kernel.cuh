@@ -21,6 +21,7 @@
 #define SPM_B200_DECODE_KERNEL_CUH_
 
 #include <cstdint>
+#include <type_traits>
 
 namespace spm_b200 {
 
@@ -30,6 +31,17 @@ constexpr uint32_t kDecKindNormal = 0u, kDecKindControl = 1u, kDecKindUnknown = 
 constexpr uint32_t kDecLeadWs = 1u << 2;  // normal piece that starts with U+2581
 constexpr uint32_t kDecBadByte = 1u << 3; // BYTE piece that is not "<0xXX>" (PieceToByte fails, model_interface.cc:214-230)
 constexpr uint32_t kDecByteShift = 8;
+
+// spm_decode_stream_state as the kernel sees it (16 bytes): word = flags | held[0] << 8 | held[1] << 16 | held[2] << 24
+struct alignas(16) DecStreamState {
+  unsigned long long text_bytes;
+  uint32_t ids;
+  uint32_t word;
+};
+constexpr uint32_t kStDone = 1u;          // the row has finished
+constexpr uint32_t kStHeldShift = 1;      // bits 1-2: held byte ids (0..3)
+constexpr uint32_t kStHeldMask = 3u << kStHeldShift;
+constexpr uint32_t kStBosOver = 1u << 3;  // the next non-byte token is decoded with is_bos_ws false
 
 struct KDecode {
   const int32_t *ids;
@@ -57,6 +69,23 @@ struct KDecode {
   uint32_t *tok_end;
 };
 
+// STREAM mode's own arguments (decode_warp_kernel<IdT, true, false, true>, spm_decode_stream_device), a second kernel
+// parameter so that KDecode, and with it the code of the other modes, stays as it is.  Rows are read as in ROWS mode,
+// but row i's length comes from decode_row_end (row_cap, lengths, stop_id) and KDecode::row_len is not used; row i
+// continues the stream described by state_in[i] and leaves its new state in state_out[i].  fin (nullable): rows to
+// finish.
+struct KDecodeStream {
+  const DecStreamState *state_in;
+  DecStreamState *state_out;
+  const int32_t *lengths;
+  const int32_t *fin;
+  long long stop_id;
+  uint32_t row_cap;
+};
+struct KNoStream {};
+template <bool STREAM>
+using KStreamArg = typename std::conditional<STREAM, KDecodeStream, KNoStream>::type;
+
 // IsValidDecodeUTF8 (src/util.h:173-176 over DecodeUTF8, src/util.cc:51-84): bytes consumed by one valid character
 // at b[0..avail), 0 if the byte is structurally invalid (the caller then consumes one byte).
 __device__ __forceinline__ uint32_t dec_utf8_valid(const uint32_t *b, uint32_t avail) {
@@ -78,29 +107,66 @@ __device__ __forceinline__ uint32_t dec_utf8_valid(const uint32_t *b, uint32_t a
   return 0;
 }
 
+// The bytes dec_utf8_valid reads to decide at lead byte b0: with that many available (or the run ended) its result is
+// final.  1 for ASCII and for bytes that cannot lead a character, else the length the lead byte announces.
+__device__ __forceinline__ uint32_t dec_utf8_need(uint32_t b0) {
+  return (b0 & 0xE0u) == 0xC0u ? 2u : (b0 & 0xF0u) == 0xE0u ? 3u : (b0 & 0xF8u) == 0xF0u ? 4u : 1u;
+}
+
 // Sequential restatement for one list (lists with BYTE pieces); WRITE = false only counts.  IdT: the ids' type (every
 // id has been checked to lie in [0, vocab) before).  ENDS (with WRITE): also the end of every token's surface, as
 // ProcessBytePieces sets them: the first c-1 byte tokens of a valid c-byte character end where they begin and the last
 // one after the character, an invalid byte's token after its U+FFFD.
-template <bool WRITE, typename IdT = int32_t, bool ENDS = false>
-__device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, unsigned long long a, uint32_t L, uint8_t *out) {
+// STREAM: the list continues a stream whose state word (DecStreamState::word) is *sw: its held byte values come first,
+// the leading-U+2581 rule starts from its kStBosOver bit, and unless kStDone is set a trailing byte run whose next
+// decision lacks bytes (fewer than dec_utf8_need of them) is held instead of decoded.  *sw is updated to the new state.
+template <bool WRITE, typename IdT = int32_t, bool ENDS = false, bool STREAM = false>
+__device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, unsigned long long a, uint32_t L, uint8_t *out,
+                                                           uint32_t *sw = nullptr) {
   const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   uint32_t n = 0;  // bytes of text so far
   bool is_bos_ws = true, bos_ws_seen = false;
   uint32_t i = 0;
+  uint32_t h = 0, held = 0;  // STREAM: held bytes before the ids, and after them
+  if constexpr (STREAM) {
+    h = (*sw & kStHeldMask) >> kStHeldShift;
+    L += h;
+    is_bos_ws = !(*sw & kStBosOver);
+  }
+  // STREAM: the info word of element k of the list, the held bytes first, then the ids
+  auto info_at = [&](uint32_t k) -> uint32_t {
+    if (k < h) return kDecKindByte | (((*sw >> (8 + 8 * k)) & 0xFFu) << kDecByteShift);
+    return __ldg(D.dec_info + static_cast<int32_t>(ids[a + (k - h)]));
+  };
   while (i < L) {
-    const int32_t id = static_cast<int32_t>(ids[a + i]);
-    const uint32_t info = __ldg(D.dec_info + id);
+    int32_t id;
+    uint32_t info;
+    if constexpr (STREAM) {
+      id = i < h ? 0 : static_cast<int32_t>(ids[a + (i - h)]);
+      info = info_at(i);
+    } else {
+      id = static_cast<int32_t>(ids[a + i]);
+      info = __ldg(D.dec_info + id);
+    }
     const uint32_t kind = info & kDecKindMask;
     if (kind == kDecKindByte) {
       // one Unicode character from the run of byte pieces that starts here
       uint32_t b[4] = {info >> kDecByteShift, 0, 0, 0};
       uint32_t avail = 1;
       while (avail < 4 && i + avail < L) {
-        const uint32_t inf2 = __ldg(D.dec_info + static_cast<int32_t>(ids[a + i + avail]));
+        uint32_t inf2;
+        if constexpr (STREAM) inf2 = info_at(i + avail);
+        else inf2 = __ldg(D.dec_info + static_cast<int32_t>(ids[a + i + avail]));
         if ((inf2 & kDecKindMask) != kDecKindByte) break;
         b[avail] = inf2 >> kDecByteShift;
         ++avail;
+      }
+      if constexpr (STREAM) {
+        if (!(*sw & kStDone) && i + avail == L && avail < dec_utf8_need(b[0])) {
+          held = avail;  // <= 3: the decision at i waits for more bytes
+          for (uint32_t k = 0; k < avail; ++k) held |= b[k] << (8 + 8 * k);
+          break;
+        }
       }
       const uint32_t c = dec_utf8_valid(b, avail);
       if (c == 0) {
@@ -132,22 +198,76 @@ __device__ __forceinline__ uint32_t decode_list_sequential(const KDecode &D, uns
     bos_ws_seen = has_bos_ws;
     ++i;
   }
+  if constexpr (STREAM) {
+    // the held bytes are decoded before any later token, so they too close the rule
+    const bool over = !is_bos_ws || bos_ws_seen || n != 0 || held != 0;
+    *sw = (*sw & kStDone) | ((held & 3u) << kStHeldShift) | (held & ~0xFFu) | (over ? kStBosOver : 0u);
+  }
   return n;
+}
+
+// The end of row `row` of a padded id tensor, for the whole warp: min(row_len, lengths[row]) ids (row_len when lengths
+// is null; a negative length is 0), cut before the first stop_id in them when stop_id >= 0.
+template <typename IdT>
+__device__ __forceinline__ uint32_t decode_row_end(const IdT *ids, unsigned long long row_stride, uint32_t row,
+                                                   uint32_t row_len, const int32_t *lengths, long long stop_id,
+                                                   uint32_t lane) {
+  uint32_t L = row_len;
+  if (lengths) L = min(L, static_cast<uint32_t>(max(lengths[row], 0)));
+  if (stop_id >= 0) {
+    const IdT *r = ids + static_cast<unsigned long long>(row) * row_stride;
+    for (uint32_t base = 0; base < L; base += 32) {
+      const uint32_t t = base + lane;
+      const uint32_t hit = __ballot_sync(0xFFFFFFFFu, t < L && static_cast<long long>(r[t]) == stop_id);
+      if (hit) {
+        L = base + __ffs(hit) - 1u;
+        break;
+      }
+    }
+  }
+  return L;
+}
+
+// STREAM: row i's new state after `bytes` more text, `ids` more ids and with state word w.  text_bytes and ids are read
+// again rather than kept in registers through the row.
+__device__ __forceinline__ void dec_put_state(const KDecodeStream &S, uint32_t i, uint32_t bytes, uint32_t ids, uint32_t w) {
+  const DecStreamState o = S.state_in[i];
+  S.state_out[i] = DecStreamState{o.text_bytes + bytes, o.ids + ids, w};
 }
 
 // IdT, ROWS: the ids are int32 or int64, and list i is either [id_offsets[i], id_offsets[i+1]) (packed) or row_len[i]
 // ids from i * row_stride (rows of a padded [n, row_stride] tensor).  ENDS: also write D.tok_end (packed lists only).
 // Template flags, so that the packed int32 instantiation keeps its code.
-template <typename IdT = int32_t, bool ROWS = false, bool ENDS = false>
-__global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
+// STREAM (with ROWS): each row is the next ids of a stream, described by S (KDecodeStream).  A done row writes no text and
+// keeps its state; its ids are not read.  Otherwise the row's text is the part of its stream's text that this call
+// settles, and the new state goes to state_out (copied over state_in by the host only when the call succeeds).
+template <typename IdT = int32_t, bool ROWS = false, bool ENDS = false, bool STREAM = false>
+__global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D, const KStreamArg<STREAM> S) {
   static_assert(ROWS || sizeof(IdT) == 4, "packed lists are int32");
   static_assert(!(ROWS && ENDS), "token ends are written for packed lists only");
+  static_assert(ROWS || !STREAM, "streams are rows");
   const IdT *ids = reinterpret_cast<const IdT *>(D.ids);
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t sent = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; sent < D.n; sent += warps) {
     unsigned long long a, len64;
-    if constexpr (ROWS) {
+    // STREAM: the row's state word, with kStDone when this call finishes the row; ovf: its id count would overflow
+    uint32_t word = 0;
+    bool ovf = false;
+    if constexpr (STREAM) {
+      const DecStreamState ss = S.state_in[sent];
+      word = ss.word;
+      if (word & kStDone) {
+        if (lane == 0) { D.sent_start[sent] = 0; D.sent_count[sent] = 0; S.state_out[sent] = ss; }
+        continue;
+      }
+      a = static_cast<unsigned long long>(sent) * D.row_stride;
+      len64 = decode_row_end(ids, D.row_stride, sent, S.row_cap, S.lengths, S.stop_id, lane);
+      // the row stops at stop_id when the cut above shortened it
+      const uint32_t lim = S.lengths ? min(S.row_cap, static_cast<uint32_t>(max(S.lengths[sent], 0))) : S.row_cap;
+      if (len64 < lim || (S.fin && S.fin[sent] != 0)) word |= kStDone;
+      ovf = ss.ids + len64 > 0xFFFFFFFFull;
+    } else if constexpr (ROWS) {
       a = static_cast<unsigned long long>(sent) * D.row_stride;
       len64 = D.row_len[sent];
     } else {
@@ -157,6 +277,7 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
     const uint32_t L = static_cast<uint32_t>(len64);
     // ---- pass 0: ids in range, any BYTE piece ----
     uint32_t err = len64 > 0x7FFFFFFFull ? 2u : 0u;  // 2 = id out of range (checked first by the reference), 1 = malformed byte piece
+    if constexpr (STREAM) if (ovf) err = 3;  // 3 = the stream's id count overflows
     int32_t err_id = 0;
     bool has_byte = false, stop = err != 0;
     for (uint32_t base = 0; base < L && !stop; base += 32) {
@@ -183,18 +304,21 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
       if (lane == 0) { D.sent_start[sent] = 0; D.sent_count[sent] = 0; }
       continue;
     }
+    if constexpr (STREAM) has_byte |= (word & kStHeldMask) != 0;
     has_byte = __any_sync(0xFFFFFFFFu, has_byte);
     uint32_t total = 0;
     unsigned long long pos = 0;
     if (has_byte) {
       // ---- sequential path on lane 0 ----
       if (lane == 0) {
-        total = decode_list_sequential<false, IdT>(D, a, L, nullptr);
+        uint32_t sw = word;
+        total = decode_list_sequential<false, IdT, false, STREAM>(D, a, L, nullptr, &sw);
         pos = atomicAdd(D.cursor, static_cast<unsigned long long>(total));
         if (pos + total > D.tmp_cap) { atomicOr(D.status + 2, 1u); total = 0; }
-        else decode_list_sequential<true, IdT, ENDS>(D, a, L, D.tmp + pos);
+        else decode_list_sequential<true, IdT, ENDS, STREAM>(D, a, L, D.tmp + pos, &word);
         D.sent_start[sent] = pos;
         D.sent_count[sent] = total;
+        if constexpr (STREAM) dec_put_state(S, sent, total, L, word);
       }
       __syncwarp();
       continue;
@@ -202,6 +326,7 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
     // ---- parallel path: one token per lane, two passes (count, write) ----
     for (int pass = 0; pass < 2; ++pass) {
       bool bos_over = !D.strip;
+      if constexpr (STREAM) bos_over = bos_over || (word & kStBosOver);
       uint32_t run = 0;
       for (uint32_t base = 0; base < L; base += 32) {
         const uint32_t t = base + lane;
@@ -251,6 +376,9 @@ __global__ void __launch_bounds__(256) decode_warp_kernel(const KDecode D) {
         pos = __shfl_sync(0xFFFFFFFFu, pos, 0);
         if (pos + total > D.tmp_cap) break;
       }
+      if constexpr (STREAM)
+        if (pass == 1 && lane == 0)
+          dec_put_state(S, sent, total, L, word | (bos_over ? kStBosOver : 0u));
     }
   }
 }
@@ -265,19 +393,7 @@ __global__ void __launch_bounds__(256) decode_row_len_kernel(const IdT *ids, uns
   const uint32_t lane = threadIdx.x & 31;
   const uint32_t warps = (gridDim.x * blockDim.x) >> 5;
   for (uint32_t row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; row < n; row += warps) {
-    uint32_t L = row_len;
-    if (lengths) L = min(L, static_cast<uint32_t>(max(lengths[row], 0)));
-    if (stop_id >= 0) {
-      const IdT *r = ids + static_cast<unsigned long long>(row) * row_stride;
-      for (uint32_t base = 0; base < L; base += 32) {
-        const uint32_t t = base + lane;
-        const uint32_t hit = __ballot_sync(0xFFFFFFFFu, t < L && static_cast<long long>(r[t]) == stop_id);
-        if (hit) {
-          L = base + __ffs(hit) - 1u;
-          break;
-        }
-      }
-    }
+    const uint32_t L = decode_row_end(ids, row_stride, row, row_len, lengths, stop_id, lane);
     if (lane == 0) len_out[row] = L;
   }
 }

@@ -365,6 +365,8 @@ struct spm_engine {
   PinBuf<char> h_dec_text;
   PinBuf<uint64_t> h_dec_text_offsets;
   PinBuf<uint32_t> h_dec_tok_end;
+  DevBuf<DecStreamState> d_dec_state;  // spm_decode_stream_device: the new states, until the call has succeeded
+  uint32_t dec_max_len = 3;            // the longest decoded piece, unk_surface or U+FFFD
   bool dec_ready = false;
   int ensure_decode_tables();
   // decode_warp_kernel's arguments for n id lists (ids indexed by the values of id_offsets), results in d_dec_tmp
@@ -395,6 +397,10 @@ struct spm_engine {
                                        : std::to_string(static_cast<int32_t>(h_ctrl32.p[3]))));
       return SPM_ERR_ARG;
     }
+    if (h_ctrl32.p[1] == 3u) {  // STREAM mode only
+      set_error("Decode: a stream's id count would overflow 2^32 - 1");
+      return SPM_ERR_UNSUPPORTED;
+    }
     if (h_ctrl32.p[1] == 1u) {
       set_error("Decode: byte piece of id " + std::to_string(h_ctrl32.p[3]) + " is not of the form <0xXX>");
       return SPM_ERR_ENCODE;
@@ -414,10 +420,12 @@ struct spm_engine {
   // The decode of n lists on st after the caller's checks: launch(tmp_cap) queues decode_warp_kernel, which is run again
   // with the exact temporary size if it overflowed; then the text is put into list order and copied into the pinned
   // results, and the call waits for it.  rows: launch runs the ROWS mode (for decode_error).  tok_end != NULL: launch
-  // runs the ENDS mode into d_dec_tok_end, whose n_tok entries are copied back too.
+  // runs the ENDS mode into d_dec_tok_end, whose n_tok entries are copied back too.  at_ok (may be empty) queues more
+  // work on st once the status words have been read back clean; the call waits for it too.
   template <typename Launch>
   int decode_text(uint32_t n, unsigned long long tmp_cap, bool rows, cudaStream_t st, Launch &&launch, const char **text,
-                  const uint64_t **text_offsets, const uint32_t **tok_end = nullptr, uint64_t n_tok = 0) {
+                  const uint64_t **text_offsets, const uint32_t **tok_end = nullptr, uint64_t n_tok = 0,
+                  const std::function<int()> &at_ok = {}) {
     CUDA_TRY(d_sent_start.ensure(n));
     CUDA_TRY(d_sent_count.ensure(n));
     CUDA_TRY(d_dec_text_offsets.ensure(n + 1));
@@ -439,6 +447,7 @@ struct spm_engine {
       break;
     }
     if (h_ctrl32.p[2]) { set_error("Decode: temporary buffer overflow persisted"); return SPM_ERR_CAPACITY; }
+    if (at_ok) SPM_TRY(at_ok());
     // offsets (exclusive scan) + gather into list order: the kernels of the encode path
     CUDA_TRY(d_dec_text.ensure(tot + 16));
     SPM_TRY(scan_total(d_sent_count.p, n, 0, d_ctrl64.p + 2, st));
@@ -1920,6 +1929,8 @@ int spm_engine::ensure_decode_tables() {
     }
   }
   off[V] = static_cast<uint32_t>(bytes.size());
+  dec_max_len = 3;
+  for (int i = 0; i < V; ++i) dec_max_len = std::max(dec_max_len, off[i + 1] - off[i]);
   std::vector<uint8_t> b(bytes.begin(), bytes.end());
   b.push_back(0);
   CUDA_TRY(d_dec_off.upload(off));
@@ -2037,9 +2048,9 @@ int spm_engine::decode_host_pipelined(const int32_t *ids, const uint64_t *id_off
       KDecode D = decode_args(p_dec_ids[k].p - id_offsets[lo], p_offsets[k].p, m, tmp_cap);
       if (tok_end) {
         D.tok_end = p_dec_tok_end[k].p - id_offsets[lo];
-        decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D);
+        decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D, {});
       } else {
-        decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+        decode_warp_kernel<<<grid, 256, 0, st>>>(D, {});
       }
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaEventRecord(ev[1], st));
@@ -2732,9 +2743,9 @@ int decode_host(spm_engine *e, const int32_t *ids, const uint64_t *id_offsets, s
                            KDecode D = e->decode_args(e->d_dec_ids.p - base, e->d_offsets.p, n32, tmp_cap);
                            if (tok_end) {
                              D.tok_end = e->d_dec_tok_end.p - base;
-                             decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D);
+                             decode_warp_kernel<int32_t, false, true><<<grid, 256, 0, st>>>(D, {});
                            } else {
-                             decode_warp_kernel<<<grid, 256, 0, st>>>(D);
+                             decode_warp_kernel<<<grid, 256, 0, st>>>(D, {});
                            }
                          },
                          text, text_offsets, tok_end, total_ids));
@@ -2798,10 +2809,66 @@ int spm_decode_ids_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, u
                            KDecode D = e->decode_args(static_cast<const int32_t *>(d_ids), nullptr, n32, tmp_cap);
                            D.row_stride = row_stride;
                            D.row_len = e->d_row_len.p;
-                           if (wide) decode_warp_kernel<int64_t, true><<<grid, 256, 0, st>>>(D);
-                           else decode_warp_kernel<int32_t, true><<<grid, 256, 0, st>>>(D);
+                           if (wide) decode_warp_kernel<int64_t, true><<<grid, 256, 0, st>>>(D, {});
+                           else decode_warp_kernel<int32_t, true><<<grid, 256, 0, st>>>(D, {});
                          },
                          text, text_offsets));
+  finish_timing(e);
+  return SPM_OK;
+}
+
+static_assert(sizeof(spm_decode_stream_state) == 16 && sizeof(DecStreamState) == 16, "a stream state is 16 bytes");
+
+int spm_decode_stream_device(spm_engine *e, const void *d_ids, uint32_t id_bytes, uint64_t row_stride, size_t n,
+                             uint32_t row_len, const int32_t *d_lengths, int64_t stop_id, const int32_t *d_final,
+                             spm_decode_stream_state *d_state, const char **text, const uint64_t **text_offsets,
+                             void *stream) {
+  if (!e || !text || !text_offsets) return SPM_ERR_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  auto set_error = [&](const std::string &m) { e->set_error(m); };
+  if (id_bytes != 4 && id_bytes != 8) { e->set_error("id_bytes must be 4 or 8"); return SPM_ERR_ARG; }
+  if (n && ((row_len && !d_ids) || !d_state)) { e->set_error("null argument"); return SPM_ERR_ARG; }
+  if (reinterpret_cast<uintptr_t>(d_state) % 16) { e->set_error("d_state must be 16-byte aligned"); return SPM_ERR_ARG; }
+  if (n >= 0xFFFFFFF0ull) { e->set_error("too many rows in one call"); return SPM_ERR_ARG; }
+  if (!e->model.denormalizer_charsmap.empty()) {
+    e->set_error("Decode: models with a denormalizer_spec are not on the device path");
+    return SPM_ERR_UNSUPPORTED;
+  }
+  CUDA_TRY(cudaSetDevice(e->device));
+  { const int rc = e->ensure_decode_tables(); if (rc) return rc; }
+  cudaStream_t st = stream ? static_cast<cudaStream_t>(stream) : e->stream;
+  e->last_launches = 0;
+  e->last_h2d = e->last_d2h = 0;
+  if (n == 0) {
+    CUDA_TRY(e->h_dec_text.ensure(1));
+    CUDA_TRY(e->h_dec_text_offsets.ensure(1));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    e->h_dec_text_offsets.p[0] = 0;
+    *text = e->h_dec_text.p;
+    *text_offsets = e->h_dec_text_offsets.p;
+    return SPM_OK;
+  }
+  const uint32_t n32 = static_cast<uint32_t>(n);
+  CUDA_TRY(e->d_dec_state.ensure(n));
+  const int grid = static_cast<int>(std::min<size_t>(static_cast<size_t>(e->sm_count) * 8, (n + 7) / 8));
+  const bool wide = id_bytes == 8;
+  DecStreamState *in = reinterpret_cast<DecStreamState *>(d_state);
+  // a row's text is at most (its ids + 3 held bytes) surfaces of at most dec_max_len bytes each, so the temporary
+  // never overflows below 1 GiB; above that decode_text's retry sizes it exactly (the kernel only reads d_state)
+  const unsigned long long bound = (static_cast<unsigned long long>(row_len) + 3ull) * e->dec_max_len * n + 16;
+  SPM_TRY(e->decode_text(n32, std::min(bound, 1ull << 30), true, st,
+                         [&](unsigned long long tmp_cap) {
+                           KDecode D = e->decode_args(static_cast<const int32_t *>(d_ids), nullptr, n32, tmp_cap);
+                           D.row_stride = row_stride;
+                           const KDecodeStream S{in, e->d_dec_state.p, d_lengths, d_final, stop_id, row_len};
+                           if (wide) decode_warp_kernel<int64_t, true, false, true><<<grid, 256, 0, st>>>(D, S);
+                           else decode_warp_kernel<int32_t, true, false, true><<<grid, 256, 0, st>>>(D, S);
+                         },
+                         text, text_offsets, nullptr, 0, [&]() -> int {
+                           CUDA_TRY(cudaMemcpyAsync(in, e->d_dec_state.p, n * sizeof(DecStreamState),
+                                                    cudaMemcpyDeviceToDevice, st));
+                           return SPM_OK;
+                         }));
   finish_timing(e);
   return SPM_OK;
 }

@@ -845,6 +845,66 @@ class Engine:
         raw = np.ctypeslib.as_array(ctypes.cast(text, ctypes.POINTER(ctypes.c_uint8)), (max(o[n], 1),))[:o[n]].tobytes()
         return [raw[o[i]:o[i + 1]].decode("utf-8", errors="replace") for i in range(n)]
 
+    def decode_stream_device(self, ids2d, state, lengths=None, stop_id=-1, final=None):
+        """spm_decode_stream_device: the next ids of n streamed sequences -> list of n str, each the text these ids
+        settle.  ids2d, lengths and stop_id are read as decode_device reads them; state: the n rows' states, a
+        contiguous CUDA tensor of n * 16 bytes (all zeros for a fresh row), updated in place when the call succeeds;
+        final: None or a contiguous int32 [n] CUDA tensor, non-zero for rows to finish in this call."""
+        import torch
+        if ids2d.dim() != 2 or ids2d.dtype not in (torch.int32, torch.int64):
+            raise ValueError("ids2d must be a 2-D int32 or int64 tensor")
+        n, L = ids2d.shape
+        if L > 1 and ids2d.stride(1) != 1:
+            raise ValueError("the ids of a row must be contiguous")
+        if lengths is not None and (lengths.dtype != torch.int32 or lengths.shape != (n,) or not lengths.is_contiguous()):
+            raise ValueError("lengths must be a contiguous int32 tensor of n entries")
+        if final is not None and (final.dtype != torch.int32 or final.shape != (n,) or not final.is_contiguous()):
+            raise ValueError("final must be a contiguous int32 tensor of n entries")
+        if (not state.is_cuda or not state.is_contiguous()
+                or state.numel() * state.element_size() != n * _capi.STREAM_STATE_BYTES):
+            raise ValueError("state must be a contiguous CUDA tensor of n * 16 bytes")
+        st = self._stream(ids2d, lengths, state, final)
+        text = ctypes.c_void_p()
+        to = ctypes.c_void_p()
+        self._check(self._lib.spm_decode_stream_device(
+            self._h, ids2d.data_ptr(), ids2d.element_size(), ids2d.stride(0), n, L,
+            lengths.data_ptr() if lengths is not None else None, stop_id,
+            final.data_ptr() if final is not None else None, state.data_ptr(), ctypes.byref(text), ctypes.byref(to), st))
+        o = np.ctypeslib.as_array(ctypes.cast(to, ctypes.POINTER(ctypes.c_uint64)), (n + 1,)).tolist()
+        raw = np.ctypeslib.as_array(ctypes.cast(text, ctypes.POINTER(ctypes.c_uint8)), (max(o[n], 1),))[:o[n]].tobytes()
+        # every text is whole UTF-8 characters, so strict decoding cannot fail
+        return [raw[o[i]:o[i + 1]].decode("utf-8") for i in range(n)]
+
+
+class DecodeStream:
+    """Streaming Decode for a batch of generated sequences (SentencePieceProcessor.decode_stream): each step() takes the
+    next ids of every slot and returns the text they settle, so the texts of a slot's steps concatenate to DecodeIds
+    of all its ids.  A slot finishes at stop_id or when final says so; then it ignores further ids until reset()."""
+
+    def __init__(self, engine, batch_size, stop_id=-1):
+        import torch
+        self._engine = engine
+        self._stop_id = stop_id
+        self.state = torch.zeros((batch_size, _capi.STREAM_STATE_BYTES), dtype=torch.uint8,
+                                 device=torch.device("cuda", engine.device))
+
+    def step(self, ids, lengths=None, final=None):
+        """ids: int32 / int64 CUDA tensor [batch_size, k] (k ids per slot, e.g. a column slice of the output), or
+        [batch_size] for one id per slot; lengths: int32 [batch_size] ids to take per slot; final: int32
+        [batch_size], non-zero to finish a slot after its ids -> list of batch_size str."""
+        if ids.dim() == 1:
+            ids = ids.unsqueeze(1)
+        return self._engine.decode_stream_device(ids, self.state, lengths, self._stop_id, final)
+
+    def reset(self, rows):
+        """Zeroes the given slots (indices, a slice or a bool mask), which start new sequences at the next step."""
+        self.state[rows] = 0
+
+    @property
+    def done(self):
+        """bool [batch_size]: the slots that have finished"""
+        return (self.state[:, _capi.STREAM_FLAGS_BYTE] & _capi.STREAM_DONE) != 0
+
 
 def _id_lists(input):
     """One id list or a list of id lists -> (single, (ids int32[], id_offsets uint64[n+1]))"""
@@ -1214,6 +1274,12 @@ class SentencePieceProcessor:
         (all L when lengths is None), cut before its first stop_id (e.g. eos_id()) when one is given."""
         self._require()
         return self._engine.decode_device(ids, lengths, -1 if stop_id is None else stop_id)
+
+    def decode_stream(self, batch_size, stop_id=None):
+        """A DecodeStream of batch_size slots for a generation loop: step(ids) returns each slot's new text as the ids
+        arrive; a slot finishes at stop_id (e.g. eos_id()) when one is given."""
+        self._require()
+        return DecodeStream(self._engine, batch_size, -1 if stop_id is None else stop_id)
 
     # python/src/sentencepiece/__init__.py Normalize, sentencepiece.i _Normalize / _NormalizeWithOffsets
     def Normalize(self, input, with_offsets=None):
